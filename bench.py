@@ -5,7 +5,7 @@ One "step" = one pass of the hot path over one batch of synthetic publish topics
     value  = topics/s with the batch resident in HBM (bfq_match_device; kernels + counter read-back)
     e2e    = topics/s through the host-buffer C-ABI call bfq_match (pinned host -> H2D -> kernels -> D2H result)
 Workload = BASELINE.json config C4 by default (10M filters over 1000 tenants, Zipf-skewed fan-out, 1M-topic batch):
-the metric is quoted "@10M filters" and it fits one B200. Under torchrun every rank owns its own tenants
+the metric is quoted "@10M filters" and it fits one H100 (2.3 GB of index). Under torchrun every rank owns its own tenants
 (tenant sharding, no data-path collective; weak scaling: each rank hosts a full-size shard) unless --scaling strong.
 
     python bench.py --gpus 1 --steps 20 --warmup 3
@@ -27,6 +27,7 @@ sys.path.insert(0, ROOT)
 
 METRIC = "publish-topics matched/sec @10M filters"
 UNIT = "topics/s"
+HBM_PEAK_GBS = 3350.0   # H100 SXM data sheet (HBM3): the roofline's denominator, a rate no copy reaches
 
 
 def metric_name(args):
@@ -57,7 +58,106 @@ def parse_args():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--max-pfanout", type=int, default=2 ** 31 - 1, help="Setting.MaxPersistentFanout (reference default INT_MAX)")
     ap.add_argument("--max-gfanout", type=int, default=100, help="Setting.MaxGroupFanout (reference default 100)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (float64, < 64 MB; "
+                         "a fixed, seeded sample where the whole result is larger), for comparing two builds output for output")
+    args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the GPU path's results; --impl reference has none")
+    return args
+
+
+DUMP_TOPICS = 1 << 20          # per-topic (per-filter) arrays: every entry up to this many, else a seeded sample of this many
+DUMP_SEGMENTS = 2048           # seeded sample of topics (filters) whose matched ranks (ids) are written out, sorted ...
+DUMP_SEGMENT_CAP = 1024        # ... the smallest this many of each
+
+
+class _DeviceArray:
+    """a device buffer the library owns, seen by torch without a copy (CUDA array interface)"""
+
+    def __init__(self, ptr, shape, typestr):
+        self.__cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (int(ptr or 0), False), "version": 2}
+
+
+def _dump_save(d, name, a):
+    np.save(os.path.join(d, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
+
+
+def _dump_sample(n, k, seed):
+    """the entries a dump covers: all of 0..n-1 when n <= k, else a seeded uniform sample of k (the same for every run)"""
+    if n <= k:
+        return np.arange(n, dtype=np.int64)
+    return np.sort(np.random.default_rng(seed).choice(n, k, replace=False)).astype(np.int64)
+
+
+def _dump_segments(d, offsets, sorted_segment):
+    """DUMP_SEGMENTS seeded segments of a CSR result: segment_index, segment_offsets, segment_values (each segment sorted
+    ascending and cut to its DUMP_SEGMENT_CAP smallest entries, so that the order a kernel emitted them in does not matter)"""
+    n = len(offsets) - 1
+    sel = _dump_sample(n, DUMP_SEGMENTS, 0x5E6)
+    parts, off = [], np.zeros(len(sel) + 1, np.int64)
+    for j, i in enumerate(sel.tolist()):
+        v = sorted_segment(int(offsets[i]), int(offsets[i + 1]))[:DUMP_SEGMENT_CAP]
+        parts.append(v)
+        off[j + 1] = off[j] + len(v)
+    _dump_save(d, "segment_index", sel)
+    _dump_save(d, "segment_offsets", off)
+    _dump_save(d, "segment_values", np.concatenate(parts) if parts else np.zeros(0))
+
+
+def _throttle_summary(thr, n, sel):
+    """throttle events {topic, rank, kind} -> per topic of `sel`: [persistent-cap events, group-cap events, sum of the throttled
+    ranks] (a fixed shape whatever the number of events, independent of the order the kernel emitted them in)"""
+    out = np.zeros((n, 3), np.float64)
+    if len(thr):
+        t = thr[:, 0].astype(np.int64)
+        np.add.at(out[:, 0], t, thr[:, 2] == 1)
+        np.add.at(out[:, 1], t, thr[:, 2] == 2)
+        np.add.at(out[:, 2], t, thr[:, 1].astype(np.float64))
+    return out[sel]
+
+
+def dump_forward(res, n, dev, d):
+    """the last timed step's device result (bfq_match_device): per topic the matched routes before caps, the surviving routes
+    (bfq_expand_device), the matched filter ranges and the throttle events (per kind, and the sum of the throttled ranks); the
+    sorted surviving route ranks of a seeded topic sample"""
+    import torch
+    os.makedirs(d, exist_ok=True)
+    mask32 = 0xFFFFFFFF
+
+    def u32(ptr, shape):
+        if not ptr or shape[0] == 0:
+            return torch.zeros(shape, dtype=torch.int64, device=dev)
+        return torch.as_tensor(_DeviceArray(ptr, shape, "<i4"), device=dev).to(torch.int64) & mask32
+
+    d_off = torch.empty(n + 1, dtype=torch.int64, device=dev)
+    total = res.expand(d_off.data_ptr(), None, 0)
+    d_ranks = torch.empty(max(total, 1), dtype=torch.int64, device=dev)
+    res.expand(d_off.data_ptr(), d_ranks.data_ptr(), total)
+    torch.cuda.synchronize(dev)
+    off = d_off.cpu().numpy()
+    sel = _dump_sample(n, DUMP_TOPICS, 0x70C)
+    d_sel = torch.from_numpy(sel).to(dev)
+    _dump_save(d, "topic_index", sel)
+    _dump_save(d, "topic_route_count", u32(res.d_route_count, (n,))[d_sel].cpu().numpy())
+    _dump_save(d, "topic_range_count", (u32(res.d_span_count, (n,)) & 0x3FFFFFFF)[d_sel].cpu().numpy())
+    _dump_save(d, "topic_surviving_routes", np.diff(off)[sel])
+    _dump_segments(d, off, lambda a, b: torch.sort(d_ranks[a:b]).values[:DUMP_SEGMENT_CAP].cpu().numpy())
+    _dump_save(d, "topic_throttled", _throttle_summary(u32(res.d_throttled, (int(res.n_throttled), 3)).cpu().numpy(), n, sel))
+    torch.cuda.synchronize(dev)
+
+
+def dump_inverse(res, d):
+    """the last timed step's bfq_rmatch result: per query filter the total matches and the ids returned (their count, and the
+    sorted ids of a seeded filter sample)"""
+    os.makedirs(d, exist_ok=True)
+    off = np.asarray(res.offsets, np.int64)
+    ids = np.asarray(res.ids)
+    sel = _dump_sample(res.n_filters, DUMP_TOPICS, 0x70C)
+    _dump_save(d, "filter_index", sel)
+    _dump_save(d, "filter_total_matches", np.asarray(res.totals)[sel])
+    _dump_save(d, "filter_returned_ids", np.diff(off)[sel])
+    _dump_segments(d, off, lambda a, b: np.sort(ids[a:b])[:DUMP_SEGMENT_CAP])
 
 
 def dist_env():
@@ -165,12 +265,7 @@ def make_roofline(sample_topic_bytes, st, ns, n_topics_per_launch, kernel_ms, gp
     kernel's duration. Duplicate topics count like any other topic (the figure is per topic of the batch, whatever the
     kernel does about repeats)."""
     per_topic = (sample_topic_bytes + 4 * ns + 32 * st["V"] + 8 * st["P"] + 8 * st["ranges"] + 4 * ns) / ns
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = HBM_PEAK_GBS
     achieved = per_topic * n_topics_per_launch / (kernel_ms / 1000.0) / 1e9
     # dram__bytes_read.sum + dram__bytes_write.sum of this kernel cannot be measured inside a bench run (ncu replays every
     # launch ~40 times); it comes from the committed `ncu --set full` capture of the same command, named here, or is null
@@ -183,8 +278,7 @@ def make_roofline(sample_topic_bytes, st, ns, n_topics_per_launch, kernel_ms, gp
         pass
     roof = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
             "traffic_source": traffic_src,
-            "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured copy)" if peaks else "fallback 6650 GB/s",
-            "frac_of_nominal_8000": achieved / 8000.0,
+            "peak_source": "H100 SXM data sheet, 3350 GB/s",
             "kernel": "match_topics_lane_kernel (tier 0, one lane per distinct topic)", "kernel_ms": kernel_ms, "alg_bytes_per_topic": per_topic,
             "alg_counters_per_topic": {"V": st["V"] / ns, "P": st["P"] / ns, "ranges": st["ranges"] / ns, "R": st["R"] / ns},
             "note": "algorithmic bytes per topic measured by the oracle over %d topics (%s)" % (ns, "the whole batch" if ns == n_topics_per_launch else "uniform random sample")}
@@ -403,6 +497,8 @@ def main_inverse(args, rank, world, local):
         k_ms.append(last.timings_ms["device_rmatch_kernel"])
     sampler.end()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:
+        dump_inverse(last, args.dump_outputs)
     idx.match_blobs(tenants, f_blob, f_off, f_tt, None)          # warm: the first unlimited call grows the id / range buffers
     unl = idx.match_blobs(tenants, f_blob, f_off, f_tt, None)
     if numa:
@@ -435,15 +531,10 @@ def main_inverse(args, rank, world, local):
         # (counted by the oracle), ranges = rank ranges the kernel emits (a '#' subtree or a final '+' level is ONE range)
         alg = fbytes + 4 * n + 32 * visited + 8 * last.n_ranges
         k = float(np.mean(k_ms))
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except Exception:
-            pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
+        peak = HBM_PEAK_GBS
         ach = alg / (k / 1000.0) / 1e9
         line["roofline"] = {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": None,
-                            "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured copy)" if peaks else "fallback 6650 GB/s",
+                            "peak_source": "H100 SXM data sheet, 3350 GB/s",
                             "kernel": "rmatch_kernel (one warp per filter over the BFS-numbered topic trie)", "kernel_ms": k,
                             "alg_bytes_per_filter": alg / n, "alg_counters_per_filter": {"V": visited / n, "ranges": last.n_ranges / n},
                             "note": "V counted by the oracle over all %d filters; the reference's lookup visits EVERY child of a '+' level "
@@ -519,7 +610,7 @@ def main():
     h_off = torch.from_numpy(np.ascontiguousarray(w.topic_off)).pin_memory()
     h_tt = torch.from_numpy(np.ascontiguousarray(w.topic_tenant[:max(n, 1)])).pin_memory()
     d_topics, d_off, d_tt = h_topics.to(dev), h_off.to(dev), h_tt.to(dev)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 50 MB L2
     stream = torch.cuda.current_stream(dev)
 
     nt = len(w.tenants)
@@ -642,6 +733,8 @@ def main():
     if world > 1:
         dist.barrier()
     out = last[0] if xch is None else pipe["gathered"]
+    if args.dump_outputs and rank == 0:
+        dump_forward(out, n, dev, args.dump_outputs)
     if xch is not None:
         n_ranges, n_overflow, n_distinct = out.n_ranges, out.n_overflow_topics, out.n_distinct_topics
     step_ms = [a.elapsed_time(b) for a, b in ev] if ev is not None else [step_total / args.steps] * args.steps

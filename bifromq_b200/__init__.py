@@ -1,4 +1,4 @@
-"""bifromq_b200 — B200-native batched MQTT topic-filter matcher behind apache/bifromq's dist-worker /
+"""bifromq_b200 — H100-native batched MQTT topic-filter matcher behind apache/bifromq's dist-worker /
 retain-store co-processor seams. The product is the CUDA library (csrc/, C-ABI in include/bfq_gpumatch.h);
 this package is the thin host-side mirror of the reference's Java interfaces used by tests and bench.py.
 """

@@ -610,7 +610,7 @@ int32_t finish_core(const CoreCtx& c, const SubBatch& sb, CoreOut* out, bool* re
         const uint64_t capR = 2 * ((uint64_t) c.s->flat.max_tenant_nodes + 2) + 2;
         const uint64_t per_warp = 4 * capF + capR;   // uint2 units: two frontier buffers of uint4 entries + ranges
         uint64_t warps = std::min<uint64_t>(hc[CTR_OVERFLOW], std::max<uint64_t>(8, (1ull << 31) / (per_warp * sizeof(uint2))));
-        warps = std::min<uint64_t>(warps, 148 * 8);
+        warps = std::min<uint64_t>(warps, (uint64_t) device_sm_count() * 8);
         warps = (warps + 7) / 8 * 8;
         if (w->d_scratch.cap < (size_t) (warps * per_warp)) {
             CUDA_TRY(cudaDeviceSynchronize());   // the other compute stream of this workspace may be in tier 2 on the old scratch
@@ -885,8 +885,8 @@ int32_t commit_full(bfq_index* h) {
     CUDA_TRY(sn->d_rkind.reserve(std::max<size_t>(flat.rkind.size(), 1)));
     CUDA_TRY(sn->d_pfxP.reserve(flat.pfx_persistent.size()));
     CUDA_TRY(sn->d_pfxG.reserve(flat.pfx_group.size()));
-    // (a threaded upload through per-thread pinned bounce buffers was measured 3x SLOWER than this one pageable cudaMemcpy:
-    // 0.83 vs 0.26 s for 2.3 GB — the pinned allocations cost more than the driver's own staging loses)
+    // (one pageable cudaMemcpy: a threaded upload through per-thread pinned bounce buffers pays more for the pinned
+    // allocations than the driver's own staging loses)
     CUDA_TRY(cudaMemcpy(sn->d_slots.p, flat.slots.data(), flat.slots.size() * sizeof(Slot), cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemcpy(sn->d_tags.p, flat.tags.data(), flat.tags.size(), cudaMemcpyHostToDevice));
     if (!flat.roots.empty())
@@ -1503,8 +1503,8 @@ int32_t bfq_match(bfq_index* h, const uint8_t* tenants, const int64_t* tenant_of
     // Large batches are cut into sub-batches that flow through three streams: all H2D copies on one, the kernels +
     // compaction + D2H of consecutive sub-batches alternating on two others, so the copy of sub-batch c+1 and the
     // result read-back of c-1 overlap the kernels of c (PCIe is full duplex; the copies dominate the host path).
-    // four sub-batches: eight were measured slower (2.45 ms vs 2.1 ms per 1M C4 topics): a 125k-topic sub-batch is less than one
-    // wave of tier-0 lanes, its kernel takes as long as a 250k one
+    // four sub-batches, not eight: a 125k-topic sub-batch is less than one wave of tier-0 lanes, its kernel takes as long as
+    // a 250k one
     int C = n >= (1 << 17) ? 4 : 1;
     {
         static const int forced = [] {   // experiment switch BFQ_SUBBATCHES
@@ -1542,7 +1542,6 @@ int32_t bfq_match(bfq_index* h, const uint8_t* tenants, const int64_t* tenant_of
         if (rc != BFQ_OK) return rc;
         int64_t bounds[MAX_CHUNKS + 1];
         for (int c = 0; c <= C; c++) bounds[c] = n * c / C;
-        // (uneven cuts — 15 / 35 / 35 / 15 % — were measured slower than quarters: 2.01 vs 1.88 ms per 1M C4 topics)
         for (int c = 0; c < C && n > 0; c++) {
             const int64_t b = bounds[c], e = bounds[c + 1];
             const int64_t ob = topic_off[b], oe = topic_off[e];

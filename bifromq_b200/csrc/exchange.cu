@@ -221,7 +221,7 @@ int32_t bfq_exchange_gather(bfq_exchange* x, const bfq_device_result* res, int32
     X_CUDA(cudaMemcpyAsync(x->h_meta, x->d_meta.p, (size_t) 2 * W * sizeof(long long), cudaMemcpyDeviceToHost, st));
     X_CUDA(cudaStreamSynchronize(st));
     // every rank's slice has the same (padded) stride, so the payload travels as plain ncclAllGather calls — the ring / NVLS
-    // algorithms at full NVLink rate; per-root broadcasts of exactly-sized slices measured 3x slower at 8 ranks
+    // algorithms at full NVLink rate, where per-root broadcasts of exactly-sized slices would serialise the roots
     int64_t max_t = 1, max_r = 1;
     for (int r = 0; r < W; r++) {
         max_t = std::max<int64_t>(max_t, x->h_meta[2 * r]);

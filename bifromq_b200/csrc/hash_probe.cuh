@@ -19,17 +19,14 @@ __device__ __forceinline__ uint4 ld16(const uint4* p) {
     return __ldg(p);
 }
 
-// 32-byte load (LDG.E.256, sm_100+): the lanes of a warp read unrelated slots, so every load instruction costs one L1
-// tag lookup + wavefront PER LANE — the kernel's binding resource (ncu: ~1 tag request per cycle per SM). A 64-byte slot is
-// two of these instead of four 16-byte loads, a payload half is one.
+// One 32-byte sector as two 16-byte loads (LDG.E.128 is the widest global load sm_90 has). Both halves are issued before
+// either is used, so a lane still waits one memory round trip per sector.
 template <bool kNA>
 __device__ __forceinline__ void ld32(const void* p, uint32_t* w) {
-    if (kNA)
-        asm volatile("ld.global.nc.L1::no_allocate.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]) : "l"(p));
-    else
-        asm volatile("ld.global.nc.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7]) : "l"(p));
+    const uint4* q = reinterpret_cast<const uint4*>(p);
+    const uint4 a = ld16<kNA>(q), b = ld16<kNA>(q + 1);
+    w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w;
+    w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
 }
 
 template <bool kNA = false>
@@ -115,7 +112,7 @@ __device__ __forceinline__ uint32_t tag_candidates(const uint4& tg, uint32_t fp4
 
 // find_child for a warp whose lanes sit on different kinds of nodes (the lane-per-topic kernel). A plain
 // `big ? probe : perfect-hash` branch serialises the two sides: the BIG lanes' tag read and slot read, THEN the other lanes'
-// slot read — three dependent memory round trips per warp step (ncu: 19 % + 14 % of the stall samples on the three waits).
+// slot read — three dependent memory round trips per warp step.
 // Here phase 1 is the BIG lanes' tag read only (16 bytes, L2-resident window), and phase 2 is ONE slot read issued by every
 // lane at the same instruction, whatever kind of node it is on; second candidates / overflowed blocks (rare) loop afterwards.
 template <bool kNA = false>

@@ -685,8 +685,7 @@ void build_tenant(const KVBlob& kv, TenantBuild& tb) {
         // collision-free: ONE memory access per lookup, hit or miss. A random seed works with probability
         // ~exp(-c^2 / 2^(lg+1)), so the array needs ~c^2/16 slots for the 16-bit seed space to contain one: cheap for the
         // common small fan-outs, 4096 slots for 256 children, and beyond 2^PERFECT_LOG2_MAX the global tag table takes over
-        // (two dependent accesses — ncu: the tag wait alone was 20 % of the lane kernel's stall samples when fan-outs
-        // of 17..1000 still went there).
+        // (two dependent accesses, and a warp's lanes wait for the slowest of them).
         bool big = false;
         if (c == 1) {
             pl.lg = 0;

@@ -1,4 +1,4 @@
-// match_kernels.cu — forward match on sm_100a: a batch of publish topics against the flattened filter tries.
+// match_kernels.cu — forward match on sm_90a (H100): a batch of publish topics against the flattened filter tries.
 //
 // Replaces the hot loop of TenantRouteMatcher.matchAll
 // (bifromq-dist/bifromq-dist-worker/src/main/java/org/apache/bifromq/dist/worker/cache/TenantRouteMatcher.java:96-156)
@@ -272,22 +272,24 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32) match_topics_kernel(const 
 
 // ------------------------------------------------------------------------------------------------ tier 0
 // ONE LANE PER TOPIC, persistent lanes. The warp-per-topic walk above leaves most lanes idle when the frontier
-// is a handful of nodes (the common case: ~4 per level on BASELINE config C4; ncu: ~2100 warp instructions per
-// topic, profiles/r1_v1_*). Here every lane walks its own topic depth-first:
+// is a handful of nodes (the common case: ~4 per level on BASELINE config C4). Here every lane walks its own topic
+// depth-first:
 //   * a node has at most two continuations per level (exact child, '+' child), so the DFS parks at most ONE
 //     pending '+' branch per level: a (L_MAXLV+1)-entry per-lane array plus a bitmask, never a growing frontier;
 //   * per step a lane reads the 28 bytes at its current level start (up to three aligned 16-byte granules, word select +
 //     funnel shift), finds the '/' with a SWAR zero-byte test — the level table is filled lazily, there is no tokenising
-//     pre-pass —, issues the exact-child slot read (2 x LDG.256) and the '+' child payload read (1 x LDG.256) together and
+//     pre-pass —, issues the exact-child slot read (4 x LDG.128) and the '+' child payload read (2 x LDG.128) together and
 //     writes the discovered ranges straight to the topic's INLINE_RANGES inline slots: no staging, no output atomics;
 //   * a lane that finishes takes the next topic at once (warp-uniform refill from 32-topic chunks claimed with
-//     one atomicAdd per chunk), so a straggler never idles the other 31 lanes (v2 of this kernel waited for the
-//     whole batch of 32: ncu showed 10 of 32 lanes active, profiles/r1_v2_*);
+//     one atomicAdd per chunk), so a straggler never idles the other 31 lanes (a warp that waits for its whole batch of 32
+//     runs with a third of its lanes active);
 //   * chunks are runs of p.order — the batch sorted by (tenant, leading-level hashes), see launch_order — so the lanes of
-//     a warp walk the same part of the trie, take the same branches and finish together (profiles/r1_v8_*).
+//     a warp walk the same part of the trie, take the same branches and finish together.
 // Anything that does not fit the bounded state (> L_MAXLV levels, a level > 24 B, > INLINE_RANGES ranges, topic > 64 KB)
 // is handed, whole, to the warp-per-topic tier through defer_list.
 constexpr int L_WARPS = 4;
+constexpr int64_t LARGE_BATCH_TOPICS = 1 << 17;   // tier 0: batches of at least this many topics run with ...
+constexpr int LARGE_BATCH_CTAS_PER_SM = 4;        // ... at most this many resident CTAs per SM (see launch_match_lanes)
 constexpr int L_MAXLV = 12;
 constexpr int L_CHUNK = 32;
 constexpr int TENANT_CAPPED = 1 << 30;   // flag in the lane's tenant word: the tenant has a finite fan-out cap
@@ -303,7 +305,7 @@ struct LaneSmem {
     int32_t m_tenant[L_CHUNK];
     int32_t m_root[L_CHUNK];        // root ordinal of the topic's tenant, or -1
     // payload of the tenant root of the chunk's first topic: in locality order a chunk is almost always one tenant, and the
-    // root read at every refill was a dependent L2 access in the middle of a lock-step step (ncu: 4 % of the stall samples)
+    // root read at every refill would be a dependent L2 access in the middle of a lock-step step
     uint32_t c_root[8];
     int32_t c_ord;
 };
@@ -612,8 +614,7 @@ __global__ void __launch_bounds__(L_WARPS * 32) match_topics_lane_kernel(const M
 // Reads a topic 16 bytes at a time as four topic-aligned 32-bit words (word i of block j = topic bytes 16j + 4i .. + 3), whatever
 // the topic's alignment in the blob: one aligned 16-byte granule load per block, word select + funnel shift in registers. Bytes
 // at and after len read as 0. Only granules that hold at least one byte of the topic are read, so the reads stay inside the
-// 16-byte granules the blob occupies. (A word-at-a-time reader cost 39 instructions per 4 bytes; the tail loop alone was 41 %
-// of the prep kernel's instructions: ncu source view, profiles/r2_prep_v1.*)
+// 16-byte granules the blob occupies. (A word-at-a-time reader spends most of the prep kernel's instructions in its tail loop.)
 struct TopicQuads {
     const uint4* qp;
     int off, len, j;
@@ -1038,13 +1039,24 @@ __global__ void __launch_bounds__(256) copy_add_kernel(uint32_t* dst, const uint
 }
 }  // namespace
 
+int device_sm_count() {
+    static std::mutex mu;
+    static int sms_of[64] = {0};   // per device ordinal
+    int dev = 0;
+    cudaGetDevice(&dev);
+    std::lock_guard<std::mutex> g(mu);
+    int& sms = sms_of[dev & 63];
+    if (sms == 0 && (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms < 1)) sms = 132;
+    return sms;
+}
+
 void launch_rank_shift(Slot* slots, const RankShiftRegion* d_regions, int n_regions, cudaStream_t stream) {
     if (n_regions <= 0) return;
-    rank_shift_kernel<<<148 * 8, 256, 0, stream>>>(slots, d_regions, n_regions);
+    rank_shift_kernel<<<device_sm_count() * 8, 256, 0, stream>>>(slots, d_regions, n_regions);
 }
 void launch_copy_add(uint32_t* dst, const uint32_t* src, int64_t n, uint32_t add, cudaStream_t stream) {
     if (n <= 0) return;
-    copy_add_kernel<<<(unsigned) std::min<int64_t>((n + 255) / 256, 148 * 16), 256, 0, stream>>>(dst, src, n, add);
+    copy_add_kernel<<<(unsigned) std::min<int64_t>((n + 255) / 256, (int64_t) device_sm_count() * 16), 256, 0, stream>>>(dst, src, n, add);
 }
 
 int match_kernel_smem_bytes() { return (int) sizeof(WarpSmem) * WARPS_PER_CTA; }
@@ -1055,9 +1067,9 @@ void launch_match(const MatchParams& p, bool tier2, int n_warps_tier2, cudaStrea
         match_topics_kernel<true><<<ctas, WARPS_PER_CTA * 32, 0, stream>>>(p);
         return;
     }
-    int dev = 0, sms = 148;
+    int dev = 0;
     cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int sms = device_sm_count();
     // occupancy is a property of the device / context: cached per device ordinal
     static std::mutex occ_mu;
     static int occ_of[64] = {0};
@@ -1127,13 +1139,12 @@ void launch_finalize(const FinalizeParams& p, cudaStream_t stream) {
 }
 
 void launch_match_lanes(const MatchParams& p, cudaStream_t stream) {
-    int dev = 0, sms = 148;
+    int dev = 0;
     cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    // experiment switches (defaults are the measured best): BFQ_ROOTSTEP=0/1, BFQ_PREFETCH=0/1, BFQ_NOALLOC=0/1.
-    // Node records bypass L1 allocation when the batch is matched in locality order (neighbouring lanes share the top of the
-    // trie inside one request, so L1 is left to the topic bytes: 6 % faster) and allocate in L1 in arrival order (small
-    // batches; there the top trie levels live in L1 and bypassing it is 1.8x slower).
+    const int sms = device_sm_count();
+    // experiment switches: BFQ_ROOTSTEP=0/1, BFQ_PREFETCH=0/1, BFQ_NOALLOC=0/1, BFQ_CTAS=n, BFQ_CARVEOUT=percent.
+    // Node records allocate in L1: on an H100 that is faster than bypassing it (ld.global.nc.L1::no_allocate) in locality
+    // order as well as in arrival order — neighbouring lanes walk the same top of the trie, which then stays in L1.
     typedef void (*kern_t)(const MatchParams);
     static const kern_t kerns[8] = {match_topics_lane_kernel<false, false, false>, match_topics_lane_kernel<false, true, false>,
                                     match_topics_lane_kernel<true, false, false>,  match_topics_lane_kernel<true, true, false>,
@@ -1144,15 +1155,16 @@ void launch_match_lanes(const MatchParams& p, cudaStream_t stream) {
     static const int rootstep = getenv("BFQ_ROOTSTEP") ? atoi(getenv("BFQ_ROOTSTEP")) : 0;
     static const int prefetch = getenv("BFQ_PREFETCH") ? atoi(getenv("BFQ_PREFETCH")) : 1;
     static const int noalloc_forced = getenv("BFQ_NOALLOC") ? atoi(getenv("BFQ_NOALLOC")) : -1;
-    const int noalloc = noalloc_forced >= 0 ? noalloc_forced : (p.order != nullptr);
+    static const int ctas_forced = getenv("BFQ_CTAS") ? std::max(1, atoi(getenv("BFQ_CTAS"))) : 0;
+    const int noalloc = noalloc_forced >= 0 ? noalloc_forced : 0;
     const int variant = (noalloc ? 4 : 0) + (rootstep ? 2 : 0) + (prefetch ? 1 : 0);
     int ctas_per_sm;
     {
         std::lock_guard<std::mutex> g(setup_mu);
         int* ctas_of = ctas_by_dev[dev & 63];
         if (ctas_of[variant] == 0) {
-            // Shared memory and L1 share 256 KB per SM, and the kernel lives on L1 (topic bytes, top trie levels): with the
-            // 228 KB carve-out (what 8 resident CTAs need) only 28 KB of L1 remain and the kernel runs 1.5x slower (measured).
+            // Shared memory and L1 share 256 KB per SM, and the kernel lives on L1 (topic bytes, top trie levels): the
+            // 228 KB carve-out (what 8 resident CTAs need) would leave 28 KB of L1, leaving it to the driver is slower still.
             // Ask for the 196 KB carve-out (60 KB L1) and size the persistent grid for what fits there.
             cudaFuncAttributes fa{};
             cudaFuncGetAttributes(&fa, kerns[variant]);
@@ -1163,11 +1175,15 @@ void launch_match_lanes(const MatchParams& p, cudaStream_t stream) {
             cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kerns[variant], L_WARPS * 32, 0);
             const int fit = (int) ((196 * 1024) / (fa.sharedSizeBytes + 1024));
             if (occ > fit) occ = fit;
-            if (const char* ce = getenv("BFQ_CTAS")) occ = std::min(occ, std::max(1, atoi(ce)));   // experiment switch
+            if (ctas_forced) occ = std::min(occ, ctas_forced);
             ctas_of[variant] = occ < 1 ? 1 : occ;
         }
         ctas_per_sm = ctas_of[variant];
     }
+    // A large batch runs faster with fewer resident CTAs than fit: on an H100, 4 per SM beat 5 / 6 / 7 on 1M-topic batches
+    // (fewer requests contend for L1 and the memory system; there is work for every lane anyway). A smaller batch (below
+    // LARGE_BATCH_TOPICS, e.g. 100k topics) keeps every CTA that fits, or it would leave lanes it needs unscheduled.
+    if (!ctas_forced && p.n_topics >= LARGE_BATCH_TOPICS) ctas_per_sm = std::min(ctas_per_sm, LARGE_BATCH_CTAS_PER_SM);
     // persistent grid (SM count x resident CTAs); warps claim 32-topic chunks with one atomicAdd each
     if (p.max_ctas_per_sm > 0) ctas_per_sm = std::min(ctas_per_sm, (int) p.max_ctas_per_sm);
     int64_t ctas = (int64_t) sms * ctas_per_sm;
@@ -1210,7 +1226,7 @@ void launch_caps(const CapsParams& p, cudaStream_t stream) {
         return;
     }
     // counts on the device (the optimistic, sync-free enqueue): a fixed grid, then advance the handled mark
-    caps_kernel<<<148 * 4, CAPS_THREADS, 0, stream>>>(p);
+    caps_kernel<<<device_sm_count() * 4, CAPS_THREADS, 0, stream>>>(p);
     caps_advance_kernel<<<1, 1, 0, stream>>>(p.counters);
 }
 

@@ -190,6 +190,7 @@ struct CompactParams {
 // phase 1: counts + exclusive scan + total; phase 2: gather (after the caller has read the total and placed ranges_out)
 cudaError_t launch_compact(const CompactParams& p, void* d_scan_tmp, size_t* tmp_bytes, cudaStream_t stream, int phase);
 int match_kernel_smem_bytes();
+int device_sm_count();   // SMs of the current device (cached per ordinal): sizes the fixed and persistent grids
 
 // bfq_index_commit's delta path: the records of the tenants BEHIND a tenant that grew or shrank carry dense KV ranks, so
 // their own / '#' first-rank words move by the difference. One streaming pass over the listed slot regions.

@@ -1,4 +1,4 @@
-// rmatch_kernels.cu — inverse match on sm_100a: a batch of topic FILTERS against an index of TOPICS.
+// rmatch_kernels.cu — inverse match on sm_90a (H100): a batch of topic FILTERS against an index of TOPICS.
 //
 // Replaces RetainTopicIndex.match / TopicIndex.match
 //   (bifromq-retain/bifromq-retain-store/src/main/java/org/apache/bifromq/retain/store/index/RetainTopicIndex.java:36-138,
@@ -917,9 +917,7 @@ int32_t bfq_rmatch(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_
     p.overflow_list = h->d_overflow.p;
     p.counters = h->d_counters.p;
     unsigned long long hc[RC_COUNT];
-    int dev = 0, sms = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int sms = device_sm_count();
     int ctas_per_sm = 4;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, rmatch_kernel<false>, R_WARPS * 32, 0);
     ctas_per_sm = std::max(1, ctas_per_sm);

@@ -20,8 +20,8 @@
 // resident), SWAR-compares them with the key's fingerprint and loads only the slot(s) whose tag matches:
 //   hit  = 1 tag load (L2) + 1 slot load (HBM);  miss = 1 tag load, NO slot load (3% false positives);
 // and — what matters for one-lane-per-topic SIMT — the number of dependent memory round trips per lookup is
-// constant. (The first version used linear probing over the slots themselves: ncu showed a warp step waiting
-// for its longest probe chain, ~7 serial HBM round trips with 3 of 32 lanes active; profiles/r1_v3_*.)
+// constant. (Linear probing over the slots themselves makes a warp step wait for its longest probe chain: several
+// serial HBM round trips with most lanes idle.)
 //
 //   word  0      parent node id              (EMPTY_PARENT = free slot)
 //   word  1      token length in bytes       (LEN_PLUS for the '+' child, LEN_CONT|j for the j-th

@@ -1,4 +1,4 @@
-/* bfq_gpumatch.h — C-ABI of the B200 topic-filter matcher (libbfq_gpumatch.so).
+/* bfq_gpumatch.h — C-ABI of the H100 topic-filter matcher (libbfq_gpumatch.so).
  *
  * This is the drop-in boundary: everything a JNI shim needs to put the CUDA matcher behind
  * apache/bifromq's dist-worker / retain-store co-processors without touching their Java API.
@@ -84,8 +84,8 @@ int32_t bfq_index_apply(bfq_index* h, const uint8_t* add_keys, const int64_t* ad
 int32_t bfq_index_commit(bfq_index* h);
 int32_t bfq_index_generation(bfq_index* h, uint64_t* generation);   /* 0 before the first commit */
 /* Tuning knobs (defaults are the measured best for a handle that has the GPU to itself):
- *   "tier0_ctas_per_sm"  cap of the lane-per-topic kernel's resident CTAs per SM (0 = as many as fit, 7 on a B200). One slot
- *                        less leaves room for kernels that must run BESIDE the matching: the exchange of the previous batch
+ *   "tier0_ctas_per_sm"  cap of the lane-per-topic kernel's resident CTAs per SM (0 = the default: as many as fit, 7 on an
+ *                        H100, and at most 4 for batches of >= 131072 topics). One slot less leaves room for kernels that must run BESIDE the matching: the exchange of the previous batch
  *                        (bfq_exchange_gather on another stream) in a multi-GPU pipeline;
  *   "order_min_topics"   batches of at least this many topics are de-duplicated and matched in locality order (default 32768);
  *   "dedup"              0: match repeated (tenant, topic) pairs separately. */

@@ -9,7 +9,7 @@
 // oracle is pinned against every golden vector the reference's own tests carry for this
 // path (see tests/test_oracle_golden.py; SURVEY.md §8c lists them).
 //
-// Paths below are relative to /root/reference. Abbreviations:
+// Paths below are relative to the reference repository's root. Abbreviations:
 //   U/   = bifromq-util/src/main/java/org/apache/bifromq/util/
 //   DCP/ = bifromq-dist/bifromq-dist-coproc-proto/src/main/java/org/apache/bifromq/dist/trie/
 //   DW/  = bifromq-dist/bifromq-dist-worker/src/main/java/org/apache/bifromq/dist/worker/

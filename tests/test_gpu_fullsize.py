@@ -173,10 +173,9 @@ def test_c4_delta_commits_at_full_size(c4):
     r.close()
     want = kv.match_blobs(tb, toff, w.topics, off, c4.tt[lo:hi], hi - lo, INT_MAX, 100, O.MODE_TRIE, False, THREADS)
     assert np.array_equal(offsets, want.offsets) and np.array_equal(ranks, want.ranks)
-    # a commit costs the rebuild of the touched tenant plus a device-side copy: milliseconds for an ordinary tenant (tools/
-    # commit_bench.py records 5 ms at this size), well under a second for the 1.4M-route tenant — never a full build. The two
-    # small commits are looked at together: a single one can hit a slow cudaMalloc of the 2.7 GB snapshot copy (the commit
-    # traces under profiles/ show 0.2 - 0.4 s outliers in "device allocations")
+    # a commit costs the rebuild of the touched tenant plus a device-side copy: milliseconds for an ordinary tenant
+    # (tools/commit_bench.py times it), well under a second for the 1.4M-route tenant — never a full build. The two small
+    # commits are looked at together: a single one can hit a slow cudaMalloc of the 2.7 GB snapshot copy
     assert min(times[0], times[1]) < 0.25 and max(times) < 2.5, times
     print("delta commit seconds:", [round(t, 4) for t in times])
 

@@ -1,5 +1,5 @@
 """Pins the CPU oracle against the golden vectors the reference's own tests carry for this path
-(SURVEY.md §8c). Every case names the reference test it transcribes. Paths relative to /root/reference.
+(SURVEY.md §8c). Every case names the reference test it transcribes. Paths relative to the reference repository's root.
 
 The reference is Java and cannot run here (no JDK); these vectors are literal constants of its test
 sources, re-typed (inputs and expected outputs only).

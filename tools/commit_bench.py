@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Times bfq_index_commit's delta path at full BASELINE C4 size (10M filters): one SUB into tenants of different sizes, an UNSUB,
-a new tenant; prints one JSON line (committed under profiles/). Run on a GPU box:  BFQ_COMMIT_TRACE=1 python tools/commit_bench.py"""
+a new tenant; prints one JSON line. Run on a GPU machine:  BFQ_COMMIT_TRACE=1 python tools/commit_bench.py"""
 import json
 import os
 import sys

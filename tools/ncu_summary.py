@@ -1,4 +1,4 @@
-"""Turn ncu exports into the small JSON summaries committed under profiles/.
+"""Turn ncu exports into small JSON summaries.
 
   python tools/ncu_summary.py kernel <raw.csv from `ncu -i X.ncu-rep --page raw --csv`> <out.json> "<what>"
   python tools/ncu_summary.py launches <launch list csv from `ncu --metrics gpu__time_duration.sum --csv --log-file`> <out.json> "<what>"
