@@ -257,8 +257,9 @@ struct bfq_index {
     int64_t order_min = 32768;           // batches smaller than this are matched in arrival order (BFQ_ORDER=0: never order)
     bool dedup = true;                   // BFQ_DEDUP=0: match duplicates of a (tenant, topic) pair separately
     int32_t tier0_ctas_per_sm = 0;       // bfq_index_set_option("tier0_ctas_per_sm"): 0 = as many as fit
+    int32_t dedup_hash_bits = 64;        // bfq_index_set_option("dedup_hash_bits"): test knob, < 64 forces de-dup hash collisions
     double last_kernel_ms = 0;
-    int64_t launches = 0, overflow_topics = 0, flagged_topics = 0, deferred_topics = 0, duplicate_topics = 0;
+    int64_t launches = 0, overflow_topics = 0, flagged_topics = 0, deferred_topics = 0, duplicate_topics = 0, buffer_retries = 0;
     int64_t full_commits = 0, delta_commits = 0;
     // Releases the host image of a full build (2.3 GB of records at 10M filters: 0.4 s of page freeing) off the committing
     // thread. Touched under stage_mu only (commits are serialised); joined before the next one starts and at destroy.
@@ -541,6 +542,7 @@ int32_t enqueue_core(const CoreCtx& c, const SubBatch& sb, CoreOut* out) {
         q.hist_bits = 0;
         while (((size_t) 1 << q.hist_bits) < buckets) q.hist_bits++;
         q.dedup = c.h->dedup ? 1 : 0;
+        q.dedup_hash_mask = c.h->dedup_hash_bits >= 64 ? ~0ull : (1ull << c.h->dedup_hash_bits) - 1;
         q.counters = p.counters;
         CUDA_TRY(cudaMemsetAsync(q.hist, 0, hist_words(buckets) * sizeof(uint32_t), stream));
         if (q.dedup) CUDA_TRY(cudaMemsetAsync(q.hash_tab, 0xFF, ((size_t) q.hash_mask + 1) * sizeof(unsigned long long), stream));
@@ -675,6 +677,11 @@ void add_stats(bfq_index* h, const CoreOut& co, int64_t n, double kernel_ms) {
     if (kernel_ms >= 0) h->last_kernel_ms = kernel_ms;
 }
 
+void count_retry(bfq_index* h) {
+    std::lock_guard<std::mutex> g(h->mu);
+    h->buffer_retries++;
+}
+
 // grows the buffers a retry asked for (the caller has synchronised the device)
 int32_t grow_for_retry(Workspace* w, const CoreOut& co, int64_t n, int C) {
     if (co.want_dyn) {
@@ -740,6 +747,7 @@ int32_t device_wait(DeviceLease* L) {
         int32_t rc = finish_core(L->ctx, whole_batch(L->ws, L->n), &L->co, nullptr, L->ws->ev_done);
         if (rc == BFQ_OK) break;
         if (rc != BFQ_RETRY_GROW) return L->rc = rc;
+        count_retry(L->h);
         if (cudaDeviceSynchronize() != cudaSuccess) return L->rc = fail(BFQ_E_CUDA, "cudaDeviceSynchronize");
         rc = grow_for_retry(L->ws, L->co, L->n, 1);
         if (rc == BFQ_OK) rc = device_enqueue(L);
@@ -1249,7 +1257,10 @@ int32_t bfq_index_set_option(bfq_index* h, const char* name, int64_t value) {
     if (n == "tier0_ctas_per_sm") h->tier0_ctas_per_sm = (int32_t) std::max<int64_t>(0, std::min<int64_t>(value, 32));
     else if (n == "order_min_topics") h->order_min = value <= 0 ? (int64_t) 1 << 62 : value;
     else if (n == "dedup") h->dedup = value != 0;
-    else return fail(BFQ_E_INVALID, "unknown option: " + n);
+    else if (n == "dedup_hash_bits") {
+        if (value < 0 || value > 64) return fail(BFQ_E_INVALID, "dedup_hash_bits must be in [0, 64]");
+        h->dedup_hash_bits = (int32_t) value;
+    } else return fail(BFQ_E_INVALID, "unknown option: " + n);
     return BFQ_OK;
 }
 
@@ -1265,11 +1276,12 @@ int32_t bfq_index_stats(bfq_index* h, int64_t* stats, int32_t n) {
     std::lock_guard<std::mutex> g(h->mu);
     static const FlatIndex empty;
     const FlatIndex& f = h->snap ? h->snap->flat : empty;
-    const int64_t v[16] = {f.n_routes, (int64_t) f.tenant_ordinal.size(), f.n_nodes, (int64_t) f.n_slots,
+    const int64_t v[17] = {f.n_routes, (int64_t) f.tenant_ordinal.size(), f.n_nodes, (int64_t) f.n_slots,
                            h->snap ? h->snap->device_bytes() : 0, f.max_nodes_per_depth, h->launches, h->overflow_topics,
                            h->flagged_topics, f.n_multi, f.n_cont_chunks, h->deferred_topics, h->duplicate_topics,
-                           h->full_commits, h->delta_commits, h->snap ? (int64_t) h->snap->garbage_slots : 0};
-    for (int32_t i = 0; i < n && i < 16; i++) stats[i] = v[i];
+                           h->full_commits, h->delta_commits, h->snap ? (int64_t) h->snap->garbage_slots : 0,
+                           h->buffer_retries};
+    for (int32_t i = 0; i < n && i < 17; i++) stats[i] = v[i];
     return BFQ_OK;
 }
 
@@ -1642,6 +1654,7 @@ int32_t bfq_match(bfq_index* h, const uint8_t* tenants, const int64_t* tenant_of
         }
         if (!retry) break;
         // a slice of the range / throttled buffers was too small: grow them and redo the batch un-chunked
+        count_retry(h);
         CUDA_TRY(cudaDeviceSynchronize());
         rc = grow_for_retry(w, co, n, C);
         if (rc != BFQ_OK) return rc;

@@ -722,7 +722,7 @@ __global__ void __launch_bounds__(256, 4) order_prep_kernel(const OrderParams q,
     // ---- de-duplication: first inserter leads
     uint32_t lead = (uint32_t) i;
     if (q.dedup) {
-        h = fmix64(h);
+        h = fmix64(h) & q.dedup_hash_mask;
         const unsigned long long mine = ((unsigned long long) (uint32_t) (h >> 32) << 32) | (unsigned long long) (uint32_t) i;
         uint32_t slot = (uint32_t) h & q.hash_mask;
         while (true) {

@@ -142,6 +142,7 @@ struct OrderParams {
     uint32_t* ticket;               // zeroed
     int hist_bits;
     int dedup;                      // 0: every topic is its own leader
+    uint64_t dedup_hash_mask;       // bits of the de-dup hash kept after fmix64 (all of them but in tests: forced collisions)
     unsigned long long* counters;   // CTR_NLEAD is written by the scan
 };
 size_t order_hist_buckets(int64_t n_topics, int32_t n_tenants);   // histogram entries launch_order will use

@@ -88,13 +88,18 @@ int32_t bfq_index_generation(bfq_index* h, uint64_t* generation);   /* 0 before 
  *                        H100, and at most 4 for batches of >= 131072 topics). One slot less leaves room for kernels that must run BESIDE the matching: the exchange of the previous batch
  *                        (bfq_exchange_gather on another stream) in a multi-GPU pipeline;
  *   "order_min_topics"   batches of at least this many topics are de-duplicated and matched in locality order (default 32768);
- *   "dedup"              0: match repeated (tenant, topic) pairs separately. */
+ *   "dedup"              0: match repeated (tenant, topic) pairs separately;
+ *   "dedup_hash_bits"    test knob, 0..64 (default 64): keep only the low k bits of the de-dup hash, so that distinct topics
+ *                        share table slots and 32-bit tags on purpose and only the byte-for-byte compare tells them apart.
+ *                        Answers stay exact at any k; small k only makes the de-dup pass slower. */
 int32_t bfq_index_set_option(bfq_index* h, const char* name, int64_t value);
 
 /* stats[k], k < n: 0 routes, 1 tenants, 2 trie nodes, 3 hash-table slots, 4 device bytes, 5 max nodes per
  * depth, 6 kernel launches so far, 7 overflow (tier-2) topics so far, 8 cap-flagged topics so far,
  * 9 multi-segment filters, 10 long-token chunks, 11 topics handed from the lane-per-topic tier to the
- * warp-per-topic tier so far, 12 duplicate (tenant, topic) pairs answered from their first occurrence so far */
+ * warp-per-topic tier so far, 12 duplicate (tenant, topic) pairs answered from their first occurrence so far,
+ * 13 full commits, 14 delta commits, 15 garbage slots of the current snapshot, 16 match calls that found a range or
+ * throttle buffer too small, grew it and re-ran the batch so far */
 int32_t bfq_index_stats(bfq_index* h, int64_t* stats, int32_t n);
 /* device time of the tier-0 (lane-per-topic) match kernel of the latest completed match call on this handle, measured with
  * CUDA events recorded on the launching stream around the launch (for roofline accounting) */
