@@ -24,6 +24,7 @@
 #include <chrono>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <tuple>
@@ -470,9 +471,14 @@ struct DBuf {
 
 }  // namespace
 
+// id -> (tenant, topic); tombstones keep their slot. bfq_rindex_reset starts a new table, so ids restart at 0 there while the
+// snapshot and its results still name ids of the old one.
+using IdTable = std::vector<std::pair<std::string, std::string>>;
+
 struct bfq_rresult {
     std::vector<int64_t> offsets, ids, totals;
     double ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    std::shared_ptr<const IdTable> by_id;   // the id table of the snapshot the match ran on
 };
 
 struct bfq_rindex {
@@ -483,9 +489,10 @@ struct bfq_rindex {
     unsigned long long* h_small = nullptr;   // pinned scalars
     // staging: (tenant, topic) -> id ; id -> (tenant, topic)
     std::map<std::pair<std::string, std::string>, int64_t> staged;
-    std::vector<std::pair<std::string, std::string>> by_id;   // id -> strings (tombstones keep their slot)
+    std::shared_ptr<IdTable> by_id = std::make_shared<IdTable>();   // staging: add / load_keys append here
     std::vector<char> alive;
     bool have_snapshot = false;
+    std::shared_ptr<const IdTable> committed;   // the table by_id was when the snapshot was built (append-only since)
     // snapshot
     std::unordered_map<std::string, int32_t> tenant_root;
     uint32_t n_blocks = 0;
@@ -744,7 +751,7 @@ int32_t bfq_rindex_reset(bfq_rindex* h) {
     if (!h) return rfail(BFQ_E_INVALID, "handle is NULL");
     std::lock_guard<std::mutex> g(h->mu);
     h->staged.clear();
-    h->by_id.clear();
+    h->by_id = std::make_shared<IdTable>();   // the committed table stays with the snapshot and its results
     h->alive.clear();
     return BFQ_OK;
 }
@@ -762,8 +769,8 @@ int32_t bfq_rindex_add(bfq_rindex* h, const uint8_t* tenants, const int64_t* ten
         auto it = h->staged.find(key);
         int64_t id;
         if (it == h->staged.end()) {
-            id = (int64_t) h->by_id.size();
-            h->by_id.push_back(key);
+            id = (int64_t) h->by_id->size();
+            h->by_id->push_back(key);
             h->alive.push_back(1);
             h->staged.emplace(std::move(key), id);
         } else {
@@ -792,8 +799,8 @@ int32_t bfq_rindex_load_keys(bfq_rindex* h, const uint8_t* keys, const int64_t* 
         auto it = h->staged.find(key);
         int64_t id;
         if (it == h->staged.end()) {
-            id = (int64_t) h->by_id.size();
-            h->by_id.push_back(key);
+            id = (int64_t) h->by_id->size();
+            h->by_id->push_back(key);
             h->alive.push_back(1);
             h->staged.emplace(std::move(key), id);
         } else {
@@ -806,15 +813,18 @@ int32_t bfq_rindex_load_keys(bfq_rindex* h, const uint8_t* keys, const int64_t* 
 
 // retainMessageKey(tenant, topic) of every id in a match result, in result order: the keys of the follow-up reader.get calls of
 // RetainStoreCoProc.match (RS/RetainStoreCoProc.java:177-188), as one batch. Returns the blob length; copies if it fits.
+// The ids are resolved in the id table of the snapshot the match ran on, so a reset + reload between the match and this call
+// does not change the answer. h->mu is still taken: add / load_keys append to that same table until the next reset.
 int64_t bfq_rresult_retain_keys(bfq_rindex* h, const bfq_rresult* r, uint8_t* blob_out, int64_t blob_cap, int64_t* key_off_out) {
     if (!h || !r) return BFQ_E_INVALID;
     std::lock_guard<std::mutex> g(h->mu);
     int64_t at = 0;
     const int64_t n = (int64_t) r->ids.size();
+    const IdTable& by_id = *r->by_id;   // set by bfq_rmatch, which runs only after a commit
     for (int64_t i = 0; i < n; i++) {
         const int64_t id = r->ids[(size_t) i];
-        if (id < 0 || id >= (int64_t) h->by_id.size()) return BFQ_E_RANGE;
-        const std::string k = make_retain_key(h->by_id[(size_t) id].first, h->by_id[(size_t) id].second);
+        if (id < 0 || id >= (int64_t) by_id.size()) return BFQ_E_RANGE;
+        const std::string k = make_retain_key(by_id[(size_t) id].first, by_id[(size_t) id].second);
         if (key_off_out) key_off_out[i] = at;
         if (blob_out && at + (int64_t) k.size() <= blob_cap) memcpy(blob_out + at, k.data(), k.size());
         at += (int64_t) k.size();
@@ -837,15 +847,17 @@ int32_t bfq_rindex_remove(bfq_rindex* h, const uint8_t* tenant, int64_t tn, cons
 int32_t bfq_rindex_commit(bfq_rindex* h) {
     if (!h) return rfail(BFQ_E_INVALID, "handle is NULL");
     std::lock_guard<std::mutex> g(h->mu);
-    return rebuild(h);
+    const int32_t rc = rebuild(h);
+    if (rc == BFQ_OK) h->committed = h->by_id;
+    return rc;
 }
 
 int32_t bfq_rindex_lookup(bfq_rindex* h, int64_t id, uint8_t* tenant_out, int64_t tenant_cap, int64_t* tenant_len,
                           uint8_t* topic_out, int64_t topic_cap, int64_t* topic_len) {
     if (!h) return rfail(BFQ_E_INVALID, "handle is NULL");
     std::lock_guard<std::mutex> g(h->mu);
-    if (id < 0 || id >= (int64_t) h->by_id.size()) return rfail(BFQ_E_RANGE, "id out of range");
-    const auto& e = h->by_id[(size_t) id];
+    if (id < 0 || id >= (int64_t) h->by_id->size()) return rfail(BFQ_E_RANGE, "id out of range");
+    const auto& e = (*h->by_id)[(size_t) id];
     if (tenant_len) *tenant_len = (int64_t) e.first.size();
     if (topic_len) *topic_len = (int64_t) e.second.size();
     if (tenant_out && (int64_t) e.first.size() <= tenant_cap) memcpy(tenant_out, e.first.data(), e.first.size());
@@ -885,6 +897,7 @@ int32_t bfq_rmatch(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_
     RCUDA_TRY(h->d_counters.reserve(RC_COUNT));
     if (h->d_ranges.cap == 0) RCUDA_TRY(h->d_ranges.reserve(std::max<size_t>(1 << 18, 8 * nn)));
     auto* res = new bfq_rresult();
+    res->by_id = h->committed;
     res->offsets.assign((size_t) n + 1, 0);
     res->totals.assign((size_t) n, 0);
     if (n == 0) {

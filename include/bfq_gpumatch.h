@@ -339,7 +339,8 @@ int32_t bfq_rindex_add(bfq_rindex* h, const uint8_t* tenants, const int64_t* ten
 int32_t bfq_rindex_load_keys(bfq_rindex* h, const uint8_t* keys, const int64_t* key_off, int64_t n, int64_t* ids_out);
 int32_t bfq_rindex_remove(bfq_rindex* h, const uint8_t* tenant, int64_t tn, const uint8_t* topic, int64_t n);
 int32_t bfq_rindex_commit(bfq_rindex* h);
-/* topic id -> (tenant, topic) strings */
+/* topic id -> (tenant, topic) strings, resolved against the STAGED ids: after bfq_rindex_reset ids restart at 0, so an id of an
+ * earlier result may name another topic here (bfq_rresult_retain_keys resolves against the result's own snapshot instead) */
 int32_t bfq_rindex_lookup(bfq_rindex* h, int64_t id, uint8_t* tenant_out, int64_t tenant_cap, int64_t* tenant_len,
                           uint8_t* topic_out, int64_t topic_cap, int64_t* topic_len);
 /* match n filters; filter i is scoped to tenant filter_tenant[i]; limit[i] < 0 = unlimited, else at most
@@ -354,7 +355,11 @@ int32_t bfq_rmatch(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_
                    const int64_t* limit, bfq_rresult** out);
 int64_t bfq_rresult_num_filters(const bfq_rresult* r);
 const int64_t* bfq_rresult_offsets(const bfq_rresult* r);            /* [n_filters+1] */
-const int64_t* bfq_rresult_ids(const bfq_rresult* r, int64_t* n);    /* topic ids, ascending per filter */
+/* topic ids of filter i at [offsets[i], offsets[i + 1]). Ids are handed out in insertion order and returned in trie order, so
+ * they are NOT sorted. What holds: the ids of a filter are distinct; a filter's answer depends only on the filter, its tenant
+ * and the snapshot, not on the rest of the batch or where the filter sits in it; with limit[i] = k >= 0 the answer is the
+ * first min(k, total) ids of the unlimited answer */
+const int64_t* bfq_rresult_ids(const bfq_rresult* r, int64_t* n);
 const int64_t* bfq_rresult_total_matches(const bfq_rresult* r);      /* [n_filters] matches before the limit */
 /* ms[0..3]: wall time of the H2D section, the kernel section, the D2H section, the whole call; ms[4]: DEVICE time from
  * "inputs resident" to "ids expanded" (CUDA events on the call's stream); ms[5]: device time of rmatch_kernel alone;
@@ -362,7 +367,9 @@ const int64_t* bfq_rresult_total_matches(const bfq_rresult* r);      /* [n_filte
 int32_t bfq_rresult_timings(const bfq_rresult* r, double* ms, int32_t n);
 /* retainMessageKey of every id of the result, in result order, as one (blob, key_off[n_ids + 1]) batch: the keys of the
  * follow-up reader.get calls of RetainStoreCoProc.match (RS/RetainStoreCoProc.java:177-188). Returns the blob length (or a
- * negative BFQ_E_*); copies only if it fits blob_cap; key_off_out may be NULL. */
+ * negative BFQ_E_*); copies only if it fits blob_cap; key_off_out may be NULL. The ids are resolved against the id table of
+ * the snapshot the match ran on, which the result keeps alive: a bfq_rindex_reset + reload (or a match run between a reset
+ * and the next commit) still gets the keys of the topics the result matched. */
 int64_t bfq_rresult_retain_keys(bfq_rindex* h, const bfq_rresult* r, uint8_t* blob_out, int64_t blob_cap, int64_t* key_off_out);
 void bfq_rresult_free(bfq_rresult* r);
 
