@@ -102,6 +102,7 @@ _SIGNATURES = {
     "bfq_rresult_retain_keys": (_i64, [_vp, _vp, _vp, _i64, _vp]),
     "bfq_rindex_remove": (_i32, [_vp, C.c_char_p, _i64, C.c_char_p, _i64]),
     "bfq_rindex_commit": (_i32, [_vp]),
+    "bfq_rindex_stats": (_i32, [_vp, _vp, _i32]),
     "bfq_rindex_lookup": (_i32, [_vp, _i64, _vp, _i64, C.POINTER(_i64), _vp, _i64, C.POINTER(_i64)]),
     "bfq_rmatch": (_i32, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp, C.POINTER(_vp)]),
     "bfq_rresult_num_filters": (_i64, [_vp]),

@@ -6,7 +6,8 @@
 //    traversal bifromq-util/src/main/java/org/apache/bifromq/util/index/TopicLevelTrie.java:190-249).
 // Same machinery as the forward kernel with the roles swapped: ONE WARP PER FILTER walks the topic trie.
 //
-// Layout (HBM): the per-tenant topic tries are numbered in one global BFS, so
+// Layout (HBM): each tenant's topic trie is one region of BFS-numbered node records (see the layout comment above
+// rebuild_full; a delta commit appends the rebuilt tenants' regions), so
 //   * the children of a node — and the children of any RUN of consecutive nodes of one depth — are one
 //     contiguous id interval: a '+' level maps a frontier interval to ONE interval with two record loads,
 //     it never explodes the frontier;
@@ -26,6 +27,7 @@
 #include <map>
 #include <memory>
 #include <mutex>
+#include <set>
 #include <string>
 #include <tuple>
 #include <unordered_map>
@@ -50,7 +52,7 @@ int32_t rfail(int32_t code, const std::string& msg) { return bfq::set_error(code
         if (_e != cudaSuccess) return rfail(BFQ_E_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e)); \
     } while (0)
 
-// one topic-trie node, indexed by BFS id; rnodes has a sentinel entry at [n_nodes]
+// one topic-trie node, indexed by node id; the node array has a sentinel entry at [n_nodes]
 struct RNode {
     uint32_t child_begin;   // BFS id of the first child (children are consecutive)
     uint32_t child_count;
@@ -114,7 +116,7 @@ __device__ __forceinline__ RNode load_node(const RNode* n) {
 }
 
 // (parent, lenw, k) -> child id, or NONE; *nd = the child's record (without its '$' run), *own_next = own_prefix of the node
-// behind it — both carried in the slot's payload half (see rebuild)
+// behind it — both carried in the slot's payload half (see build_tenant)
 __device__ __forceinline__ uint32_t rprobe(const Slot* slots, const uint4* tags, uint32_t n_blocks, uint32_t parent, uint32_t lenw,
                                            const uint32_t (&k)[6], uint64_t tokh, RNode* nd, uint32_t* own_next) {
     uint32_t w[16], slot = 0;
@@ -449,6 +451,51 @@ __global__ void __launch_bounds__(256) rexpand_kernel(int64_t n, const uint32_t*
     }
 }
 
+// Inserts the exact edges of the regions a delta commit appended into the live tag table, one thread per edge. img[i] is the
+// finished 64-byte slot (key words 0..7, payload 8..15). The probe sequence is EdgeTable::place's: the first free tag of the
+// 15 usable ones in the home block, else mark the block overflowed (control byte) and go on to the next block. A tag byte is
+// claimed with atomicCAS on its 32-bit tag word, retried while other threads change that word. The caller keeps the table
+// below full (the occupancy bound of the delta path), so every thread finds a free slot.
+__global__ void __launch_bounds__(256) rinsert_edges_kernel(const Slot* __restrict__ img, int64_t n, Slot* slots, uint32_t* tags,
+                                                            uint32_t n_blocks, unsigned long long* overflowed) {
+    const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint4* src = reinterpret_cast<const uint4*>(img + i);
+    const uint4 a = src[0], b = src[1];
+    const uint32_t k[6] = {a.z, a.w, b.x, b.y, b.z, b.w};
+    const uint64_t h = edge_hash(token_hash(a.y, k), a.x);
+    const uint32_t fp = fingerprint(h);
+    uint32_t blk = home_block(h, n_blocks);
+    while (true) {
+        uint32_t* tw = tags + (size_t) blk * 4;
+        for (int q = 0; q < 4; q++) {
+            const int bytes = q == 3 ? 3 : 4;   // byte 15 of the block is the control byte
+            uint32_t cur = *reinterpret_cast<volatile uint32_t*>(tw + q);
+            while (true) {
+                int j = -1;
+                for (int t = 0; t < bytes; t++)
+                    if (((cur >> (8 * t)) & 0xFFu) == 0) {
+                        j = t;
+                        break;
+                    }
+                if (j < 0) break;
+                const uint32_t old = atomicCAS(tw + q, cur, cur | (fp << (8 * j)));
+                if (old == cur) {
+                    uint4* dst = reinterpret_cast<uint4*>(slots + (size_t) blk * BLOCK_SLOTS + (uint32_t) (q * 4 + j));
+                    dst[0] = a;
+                    dst[1] = b;
+                    dst[2] = src[2];
+                    dst[3] = src[3];
+                    return;
+                }
+                cur = old;
+            }
+        }
+        if ((atomicOr(tw + 3, 1u << 24) >> 24) == 0) atomicAdd(overflowed, 1ull);
+        blk = blk + 1 == n_blocks ? 0 : blk + 1;
+    }
+}
+
 template <typename T>
 struct DBuf {
     T* p = nullptr;
@@ -462,6 +509,25 @@ struct DBuf {
         if (e == cudaSuccess) cap = n;
         return e;
     }
+    // like reserve, but keeps the first `keep` elements (device-to-device copy on st) and grows by at least half the capacity
+    cudaError_t grow(size_t n, size_t keep, cudaStream_t st) {
+        if (n <= cap) return cudaSuccess;
+        const size_t want = std::max(n, cap + cap / 2);
+        T* q = nullptr;
+        cudaError_t e = cudaMalloc(&q, want * sizeof(T));
+        if (e != cudaSuccess) return e;
+        if (keep) e = cudaMemcpyAsync(q, p, keep * sizeof(T), cudaMemcpyDeviceToDevice, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) {
+            cudaFree(q);
+            return e;
+        }
+        if (p) cudaFree(p);
+        p = q;
+        cap = want;
+        return cudaSuccess;
+    }
+    size_t bytes() const { return cap * sizeof(T); }
     void release() {
         if (p) cudaFree(p);
         p = nullptr;
@@ -481,6 +547,13 @@ struct bfq_rresult {
     std::shared_ptr<const IdTable> by_id;   // the id table of the snapshot the match ran on
 };
 
+// where a live tenant's trie sits in the snapshot (see the layout comment above rebuild_full)
+struct TenantRegion {
+    uint32_t root = 0;      // node id of the root = first node of the region
+    uint32_t n_nodes = 0;
+    int64_t n_topics = 0;
+};
+
 struct bfq_rindex {
     int device = 0;
     std::mutex mu;
@@ -491,16 +564,27 @@ struct bfq_rindex {
     std::map<std::pair<std::string, std::string>, int64_t> staged;
     std::shared_ptr<IdTable> by_id = std::make_shared<IdTable>();   // staging: add / load_keys append here
     std::vector<char> alive;
+    std::set<std::string> dirty;   // tenants whose staged topic set changed since the last commit
+    bool need_full = true;         // the next commit is a full build (no snapshot yet, reset, bulk load onto an empty handle)
     bool have_snapshot = false;
     std::shared_ptr<const IdTable> committed;   // the table by_id was when the snapshot was built (append-only since)
     // snapshot
     std::unordered_map<std::string, int32_t> tenant_root;
+    std::unordered_map<std::string, TenantRegion> regions;   // the live tenants' regions
     uint32_t n_blocks = 0;
-    int64_t n_nodes = 0, max_nodes_per_depth = 0, n_topics = 0;
+    int64_t n_nodes = 0, max_nodes_per_depth = 0, n_topics = 0;   // n_nodes: records of every region, garbage included
+    int64_t n_dfs = 0, n_bfs = 0;          // DFS / BFS ranks handed out, garbage included
+    uint32_t next_virtual = 0;             // next free id of a long-name chunk node
+    int64_t garbage_nodes = 0;             // records of replaced regions and vanished tenants
+    int64_t used_slots = 0;                // occupied table slots, garbage included
+    int64_t overflowed_blocks = 0;
+    int64_t full_commits = 0, delta_commits = 0, last_rebuilt = 0;
     DBuf<RNode> d_nodes;
     DBuf<Slot> d_slots;
     DBuf<uint8_t> d_tags;
     DBuf<int64_t> d_dfs_to_id, d_bfs_to_id;
+    DBuf<Slot> d_new_slots;                // slot images of a delta commit
+    DBuf<unsigned long long> d_ins_ctr;
     // workspace
     DBuf<uint8_t> d_filters, d_scan_tmp;
     DBuf<int64_t> d_filter_off, d_limit, d_ids;
@@ -513,6 +597,15 @@ struct bfq_rindex {
     DBuf<unsigned long long> d_ord_ctr;
     int64_t launches = 0;
 
+    int64_t device_bytes() const {
+        return (int64_t) (d_nodes.bytes() + d_slots.bytes() + d_tags.bytes() + d_dfs_to_id.bytes() + d_bfs_to_id.bytes() +
+                          d_filters.bytes() + d_scan_tmp.bytes() + d_filter_off.bytes() + d_limit.bytes() + d_ids.bytes() +
+                          d_filter_tenant.bytes() + d_tenant_root.bytes() + d_span_begin.bytes() + d_span_count.bytes() +
+                          d_overflow.bytes() + d_total.bytes() + d_kept.bytes() + d_offsets.bytes() + d_counters.bytes() +
+                          d_ranges.bytes() + d_scratch.bytes() + d_ord_keys.bytes() + d_ord_leader.bytes() + d_order.bytes() +
+                          d_hist.bytes() + d_ord_ctr.bytes() + d_new_slots.bytes() + d_ins_ctr.bytes());
+    }
+
     ~bfq_rindex() {
         cudaSetDevice(device);
         d_nodes.release(); d_slots.release(); d_tags.release(); d_dfs_to_id.release(); d_bfs_to_id.release(); d_filters.release();
@@ -520,6 +613,7 @@ struct bfq_rindex {
         d_tenant_root.release(); d_span_begin.release(); d_span_count.release(); d_overflow.release(); d_total.release();
         d_kept.release(); d_offsets.release(); d_counters.release(); d_ranges.release(); d_scratch.release();
         d_ord_keys.release(); d_ord_leader.release(); d_order.release(); d_hist.release(); d_ord_ctr.release();
+        d_new_slots.release(); d_ins_ctr.release();
         for (auto& e : ev) if (e) cudaEventDestroy(e);
         if (h_small) cudaFreeHost(h_small);
         if (stream) cudaStreamDestroy(stream);
@@ -539,27 +633,39 @@ inline void make_tok(sv chunk, uint32_t* tok) {
     for (size_t j = 0; j < chunk.size(); j++) tok[j >> 2] |= (uint32_t) (uint8_t) chunk[j] << (8 * (j & 3));
 }
 
-struct Edge {
-    uint32_t parent, lenw, tok[TOKEN_WORDS], child;
+using Staged = std::map<std::pair<std::string, std::string>, int64_t>;
+
+// Snapshot layout. Every live tenant owns one REGION of consecutive node ids: its root first, then its trie in BFS order from
+// that root (level by level, children in bytewise name order, so the '$' children of a node are one run). Its topics get
+// consecutive DFS ranks (pre-order, own topic first) and consecutive BFS ranks (by the id of the node they end at). A full build
+// places the regions back to back in bytewise tenant order; a delta commit appends the rebuilt tenants' regions behind all
+// existing ones, and the regions they replace (and those of tenants that vanished) stay in place as garbage that no tenant root
+// reaches, until the next full build. The kernels rely on these invariants, which deltas keep:
+//   * BFS ranks are assigned in node-id order over the whole array, garbage regions included, so own_prefix is monotone;
+//   * the record after a region's last node carries that region's rank end in own_prefix: it is the next region's root, or
+//     the one sentinel record at [n_nodes], which is rewritten on every append;
+//   * node ids stay below VIRT_BASE, ranks below SPACE_BFS, and long-name chunk ids between VIRT_BASE and NONE.
+// Within a region this is exactly the layout of one tenant in a single global BFS, so answers (ids and their order), range
+// counts and tier hand-offs do not depend on where a tenant's region sits.
+struct TenantImage {
+    std::vector<RNode> rn;                    // the region's records, node_base.. (no sentinel)
+    std::vector<int64_t> dfs_to_id, bfs_to_id;
+    std::vector<Slot> slots;                  // the region's exact edges as finished slot images
+    int64_t max_depth_nodes = 0;              // the largest number of the tenant's nodes at one depth
+    uint32_t n_virtual = 0;                   // chunk-node ids used from virt_base on
 };
 
-int32_t rebuild(bfq_rindex* h) {
-    std::vector<HNode> nodes;
-    std::unordered_map<std::string, uint32_t> root_of;
-    std::vector<uint32_t> roots;
-    for (const auto& e : h->staged) {
-        const std::string& tenant = e.first.first;
-        auto it = root_of.find(tenant);
-        uint32_t cur;
-        if (it == root_of.end()) {
-            nodes.emplace_back();
-            cur = (uint32_t) nodes.size() - 1;
-            root_of.emplace(tenant, cur);
-            roots.push_back(cur);
-        } else {
-            cur = it->second;
-        }
-        for_each_level(sv(e.first.second), '/', [&](sv l) {
+constexpr uint64_t ID_LIMIT = 0x7FFFFFF0ull;     // node ids and ranks stay below this (VIRT_BASE / SPACE_BFS)
+constexpr uint64_t VIRT_LIMIT = 0xFFFFFFF0ull;   // chunk-node ids stay below this (NONE / EMPTY_PARENT)
+
+// The trie of one tenant's topics [first, last) of the staging map, with node ids from node_base, DFS ranks from dfs_base,
+// BFS ranks from bfs_base and chunk-node ids from virt_base.
+int32_t build_tenant(Staged::const_iterator first, Staged::const_iterator last, uint32_t node_base, uint32_t dfs_base,
+                     uint32_t bfs_base, uint32_t virt_base, TenantImage* out) {
+    std::vector<HNode> nodes(1);
+    for (auto it = first; it != last; ++it) {
+        uint32_t cur = 0;
+        for_each_level(sv(it->first.second), '/', [&](sv l) {
             auto c = nodes[cur].children.find(std::string(l));
             if (c == nodes[cur].children.end()) {
                 nodes.emplace_back();
@@ -570,15 +676,15 @@ int32_t rebuild(bfq_rindex* h) {
                 cur = c->second;
             }
         });
-        nodes[cur].own = e.second;
+        nodes[cur].own = it->second;
     }
     const size_t N = nodes.size();
-    if (N >= 0x7FFFFFF0ull) return rfail(BFQ_E_RANGE, "topic index too large");
-    // ---- BFS numbering (roots first, then level by level in parent order)
+    if (N >= ID_LIMIT) return rfail(BFQ_E_RANGE, "topic index too large");
+    // ---- BFS numbering from the root, level by level in parent order
     std::vector<uint32_t> order;
     order.reserve(N);
-    for (uint32_t r : roots) order.push_back(r);
-    int64_t max_depth_nodes = (int64_t) roots.size();
+    order.push_back(0);
+    int64_t max_depth_nodes = 1;
     for (size_t lo = 0, hi = order.size(); lo < hi;) {
         for (size_t i = lo; i < hi; i++)
             for (const auto& c : nodes[order[i]].children) order.push_back(c.second);
@@ -587,22 +693,23 @@ int32_t rebuild(bfq_rindex* h) {
         max_depth_nodes = std::max<int64_t>(max_depth_nodes, (int64_t) (hi - lo));
     }
     for (size_t i = 0; i < N; i++) nodes[order[i]].bfs = (uint32_t) i;
-    std::vector<RNode> rn(N + 1);
-    std::vector<int64_t> bfs_to_id, dfs_to_id;
+    TenantImage& im = *out;
+    im.rn.assign(N, RNode{});
+    im.max_depth_nodes = max_depth_nodes;
+    std::vector<RNode>& rn = im.rn;
+    std::vector<int64_t>& bfs_to_id = im.bfs_to_id;
+    std::vector<int64_t>& dfs_to_id = im.dfs_to_id;
     // child intervals + BFS topic ranks
     {
-        uint32_t next_child = (uint32_t) roots.size();
+        uint32_t next_child = node_base + 1;
         for (size_t i = 0; i < N; i++) {
             const HNode& hn = nodes[order[i]];
             RNode& r = rn[i];
             r.child_begin = next_child;
             r.child_count = (uint32_t) hn.children.size();
             next_child += r.child_count;
-            r.own_prefix = (uint32_t) bfs_to_id.size();
+            r.own_prefix = bfs_base + (uint32_t) bfs_to_id.size();
             if (hn.own >= 0) bfs_to_id.push_back(hn.own);
-            r.sys_begin = 0;
-            r.sys_count = 0;
-            r.pad = 0;
             uint32_t k = 0;
             for (const auto& c : hn.children) {
                 if (!c.first.empty() && c.first[0] == '$') {
@@ -612,96 +719,136 @@ int32_t rebuild(bfq_rindex* h) {
                 k++;
             }
         }
-        rn[N] = RNode{next_child, 0, 0, 0, (uint32_t) bfs_to_id.size(), 0, 0, 0};
     }
+    const uint32_t rank_end = bfs_base + (uint32_t) bfs_to_id.size();   // own_prefix of the record behind the region
     // DFS (pre-order) topic ranks, iterative
     {
         std::vector<std::pair<uint32_t, std::map<std::string, uint32_t>::const_iterator>> st;
-        for (uint32_t r : roots) {
-            st.clear();
-            rn[nodes[r].bfs].sub_begin = (uint32_t) dfs_to_id.size();
-            if (nodes[r].own >= 0) dfs_to_id.push_back(nodes[r].own);
-            st.push_back({r, nodes[r].children.begin()});
-            while (!st.empty()) {
-                auto& top = st.back();
-                if (top.second == nodes[top.first].children.end()) {
-                    rn[nodes[top.first].bfs].sub_end = (uint32_t) dfs_to_id.size();
-                    st.pop_back();
-                    continue;
-                }
-                uint32_t c = top.second->second;
-                ++top.second;
-                rn[nodes[c].bfs].sub_begin = (uint32_t) dfs_to_id.size();
-                if (nodes[c].own >= 0) dfs_to_id.push_back(nodes[c].own);
-                st.push_back({c, nodes[c].children.begin()});
+        rn[0].sub_begin = dfs_base;
+        if (nodes[0].own >= 0) dfs_to_id.push_back(nodes[0].own);
+        st.push_back({0u, nodes[0].children.begin()});
+        while (!st.empty()) {
+            auto& top = st.back();
+            if (top.second == nodes[top.first].children.end()) {
+                rn[nodes[top.first].bfs].sub_end = dfs_base + (uint32_t) dfs_to_id.size();
+                st.pop_back();
+                continue;
             }
+            uint32_t c = top.second->second;
+            ++top.second;
+            rn[nodes[c].bfs].sub_begin = dfs_base + (uint32_t) dfs_to_id.size();
+            if (nodes[c].own >= 0) dfs_to_id.push_back(nodes[c].own);
+            st.push_back({c, nodes[c].children.begin()});
         }
     }
-    // ---- exact-edge hash table keyed by the parent's BFS id (long names: chains of virtual nodes)
-    std::vector<Edge> edges;
-    edges.reserve(N);
-    uint32_t next_virtual = VIRT_BASE;
+    // ---- exact edges keyed by the parent's node id (long names: chains of virtual nodes)
+    auto slot_of = [](uint32_t parent, uint32_t lenw, sv chunk, uint32_t child) {
+        Slot s{};
+        s.w[W_PARENT] = parent;
+        s.w[W_LEN] = lenw;
+        make_tok(chunk, &s.w[W_TOK]);
+        s.w[W_PLUS] = child;
+        return s;
+    };
+    std::vector<Slot>& slots = im.slots;
+    slots.reserve(N);
+    uint64_t next_virtual = virt_base;
     std::map<std::tuple<uint32_t, uint32_t, std::string>, uint32_t> virt;
     for (size_t i = 0; i < N; i++) {
         const HNode& hn = nodes[order[i]];
         for (const auto& c : hn.children) {
             sv name(c.first);
-            uint32_t parent = (uint32_t) i;
+            uint32_t parent = node_base + (uint32_t) i;
             size_t off = 0;
             uint32_t j = 0;
             while (name.size() - off > TOKEN_BYTES) {
-                Edge e{};
-                e.parent = parent;
-                e.lenw = LEN_CONT | j;
-                make_tok(name.substr(off, TOKEN_BYTES), e.tok);
+                const sv chunk = name.substr(off, TOKEN_BYTES);
                 // identical chunk prefixes under the same parent share one virtual node
-                auto vk = std::make_tuple(e.parent, e.lenw, std::string((const char*) e.tok, sizeof(e.tok)));
+                auto vk = std::make_tuple(parent, LEN_CONT | j, std::string(chunk));
                 auto vit = virt.find(vk);
-                uint32_t found;
                 if (vit == virt.end()) {
-                    e.child = next_virtual++;
-                    edges.push_back(e);
-                    virt.emplace(std::move(vk), e.child);
-                    found = e.child;
+                    if (next_virtual >= VIRT_LIMIT) return rfail(BFQ_E_RANGE, "topic index too large");
+                    const uint32_t v = (uint32_t) next_virtual++;
+                    slots.push_back(slot_of(parent, LEN_CONT | j, chunk, v));
+                    virt.emplace(std::move(vk), v);
+                    parent = v;
                 } else {
-                    found = vit->second;
+                    parent = vit->second;
                 }
-                parent = found;
                 off += TOKEN_BYTES;
                 j++;
             }
-            Edge e{};
-            e.parent = parent;
-            e.lenw = (uint32_t) name.size();
-            make_tok(name.substr(off), e.tok);
-            e.child = nodes[c.second].bfs;
-            edges.push_back(e);
-        }
-    }
-    if (((uint64_t) edges.size() * 2 / BLOCK_USABLE + 64) * BLOCK_SLOTS >= 0x7FFFFFF0ull) return rfail(BFQ_E_RANGE, "topic index too large");
-    EdgeTable table;
-    table.init(edges.size());
-    for (const Edge& e : edges) {
-        const uint32_t s = table.place(e.parent, e.lenw, e.tok);
-        uint32_t* w = table.slots[s].w;
-        w[W_PLUS] = e.child;
-        if (e.child < VIRT_BASE) {
+            const uint32_t local = nodes[c.second].bfs;
+            Slot s = slot_of(parent, (uint32_t) name.size(), name.substr(off), node_base + local);
             // the child's node record rides in the slot's payload half: an exact step is tag + slot, with no third dependent
             // access for the record (words 9..14: child_begin, child_count, sub_begin, sub_end, own_prefix, own_prefix of the
             // next node; the '$' run is only needed for tenant roots, which are never reached through a slot)
-            const RNode& r = rn[e.child];
-            w[9] = r.child_begin;
-            w[10] = r.child_count;
-            w[11] = r.sub_begin;
-            w[12] = r.sub_end;
-            w[13] = r.own_prefix;
-            w[14] = rn[e.child + 1].own_prefix;
+            const RNode& r = rn[local];
+            s.w[9] = r.child_begin;
+            s.w[10] = r.child_count;
+            s.w[11] = r.sub_begin;
+            s.w[12] = r.sub_end;
+            s.w[13] = r.own_prefix;
+            s.w[14] = local + 1 < N ? rn[local + 1].own_prefix : rank_end;
+            slots.push_back(s);
         }
     }
+    im.n_virtual = (uint32_t) (next_virtual - virt_base);
+    return BFQ_OK;
+}
+
+template <typename T>
+void append(std::vector<T>& a, const std::vector<T>& b) {
+    a.insert(a.end(), b.begin(), b.end());
+}
+
+// the half-open run of one tenant's topics in the staging map
+std::pair<Staged::const_iterator, Staged::const_iterator> tenant_run(const Staged& staged, Staged::const_iterator first) {
+    auto last = first;
+    while (last != staged.end() && last->first.first == first->first.first) ++last;
+    return {first, last};
+}
+
+// Full build: build_tenant over every tenant, regions back to back in bytewise tenant order, one fresh tag table.
+int32_t rebuild_full(bfq_rindex* h) {
+    std::vector<RNode> rn;
+    std::vector<int64_t> dfs_to_id, bfs_to_id;
+    std::vector<Slot> imgs;
+    std::unordered_map<std::string, TenantRegion> regions;
+    int64_t max_depth_nodes = 0;
+    uint64_t next_virtual = VIRT_BASE;
+    for (auto it = h->staged.cbegin(); it != h->staged.cend();) {
+        const auto run = tenant_run(h->staged, it);
+        TenantImage im;
+        const int32_t rc = build_tenant(run.first, run.second, (uint32_t) rn.size(), (uint32_t) dfs_to_id.size(),
+                                        (uint32_t) bfs_to_id.size(), (uint32_t) next_virtual, &im);
+        if (rc != BFQ_OK) return rc;
+        if (rn.size() + im.rn.size() + 1 >= ID_LIMIT || dfs_to_id.size() + im.dfs_to_id.size() >= ID_LIMIT)
+            return rfail(BFQ_E_RANGE, "topic index too large");
+        TenantRegion reg;
+        reg.root = (uint32_t) rn.size();
+        reg.n_nodes = (uint32_t) im.rn.size();
+        reg.n_topics = (int64_t) im.dfs_to_id.size();
+        regions.emplace(it->first.first, reg);
+        append(rn, im.rn);
+        append(dfs_to_id, im.dfs_to_id);
+        append(bfs_to_id, im.bfs_to_id);
+        append(imgs, im.slots);
+        next_virtual += im.n_virtual;
+        max_depth_nodes = std::max(max_depth_nodes, im.max_depth_nodes);
+        it = run.second;
+    }
+    const size_t N = rn.size();
+    rn.push_back(RNode{(uint32_t) N, 0, 0, 0, (uint32_t) bfs_to_id.size(), 0, 0, 0});   // the sentinel
+    if (((uint64_t) imgs.size() * 2 / BLOCK_USABLE + 64) * BLOCK_SLOTS >= ID_LIMIT) return rfail(BFQ_E_RANGE, "topic index too large");
+    EdgeTable table;
+    table.init(imgs.size());
+    for (const Slot& s : imgs) table.slots[table.place(s.w[W_PARENT], s.w[W_LEN], &s.w[W_TOK])] = s;
     SlotVec& slots = table.slots;
     // ---- upload
     RCUDA_TRY(cudaSetDevice(h->device));
     RCUDA_TRY(cudaStreamSynchronize(h->stream));
+    h->need_full = true;   // until the upload is complete
     RCUDA_TRY(h->d_nodes.reserve(rn.size()));
     RCUDA_TRY(h->d_slots.reserve(slots.size()));
     RCUDA_TRY(h->d_tags.reserve(table.tags.size()));
@@ -715,12 +862,130 @@ int32_t rebuild(bfq_rindex* h) {
         RCUDA_TRY(cudaMemcpy(h->d_bfs_to_id.p, bfs_to_id.data(), bfs_to_id.size() * 8, cudaMemcpyHostToDevice));
     }
     h->tenant_root.clear();
-    for (const auto& e : root_of) h->tenant_root[e.first] = (int32_t) nodes[e.second].bfs;
+    for (const auto& e : regions) h->tenant_root[e.first] = (int32_t) e.second.root;
+    h->last_rebuilt = (int64_t) regions.size();
+    h->regions = std::move(regions);
     h->n_blocks = table.n_blocks;
     h->n_nodes = (int64_t) N;
-    h->n_topics = (int64_t) dfs_to_id.size();
+    h->n_dfs = h->n_topics = (int64_t) dfs_to_id.size();
+    h->n_bfs = (int64_t) bfs_to_id.size();
+    h->next_virtual = (uint32_t) next_virtual;
     h->max_nodes_per_depth = max_depth_nodes;
+    h->garbage_nodes = 0;
+    h->used_slots = (int64_t) imgs.size();
+    h->overflowed_blocks = table.overflowed_blocks;
+    h->full_commits++;
+    h->dirty.clear();
+    h->need_full = false;
     h->have_snapshot = true;
+    return BFQ_OK;
+}
+
+// Bounds of the delta path: past them a commit is a full build.
+constexpr int64_t GARBAGE_SLACK = 4096;   // garbage nodes may exceed a quarter of the live nodes by this much
+constexpr int64_t OCCUPANCY_NUM = 3, OCCUPANCY_DEN = 4;   // occupied table slots, garbage included, <= 3/4 of the usable ones
+constexpr int32_t NEED_FULL = 1;
+
+// Delta commit: rebuild only the dirty tenants, each into a fresh region appended behind the existing ones, and insert their
+// edges into the live tag table on the device. Returns NEED_FULL (nothing changed) when the commit must be a full build.
+int32_t commit_delta(bfq_rindex* h) {
+    if (h->need_full || !h->have_snapshot) return NEED_FULL;
+    if (h->dirty.empty()) {   // nothing changed: no device work
+        h->last_rebuilt = 0;
+        return BFQ_OK;
+    }
+    std::vector<RNode> rn;
+    std::vector<int64_t> dfs_to_id, bfs_to_id;
+    std::vector<Slot> imgs;
+    std::vector<std::pair<std::string, TenantRegion>> fresh;   // rebuilt tenants and their new regions
+    std::vector<std::string> gone;                              // tenants whose topics were all removed
+    int64_t garbage = h->garbage_nodes, max_depth_nodes = h->max_nodes_per_depth, n_topics = h->n_topics;
+    uint64_t next_virtual = h->next_virtual;
+    const uint64_t node0 = (uint64_t) h->n_nodes, dfs0 = (uint64_t) h->n_dfs, bfs0 = (uint64_t) h->n_bfs;
+    for (const std::string& t : h->dirty) {
+        auto old = h->regions.find(t);
+        if (old != h->regions.end()) {
+            garbage += old->second.n_nodes;
+            n_topics -= old->second.n_topics;
+        }
+        const auto run = tenant_run(h->staged, h->staged.lower_bound({t, std::string()}));
+        if (run.first == run.second || run.first->first.first != t) {
+            if (old != h->regions.end()) gone.push_back(t);
+            continue;
+        }
+        const uint64_t nb = node0 + rn.size(), db = dfs0 + dfs_to_id.size(), bb = bfs0 + bfs_to_id.size();
+        if (nb + 1 >= ID_LIMIT || db >= ID_LIMIT || bb >= ID_LIMIT || next_virtual >= VIRT_LIMIT) return NEED_FULL;
+        TenantImage im;
+        if (build_tenant(run.first, run.second, (uint32_t) nb, (uint32_t) db, (uint32_t) bb, (uint32_t) next_virtual, &im) != BFQ_OK)
+            return NEED_FULL;
+        TenantRegion reg;
+        reg.root = (uint32_t) nb;
+        reg.n_nodes = (uint32_t) im.rn.size();
+        reg.n_topics = (int64_t) im.dfs_to_id.size();
+        fresh.emplace_back(t, reg);
+        n_topics += reg.n_topics;
+        append(rn, im.rn);
+        append(dfs_to_id, im.dfs_to_id);
+        append(bfs_to_id, im.bfs_to_id);
+        append(imgs, im.slots);
+        next_virtual += im.n_virtual;
+        max_depth_nodes = std::max(max_depth_nodes, im.max_depth_nodes);
+    }
+    const uint64_t n_nodes = node0 + rn.size(), n_dfs = dfs0 + dfs_to_id.size(), n_bfs = bfs0 + bfs_to_id.size();
+    if (n_nodes + 1 >= ID_LIMIT || n_dfs >= ID_LIMIT || n_bfs >= ID_LIMIT) return NEED_FULL;
+    if (garbage > ((int64_t) n_nodes - garbage) / 4 + GARBAGE_SLACK) return NEED_FULL;
+    const int64_t used = h->used_slots + (int64_t) imgs.size();
+    if (used * OCCUPANCY_DEN > (int64_t) h->n_blocks * BLOCK_USABLE * OCCUPANCY_NUM) return NEED_FULL;
+    // ---- device patch, on the handle's stream, finished before the handle lock is released
+    cudaStream_t st = h->stream;
+    RCUDA_TRY(cudaSetDevice(h->device));
+    h->need_full = true;   // until the patch is complete: a failed patch leaves the device arrays to the next full build
+    RCUDA_TRY(h->d_nodes.grow(n_nodes + 1, node0, st));   // the old sentinel is overwritten by the first appended root
+    RCUDA_TRY(h->d_dfs_to_id.grow(std::max<uint64_t>(n_dfs, 1), dfs0, st));
+    RCUDA_TRY(h->d_bfs_to_id.grow(std::max<uint64_t>(n_bfs, 1), bfs0, st));
+    rn.push_back(RNode{(uint32_t) n_nodes, 0, 0, 0, (uint32_t) n_bfs, 0, 0, 0});   // the new sentinel
+    RCUDA_TRY(cudaMemcpyAsync(h->d_nodes.p + node0, rn.data(), rn.size() * sizeof(RNode), cudaMemcpyHostToDevice, st));
+    if (!dfs_to_id.empty()) {
+        RCUDA_TRY(cudaMemcpyAsync(h->d_dfs_to_id.p + dfs0, dfs_to_id.data(), dfs_to_id.size() * 8, cudaMemcpyHostToDevice, st));
+        RCUDA_TRY(cudaMemcpyAsync(h->d_bfs_to_id.p + bfs0, bfs_to_id.data(), bfs_to_id.size() * 8, cudaMemcpyHostToDevice, st));
+    }
+    unsigned long long overflowed = 0;
+    if (!imgs.empty()) {
+        RCUDA_TRY(h->d_new_slots.reserve(imgs.size()));
+        RCUDA_TRY(h->d_ins_ctr.reserve(1));
+        RCUDA_TRY(cudaMemcpyAsync(h->d_new_slots.p, imgs.data(), imgs.size() * sizeof(Slot), cudaMemcpyHostToDevice, st));
+        RCUDA_TRY(cudaMemsetAsync(h->d_ins_ctr.p, 0, sizeof(unsigned long long), st));
+        const int64_t n = (int64_t) imgs.size();
+        rinsert_edges_kernel<<<(unsigned) ((n + 255) / 256), 256, 0, st>>>(h->d_new_slots.p, n, h->d_slots.p,
+                                                                           reinterpret_cast<uint32_t*>(h->d_tags.p), h->n_blocks,
+                                                                           h->d_ins_ctr.p);
+        h->launches++;
+        RCUDA_TRY(cudaGetLastError());
+        RCUDA_TRY(cudaMemcpyAsync(&overflowed, h->d_ins_ctr.p, sizeof(overflowed), cudaMemcpyDeviceToHost, st));
+    }
+    RCUDA_TRY(cudaStreamSynchronize(st));
+    // ---- publish
+    for (const std::string& t : gone) {
+        h->regions.erase(t);
+        h->tenant_root.erase(t);
+    }
+    for (const auto& f : fresh) {
+        h->regions[f.first] = f.second;
+        h->tenant_root[f.first] = (int32_t) f.second.root;
+    }
+    h->n_nodes = (int64_t) n_nodes;
+    h->n_dfs = (int64_t) n_dfs;
+    h->n_bfs = (int64_t) n_bfs;
+    h->n_topics = n_topics;
+    h->next_virtual = (uint32_t) next_virtual;
+    h->max_nodes_per_depth = max_depth_nodes;
+    h->garbage_nodes = garbage;
+    h->used_slots = used;
+    h->overflowed_blocks += (int64_t) overflowed;
+    h->last_rebuilt = (int64_t) fresh.size();
+    h->delta_commits++;
+    h->dirty.clear();
+    h->need_full = false;
     return BFQ_OK;
 }
 
@@ -753,6 +1018,8 @@ int32_t bfq_rindex_reset(bfq_rindex* h) {
     h->staged.clear();
     h->by_id = std::make_shared<IdTable>();   // the committed table stays with the snapshot and its results
     h->alive.clear();
+    h->dirty.clear();
+    h->need_full = true;
     return BFQ_OK;
 }
 
@@ -772,6 +1039,7 @@ int32_t bfq_rindex_add(bfq_rindex* h, const uint8_t* tenants, const int64_t* ten
             id = (int64_t) h->by_id->size();
             h->by_id->push_back(key);
             h->alive.push_back(1);
+            h->dirty.insert(key.first);
             h->staged.emplace(std::move(key), id);
         } else {
             id = it->second;
@@ -788,6 +1056,7 @@ int32_t bfq_rindex_add(bfq_rindex* h, const uint8_t* tenants, const int64_t* ten
 int32_t bfq_rindex_load_keys(bfq_rindex* h, const uint8_t* keys, const int64_t* key_off, int64_t n, int64_t* ids_out) {
     if (!h || n < 0 || (n > 0 && (!keys || !key_off))) return rfail(BFQ_E_INVALID, "bad argument");
     std::lock_guard<std::mutex> g(h->mu);
+    if (h->staged.empty()) h->need_full = true;   // a bulk load onto an empty handle: one full build beats a delta per tenant
     for (int64_t i = 0; i < n; i++) {
         sv tenant;
         std::string topic;
@@ -802,6 +1071,7 @@ int32_t bfq_rindex_load_keys(bfq_rindex* h, const uint8_t* keys, const int64_t* 
             id = (int64_t) h->by_id->size();
             h->by_id->push_back(key);
             h->alive.push_back(1);
+            h->dirty.insert(key.first);
             h->staged.emplace(std::move(key), id);
         } else {
             id = it->second;
@@ -839,6 +1109,7 @@ int32_t bfq_rindex_remove(bfq_rindex* h, const uint8_t* tenant, int64_t tn, cons
     auto it = h->staged.find({std::string((const char*) tenant, (size_t) tn), std::string((const char*) topic, (size_t) n)});
     if (it != h->staged.end()) {
         h->alive[(size_t) it->second] = 0;
+        h->dirty.insert(it->first.first);
         h->staged.erase(it);
     }
     return BFQ_OK;
@@ -847,9 +1118,20 @@ int32_t bfq_rindex_remove(bfq_rindex* h, const uint8_t* tenant, int64_t tn, cons
 int32_t bfq_rindex_commit(bfq_rindex* h) {
     if (!h) return rfail(BFQ_E_INVALID, "handle is NULL");
     std::lock_guard<std::mutex> g(h->mu);
-    const int32_t rc = rebuild(h);
+    int32_t rc = commit_delta(h);
+    if (rc == NEED_FULL) rc = rebuild_full(h);
     if (rc == BFQ_OK) h->committed = h->by_id;
     return rc;
+}
+
+int32_t bfq_rindex_stats(bfq_rindex* h, int64_t* stats, int32_t n) {
+    if (!h || (!stats && n > 0)) return rfail(BFQ_E_INVALID, "bad argument");
+    std::lock_guard<std::mutex> g(h->mu);
+    const int64_t v[11] = {h->n_topics, (int64_t) h->regions.size(), h->n_nodes, h->garbage_nodes, h->used_slots,
+                           (int64_t) h->n_blocks * BLOCK_USABLE, h->full_commits, h->delta_commits, h->last_rebuilt,
+                           h->device_bytes(), h->overflowed_blocks};
+    for (int32_t i = 0; i < n && i < 11; i++) stats[i] = v[i];
+    return BFQ_OK;
 }
 
 int32_t bfq_rindex_lookup(bfq_rindex* h, int64_t id, uint8_t* tenant_out, int64_t tenant_cap, int64_t* tenant_len,

@@ -89,6 +89,15 @@ class GpuTopicMatchIndex:
     def commit(self):
         N.check(N.lib.bfq_rindex_commit(self._h))
 
+    STAT_NAMES = ["topics", "tenants", "nodes", "garbage_nodes", "used_slots", "usable_slots", "full_commits", "delta_commits",
+                  "rebuilt_tenants", "device_bytes", "overflowed_blocks"]
+
+    def stats(self):
+        """bfq_rindex_stats of the committed snapshot, by name"""
+        s = np.zeros(len(self.STAT_NAMES), np.int64)
+        N.check(N.lib.bfq_rindex_stats(self._h, s.ctypes.data, len(s)))
+        return dict(zip(self.STAT_NAMES, s.tolist()))
+
     def lookup(self, topic_id):
         tl, pl = C.c_int64(0), C.c_int64(0)
         N.check(N.lib.bfq_rindex_lookup(self._h, int(topic_id), None, 0, C.byref(tl), None, 0, C.byref(pl)))

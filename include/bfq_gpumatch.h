@@ -338,7 +338,24 @@ int32_t bfq_rindex_add(bfq_rindex* h, const uint8_t* tenants, const int64_t* ten
  * alone. ids_out[i] = the topic's id, or -1 for bytes that are not a retain key (skipped). */
 int32_t bfq_rindex_load_keys(bfq_rindex* h, const uint8_t* keys, const int64_t* key_off, int64_t n, int64_t* ids_out);
 int32_t bfq_rindex_remove(bfq_rindex* h, const uint8_t* tenant, int64_t tn, const uint8_t* topic, int64_t n);
+/* Publishes the staged topics as the snapshot that bfq_rmatch reads. Each tenant's trie is one region of the device arrays.
+ * Delta path: a commit rebuilds only the tenants whose staged topic set changed since the last commit (an add of a new
+ * (tenant, topic) or a remove of a staged one; re-adding an existing topic changes nothing). Each rebuilt tenant gets a
+ * fresh region behind the existing ones, and its exact edges are inserted into the device hash table by a kernel. The
+ * region it replaces, and that of a tenant whose topics were all removed, stay behind as garbage. A commit with nothing
+ * changed does no device work. The commit is a full build instead (every tenant, fresh table, no garbage) when:
+ *   - there is no snapshot yet, or bfq_rindex_reset ran, or bfq_rindex_load_keys ran on an empty staging set;
+ *   - garbage nodes would exceed a quarter of the live nodes plus 4096;
+ *   - occupied table slots, garbage included, would exceed 3/4 of the usable slots;
+ *   - a node id, rank or long-name chunk id space would run out.
+ * Both paths give the same answers (ids and their order) as a fresh handle given the same add / remove history and
+ * committed once. The commit holds the handle lock and returns after the device is patched. */
 int32_t bfq_rindex_commit(bfq_rindex* h);
+/* stats[k], k < n, of the committed snapshot: 0 live topics, 1 live tenants, 2 node records (garbage included), 3 garbage
+ * nodes, 4 occupied hash-table slots (garbage included), 5 usable hash-table slots, 6 full commits so far, 7 delta commits
+ * so far (a commit with nothing changed counts as neither), 8 tenants whose region the last commit built (0 when nothing
+ * changed), 9 device bytes held by the handle, 10 hash-table blocks that overflowed into the next block */
+int32_t bfq_rindex_stats(bfq_rindex* h, int64_t* stats, int32_t n);
 /* topic id -> (tenant, topic) strings, resolved against the STAGED ids: after bfq_rindex_reset ids restart at 0, so an id of an
  * earlier result may name another topic here (bfq_rresult_retain_keys resolves against the result's own snapshot instead) */
 int32_t bfq_rindex_lookup(bfq_rindex* h, int64_t id, uint8_t* tenant_out, int64_t tenant_cap, int64_t* tenant_len,
