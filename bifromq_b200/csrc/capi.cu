@@ -258,8 +258,10 @@ struct bfq_index {
     bool dedup = true;                   // BFQ_DEDUP=0: match duplicates of a (tenant, topic) pair separately
     int32_t tier0_ctas_per_sm = 0;       // bfq_index_set_option("tier0_ctas_per_sm"): 0 = as many as fit
     int32_t dedup_hash_bits = 64;        // bfq_index_set_option("dedup_hash_bits"): test knob, < 64 forces de-dup hash collisions
+    bool fanout_global = false;          // bfq_index_set_option("fanout_global"): test knob, every fan-out takes the global pass
     double last_kernel_ms = 0;
     int64_t launches = 0, overflow_topics = 0, flagged_topics = 0, deferred_topics = 0, duplicate_topics = 0, buffer_retries = 0;
+    int64_t global_fanouts = 0;
     int64_t full_commits = 0, delta_commits = 0;
     // Releases the host image of a full build (2.3 GB of records at 10M filters: 0.4 s of page freeing) off the committing
     // thread. Touched under stage_mu only (commits are serialised); joined before the next one starts and at destroy.
@@ -1260,7 +1262,8 @@ int32_t bfq_index_set_option(bfq_index* h, const char* name, int64_t value) {
     else if (n == "dedup_hash_bits") {
         if (value < 0 || value > 64) return fail(BFQ_E_INVALID, "dedup_hash_bits must be in [0, 64]");
         h->dedup_hash_bits = (int32_t) value;
-    } else return fail(BFQ_E_INVALID, "unknown option: " + n);
+    } else if (n == "fanout_global") h->fanout_global = value != 0;
+    else return fail(BFQ_E_INVALID, "unknown option: " + n);
     return BFQ_OK;
 }
 
@@ -1276,12 +1279,12 @@ int32_t bfq_index_stats(bfq_index* h, int64_t* stats, int32_t n) {
     std::lock_guard<std::mutex> g(h->mu);
     static const FlatIndex empty;
     const FlatIndex& f = h->snap ? h->snap->flat : empty;
-    const int64_t v[17] = {f.n_routes, (int64_t) f.tenant_ordinal.size(), f.n_nodes, (int64_t) f.n_slots,
+    const int64_t v[18] = {f.n_routes, (int64_t) f.tenant_ordinal.size(), f.n_nodes, (int64_t) f.n_slots,
                            h->snap ? h->snap->device_bytes() : 0, f.max_nodes_per_depth, h->launches, h->overflow_topics,
                            h->flagged_topics, f.n_multi, f.n_cont_chunks, h->deferred_topics, h->duplicate_topics,
                            h->full_commits, h->delta_commits, h->snap ? (int64_t) h->snap->garbage_slots : 0,
-                           h->buffer_retries};
-    for (int32_t i = 0; i < n && i < 17; i++) stats[i] = v[i];
+                           h->buffer_retries, h->global_fanouts};
+    for (int32_t i = 0; i < n && i < 18; i++) stats[i] = v[i];
     return BFQ_OK;
 }
 
@@ -1938,7 +1941,8 @@ int32_t ensure_fan_table(bfq_index* h, Snapshot* s, std::shared_ptr<Snapshot::Fa
         std::lock_guard<std::mutex> gd(h->deliverers->mu);
         ft->n_deliverers = (uint32_t) h->deliverers->list.size() + 1;
     }
-    if (ft->n_deliverers > fanout_max_deliverers()) return fail(BFQ_E_RANGE, "more distinct (subBrokerId, delivererKey) pairs than the fan-out pass counts per tile");
+    // ids share rdeliv[] with FO_GROUP_BIT, and n_deliverers and the global pass's n_deliverers + 1 counts are int32
+    if (ft->n_deliverers > 0x7FFFFFFEu) return fail(BFQ_E_RANGE, "more than 2^31 - 3 distinct (subBrokerId, delivererKey) pairs on one handle");
     CUDA_TRY(ft->d_rdeliv.reserve(rdeliv.size()));
     CUDA_TRY(ft->d_gmem_off.reserve(gmem_off.size()));
     CUDA_TRY(ft->d_gmem_deliv.reserve(std::max<size_t>(gmem_deliv.size(), 1)));
@@ -1966,12 +1970,15 @@ int32_t bfq_fanout_device(const bfq_device_result* res, const int64_t* d_offsets
     int32_t rc = ensure_fan_table(h, L->snap.get(), &ft);
     if (rc != BFQ_OK) return rc;
     cudaStream_t st = (cudaStream_t) stream;
-    const int64_t tile = fanout_tile();
-    const size_t n_tiles = (size_t) std::max<int64_t>(1, (n_pairs + tile - 1) / tile);
-    const size_t cells = (size_t) ft->n_deliverers * n_tiles;
-    if (cells >= 0x7FFFFFF0ull) return fail(BFQ_E_RANGE, "fan-out count matrix too large (deliverers x tiles); split the batch");
-    CUDA_TRY(w->d_fo_counts.reserve(cells));
-    CUDA_TRY(w->d_fo_base.reserve(cells));
+    bool force_global;
+    {
+        std::lock_guard<std::mutex> g(h->mu);
+        force_global = h->fanout_global;
+    }
+    const bool tiled = !force_global && fanout_tiled(ft->n_deliverers, n_pairs);
+    const size_t words = fanout_scratch_words(ft->n_deliverers, n_pairs, tiled);
+    CUDA_TRY(w->d_fo_counts.reserve(words));
+    CUDA_TRY(w->d_fo_base.reserve(words));
     CUDA_TRY(w->d_pack_offsets.reserve((size_t) ft->n_deliverers + 1));
     CUDA_TRY(w->d_pack_topic.reserve((size_t) std::max<int64_t>(n_pairs, 1)));
     CUDA_TRY(w->d_pack_rank.reserve((size_t) std::max<int64_t>(n_pairs, 1)));
@@ -1986,16 +1993,16 @@ int32_t bfq_fanout_device(const bfq_device_result* res, const int64_t* d_offsets
     p.gmem_deliv = ft->d_gmem_deliv.p;
     p.gordered = ft->d_gordered.p;
     p.n_deliverers = ft->n_deliverers;
-    p.tile_counts = w->d_fo_counts.p;
-    p.tile_base = w->d_fo_base.p;
+    p.counts = w->d_fo_counts.p;
+    p.base = w->d_fo_base.p;
     p.pack_offsets = w->d_pack_offsets.p;
     p.pack_topic = w->d_pack_topic.p;
     p.pack_rank = w->d_pack_rank.p;
     p.pack_member = w->d_pack_member.p;
     size_t tmp_bytes = 0;
-    CUDA_TRY(launch_fanout(p, nullptr, &tmp_bytes, st));
+    CUDA_TRY(launch_fanout(p, tiled, nullptr, &tmp_bytes, st));
     CUDA_TRY(w->d_fo_tmp.reserve(tmp_bytes + 256));
-    CUDA_TRY(launch_fanout(p, w->d_fo_tmp.p, &tmp_bytes, st));
+    CUDA_TRY(launch_fanout(p, tiled, w->d_fo_tmp.p, &tmp_bytes, st));
     out->d_pack_offsets = (const int64_t*) w->d_pack_offsets.p;
     out->d_pack_topic = w->d_pack_topic.p;
     out->d_pack_rank = w->d_pack_rank.p;
@@ -2006,6 +2013,7 @@ int32_t bfq_fanout_device(const bfq_device_result* res, const int64_t* d_offsets
     out->generation = L->snap->generation;
     std::lock_guard<std::mutex> g(h->mu);
     h->launches += 5;
+    if (!tiled) h->global_fanouts++;
     return BFQ_OK;
 }
 

@@ -9,15 +9,21 @@
 //   input   the device CSR of a completed match (surviving ranks per topic, caps applied: bfq_expand_device)
 //   output  every (topic, route) pair of the batch grouped by DELIVERER id: pack_offsets[D + 1], pack_topic[], pack_rank[]
 //           (+ pack_member[] for shared subscriptions: the index of the member the pair was resolved to)
-// A deliverer id is a dense index over the distinct (subBrokerId, delivererKey) pairs of the index, interned on the host when a
-// snapshot is first used for fan-out (bfq_fanout_deliverer gives the pair back). Unordered shared subscriptions pick member
+// A deliverer id is a dense index over the distinct (subBrokerId, delivererKey) pairs the handle has interned since it was
+// created, interned on the host when a snapshot is first used for fan-out (bfq_fanout_deliverer gives the pair back); ids are
+// never freed, so a handle that has seen many deliverers carries them all. Unordered shared subscriptions pick member
 // hash(topic position, route rank) mod n — the reference picks uniformly at random (ThreadLocalRandom), so any member is a valid
 // outcome and the pick here is reproducible; ORDERED shared subscriptions need the publisher of each message
 // (RendezvousHash over ClientInfo.hashCode(), :253-270) which a topic batch does not carry: their pairs are grouped under the
 // reserved deliverer id BFQ_FANOUT_ORDERED_SHARE with every member left to the host.
 //
-// Kernels: a two-pass radix partition on the deliverer id. Pass 1 counts per (CTA tile, deliverer) in shared memory; a scan over
-// the [deliverer][tile] count matrix gives every tile its write cursor per deliverer; pass 2 re-reads the tile and scatters.
+// Kernels: a two-pass radix partition on the deliverer id, in one of two forms.
+//   tile pass    pass 1 counts per (CTA tile, deliverer) in shared memory; a scan over the [deliverer][tile] count matrix gives
+//                every tile its write cursor per deliverer; pass 2 re-reads the tile and scatters. Used while the matrix has
+//                no more cells than the batch has pairs (so at most FO_TILE ids: a 16 KB shared histogram).
+//   global pass  pass 1 counts per deliverer in global memory (warp-aggregated atomics), an exclusive scan over the D + 1
+//                counts gives every deliverer its segment, pass 2 re-reads the pairs and claims slots with the same atomics.
+//                Scratch is 2 x (D + 1) words whatever the batch; used for many deliverers or a small batch.
 // Per pair: one 8-byte rank read (streaming), one 4-byte deliverer-id read (the table is 4 bytes per route: L2 resident at
 // 10M filters), 12 bytes written. HBM-streaming bound.
 #include <cuda_runtime.h>
@@ -42,7 +48,6 @@ namespace {
 
 constexpr int FO_THREADS = 256;
 constexpr int FO_TILE = 4096;          // pairs per tile
-constexpr uint32_t FO_MAX_D = 8192;    // deliverer ids a tile counts in shared memory (32 KB); more -> BFQ_E_RANGE
 
 __device__ __forceinline__ uint32_t fo_mix(uint32_t a, uint32_t b) {
     uint32_t h = a * 0x9E3779B1u ^ (b + 0x7F4A7C15u + (a << 6) + (a >> 2));
@@ -77,10 +82,25 @@ __device__ __forceinline__ uint32_t fo_topic_of(const int64_t* offsets, int64_t 
     return (uint32_t) lo;
 }
 
+// global pass: the lanes of a warp that hold the same deliverer take consecutive slots of ctr[d] with one atomic (a batch whose
+// pairs all go to one deliverer costs one atomic per warp step, not one per pair); returns this lane's slot
+__device__ __forceinline__ uint32_t fo_claim(uint32_t* ctr, uint32_t d) {
+    const uint32_t peers = __match_any_sync(__activemask(), d);
+    const uint32_t lane = threadIdx.x & 31u;
+    const int leader = __ffs(peers) - 1;
+    uint32_t base = 0;
+    if ((int) lane == leader) base = atomicAdd(&ctr[d], (uint32_t) __popc(peers));
+    base = __shfl_sync(peers, base, leader);
+    return base + (uint32_t) __popc(peers & ((1u << lane) - 1u));
+}
+
+template <bool GLOBAL>
 __global__ void __launch_bounds__(FO_THREADS) fanout_count_kernel(const FanoutParams p) {
     extern __shared__ uint32_t hist[];
-    for (uint32_t i = threadIdx.x; i < p.n_deliverers; i += FO_THREADS) hist[i] = 0;
-    __syncthreads();
+    if constexpr (!GLOBAL) {
+        for (uint32_t i = threadIdx.x; i < p.n_deliverers; i += FO_THREADS) hist[i] = 0;
+        __syncthreads();
+    }
     // a thread owns FO_TILE / FO_THREADS consecutive pairs (one 128-byte line of ranks): one binary search for the first one's
     // topic, then the topic index only walks forward
     constexpr int PER = FO_TILE / FO_THREADS;
@@ -91,18 +111,25 @@ __global__ void __launch_bounds__(FO_THREADS) fanout_count_kernel(const FanoutPa
             const int64_t j = j0 + q;
             while (p.offsets[t + 1] <= j) t++;
             uint32_t member;
-            atomicAdd(&hist[fo_deliverer(p, t, p.ranks[j], &member)], 1u);
+            const uint32_t d = fo_deliverer(p, t, p.ranks[j], &member);
+            if constexpr (GLOBAL) fo_claim(p.counts, d);
+            else atomicAdd(&hist[d], 1u);
         }
     }
-    __syncthreads();
-    // count matrix in [deliverer][tile] order: its exclusive scan is, for every deliverer, the cursor of every tile
-    for (uint32_t i = threadIdx.x; i < p.n_deliverers; i += FO_THREADS) p.tile_counts[(uint64_t) i * gridDim.x + blockIdx.x] = hist[i];
+    if constexpr (!GLOBAL) {
+        __syncthreads();
+        // count matrix in [deliverer][tile] order: its exclusive scan is, for every deliverer, the cursor of every tile
+        for (uint32_t i = threadIdx.x; i < p.n_deliverers; i += FO_THREADS) p.counts[(uint64_t) i * gridDim.x + blockIdx.x] = hist[i];
+    }
 }
 
+template <bool GLOBAL>
 __global__ void __launch_bounds__(FO_THREADS) fanout_scatter_kernel(const FanoutParams p) {
     extern __shared__ uint32_t cur[];
-    for (uint32_t i = threadIdx.x; i < p.n_deliverers; i += FO_THREADS) cur[i] = 0;
-    __syncthreads();
+    if constexpr (!GLOBAL) {
+        for (uint32_t i = threadIdx.x; i < p.n_deliverers; i += FO_THREADS) cur[i] = 0;
+        __syncthreads();
+    }
     constexpr int PER = FO_TILE / FO_THREADS;
     const int64_t j0 = (int64_t) blockIdx.x * FO_TILE + (int64_t) threadIdx.x * PER;
     if (j0 < p.n_pairs) {
@@ -113,7 +140,9 @@ __global__ void __launch_bounds__(FO_THREADS) fanout_scatter_kernel(const Fanout
             uint32_t member;
             const int64_t r = p.ranks[j];
             const uint32_t d = fo_deliverer(p, t, r, &member);
-            const uint32_t at = p.tile_base[(uint64_t) d * gridDim.x + blockIdx.x] + atomicAdd(&cur[d], 1u);
+            uint32_t at;
+            if constexpr (GLOBAL) at = fo_claim(p.base, d);   // base[d] is deliverer d's write cursor
+            else at = p.base[(uint64_t) d * gridDim.x + blockIdx.x] + atomicAdd(&cur[d], 1u);
             p.pack_topic[at] = t;
             p.pack_rank[at] = (uint32_t) r;
             if (p.pack_member) p.pack_member[at] = member;
@@ -121,34 +150,53 @@ __global__ void __launch_bounds__(FO_THREADS) fanout_scatter_kernel(const Fanout
     }
 }
 
-// pack_offsets[d] = tile_base[d][0]; pack_offsets[D] = n_pairs
+// pack_offsets[d] = base[d][0] (the first tile's cursor of deliverer d); pack_offsets[D] = n_pairs
 __global__ void fanout_offsets_kernel(const FanoutParams p, uint32_t n_tiles) {
     const uint32_t d = blockIdx.x * blockDim.x + threadIdx.x;
-    if (d < p.n_deliverers) p.pack_offsets[d] = (long long) p.tile_base[(uint64_t) d * n_tiles];
+    if (d < p.n_deliverers) p.pack_offsets[d] = (long long) p.base[(uint64_t) d * n_tiles];
     if (d == p.n_deliverers) p.pack_offsets[d] = (long long) p.n_pairs;
 }
 
+uint32_t fo_tiles(int64_t n_pairs) { return (uint32_t) std::max<int64_t>(1, (n_pairs + FO_TILE - 1) / FO_TILE); }
+
 }  // namespace
 
-cudaError_t launch_fanout(const FanoutParams& p, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream) {
-    const uint32_t n_tiles = (uint32_t) std::max<int64_t>(1, (p.n_pairs + FO_TILE - 1) / FO_TILE);
-    const size_t cells = (size_t) p.n_deliverers * n_tiles;
-    if (!d_tmp) return cub::DeviceScan::ExclusiveSum(nullptr, *tmp_bytes, p.tile_counts, p.tile_base, (int) std::min<size_t>(cells, 0x7FFFFFFF), stream);
-    const size_t smem = (size_t) p.n_deliverers * sizeof(uint32_t);
-    if (smem > 48 * 1024) {
-        cudaFuncSetAttribute(fanout_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
-        cudaFuncSetAttribute(fanout_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
+// The tile pass while its [deliverer][tile] matrix has at most one cell per pair (FO_TILE cells for a batch of less than one
+// tile): its scratch stays at most 8 bytes per pair, and n_deliverers <= FO_TILE follows, so the histogram fits in 16 KB of
+// shared memory. Otherwise the global pass, whose scratch is 8 bytes per deliverer id.
+bool fanout_tiled(uint32_t n_deliverers, int64_t n_pairs) {
+    const uint64_t cells = (uint64_t) n_deliverers * fo_tiles(n_pairs);
+    return cells <= (uint64_t) std::min<int64_t>(std::max<int64_t>(n_pairs, FO_TILE), 0x7FFFFFFF);
+}
+
+size_t fanout_scratch_words(uint32_t n_deliverers, int64_t n_pairs, bool tiled) {
+    return tiled ? (size_t) n_deliverers * fo_tiles(n_pairs) : (size_t) n_deliverers + 1;
+}
+
+cudaError_t launch_fanout(const FanoutParams& p, bool tiled, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream) {
+    const uint32_t n_tiles = fo_tiles(p.n_pairs);
+    const int cells = (int) fanout_scratch_words(p.n_deliverers, p.n_pairs, tiled);
+    if (!d_tmp) return cub::DeviceScan::ExclusiveSum(nullptr, *tmp_bytes, p.counts, p.base, cells, stream);
+    if (!tiled) {
+        // counts[D] stays 0, so the exclusive scan's last entry is n_pairs
+        cudaError_t e = cudaMemsetAsync(p.counts, 0, (size_t) cells * sizeof(uint32_t), stream);
+        if (e != cudaSuccess) return e;
+        fanout_count_kernel<true><<<n_tiles, FO_THREADS, 0, stream>>>(p);
+        e = cub::DeviceScan::ExclusiveSum(d_tmp, *tmp_bytes, p.counts, p.base, cells, stream);
+        if (e != cudaSuccess) return e;
+        // offsets before the scatter: the scatter advances base[] as its cursors
+        fanout_offsets_kernel<<<(p.n_deliverers + 1 + 255) / 256, 256, 0, stream>>>(p, 1);
+        fanout_scatter_kernel<true><<<n_tiles, FO_THREADS, 0, stream>>>(p);
+        return cudaGetLastError();
     }
-    fanout_count_kernel<<<n_tiles, FO_THREADS, smem, stream>>>(p);
-    cudaError_t e = cub::DeviceScan::ExclusiveSum(d_tmp, *tmp_bytes, p.tile_counts, p.tile_base, (int) cells, stream);
+    const size_t smem = (size_t) p.n_deliverers * sizeof(uint32_t);   // <= 16 KB (fanout_tiled)
+    fanout_count_kernel<false><<<n_tiles, FO_THREADS, smem, stream>>>(p);
+    cudaError_t e = cub::DeviceScan::ExclusiveSum(d_tmp, *tmp_bytes, p.counts, p.base, cells, stream);
     if (e != cudaSuccess) return e;
-    fanout_scatter_kernel<<<n_tiles, FO_THREADS, smem, stream>>>(p);
+    fanout_scatter_kernel<false><<<n_tiles, FO_THREADS, smem, stream>>>(p);
     fanout_offsets_kernel<<<(p.n_deliverers + 1 + 255) / 256, 256, 0, stream>>>(p, n_tiles);
     return cudaGetLastError();
 }
-
-uint32_t fanout_max_deliverers() { return FO_MAX_D; }
-int64_t fanout_tile() { return FO_TILE; }
 
 // ------------------------------------------------------------------------------------------------ host: interning
 namespace {

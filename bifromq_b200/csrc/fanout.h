@@ -28,21 +28,24 @@ struct FanoutParams {
     const uint32_t* gmem_deliv;      // deliverer id of every member
     const uint8_t* gordered;         // [n_groups] 1 = $oshare (left to the host)
     uint32_t n_deliverers;           // ids are [0, n_deliverers); the last one is the reserved "ordered share" id
-    // scratch
-    uint32_t* tile_counts;           // [n_deliverers * n_tiles]
-    uint32_t* tile_base;             // [n_deliverers * n_tiles]
+    // scratch, fanout_scratch_words() each: the tile pass's [deliverer][tile] count matrix and its scan, or the global pass's
+    // D + 1 counts and their scan (the write cursors)
+    uint32_t* counts;
+    uint32_t* base;
     // outputs
     long long* pack_offsets;         // [n_deliverers + 1]
     uint32_t* pack_topic;            // [n_pairs]
     uint32_t* pack_rank;             // [n_pairs]
     uint32_t* pack_member;           // [n_pairs] member index of a shared subscription, 0xFFFFFFFF otherwise
 };
+// true: the shared-memory tile pass fits (few deliverers for the batch); false: the global pass. Both give the same grouping.
+bool fanout_tiled(uint32_t n_deliverers, int64_t n_pairs);
+size_t fanout_scratch_words(uint32_t n_deliverers, int64_t n_pairs, bool tiled);
 // d_tmp == nullptr: query the scan scratch size
-cudaError_t launch_fanout(const FanoutParams& p, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream);
-uint32_t fanout_max_deliverers();
-int64_t fanout_tile();
+cudaError_t launch_fanout(const FanoutParams& p, bool tiled, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream);
 
-// (subBrokerId, delivererKey) -> dense id, append-only and shared by every snapshot of an index (ids stay valid across commits)
+// (subBrokerId, delivererKey) -> dense id, append-only and shared by every snapshot of an index (ids stay valid across commits
+// and resets, and are never freed)
 struct DelivererTable {
     std::mutex mu;
     std::unordered_map<std::string, uint32_t> ids;

@@ -177,11 +177,11 @@ class GpuRouteIndex:
         N.check(N.lib.bfq_index_commit(self._h))
 
     def stats(self):
-        s = np.zeros(17, np.int64)
-        N.check(N.lib.bfq_index_stats(self._h, s.ctypes.data, 17))
+        s = np.zeros(18, np.int64)
+        N.check(N.lib.bfq_index_stats(self._h, s.ctypes.data, 18))
         names = ["routes", "tenants", "nodes", "slots", "device_bytes", "max_nodes_per_depth", "launches",
                  "overflow_topics", "flagged_topics", "multi_segment_filters", "long_token_chunks", "deferred_topics",
-                 "duplicate_topics", "full_commits", "delta_commits", "garbage_slots", "buffer_retries"]
+                 "duplicate_topics", "full_commits", "delta_commits", "garbage_slots", "buffer_retries", "global_fanouts"]
         return dict(zip(names, s.tolist()))
 
     def deliverer(self, deliverer_id):

@@ -91,7 +91,9 @@ int32_t bfq_index_generation(bfq_index* h, uint64_t* generation);   /* 0 before 
  *   "dedup"              0: match repeated (tenant, topic) pairs separately;
  *   "dedup_hash_bits"    test knob, 0..64 (default 64): keep only the low k bits of the de-dup hash, so that distinct topics
  *                        share table slots and 32-bit tags on purpose and only the byte-for-byte compare tells them apart.
- *                        Answers stay exact at any k; small k only makes the de-dup pass slower. */
+ *                        Answers stay exact at any k; small k only makes the de-dup pass slower;
+ *   "fanout_global"      test knob, 0/1 (default 0): 1 makes every bfq_fanout_device take the global-count pass that large
+ *                        deliverer counts use, so it can be checked on small cases. The grouping is the same either way. */
 int32_t bfq_index_set_option(bfq_index* h, const char* name, int64_t value);
 
 /* stats[k], k < n: 0 routes, 1 tenants, 2 trie nodes, 3 hash-table slots, 4 device bytes, 5 max nodes per
@@ -99,7 +101,8 @@ int32_t bfq_index_set_option(bfq_index* h, const char* name, int64_t value);
  * 9 multi-segment filters, 10 long-token chunks, 11 topics handed from the lane-per-topic tier to the
  * warp-per-topic tier so far, 12 duplicate (tenant, topic) pairs answered from their first occurrence so far,
  * 13 full commits, 14 delta commits, 15 garbage slots of the current snapshot, 16 match calls that found a range or
- * throttle buffer too small, grew it and re-ran the batch so far */
+ * throttle buffer too small, grew it and re-ran the batch so far, 17 bfq_fanout_device calls that took the global-count
+ * pass (rather than the shared-memory tile pass) so far */
 int32_t bfq_index_stats(bfq_index* h, int64_t* stats, int32_t n);
 /* device time of the tier-0 (lane-per-topic) match kernel of the latest completed match call on this handle, measured with
  * CUDA events recorded on the launching stream around the launch (for roofline accounting) */
@@ -245,8 +248,18 @@ int32_t bfq_range_lookup(int32_t device_ordinal, const uint8_t* tenants, const i
  * pair, d_pack_member the member index a $share subscription was resolved to (0xFFFFFFFF for ordinary routes; members in the
  * order of the stored RouteGroup). An unordered share picks member hash(topic position, rank) mod n (the reference picks
  * uniformly at random: any member is valid); ORDERED shares need each message's publisher (rendezvous hash of ClientInfo) and
- * are grouped, unresolved, under the last id (ordered_share_id) for the host. Ids are dense over the distinct
- * (subBrokerId, delivererKey) pairs of the index, stable across commits; bfq_fanout_deliverer gives the pair back.
+ * are grouped, unresolved, under the last id (ordered_share_id) for the host; a shared subscription whose stored RouteGroup
+ * has no member is parked there too (member 0xFFFFFFFF). Order inside a deliverer's pairs is unspecified.
+ * Deliverer ids: every (subBrokerId, delivererKey) pair the handle has interned since it was created, in first-seen order.
+ * An id is never reused and never freed: it stays valid across commits, resets and reloads, and routes that were removed
+ * keep their ids. So a handle with much deliverer churn carries every id it has seen, and each call writes
+ * d_pack_offsets over all of them (8 bytes per id). Scratch: the tile pass (chosen while ids x 4096-pair tiles is at most
+ * max(n_pairs, 4096), so for at most 4096 ids) needs 8 bytes per (id, tile) cell, at most 8 bytes per pair; the global pass
+ * (every other case) needs 8 bytes per id. bfq_fanout_deliverer gives an
+ * id's pair back. The ordered-share id is the number of ids interned when the result's snapshot was first fanned out:
+ * always use the result's ordered_share_id; bfq_fanout_deliverer may resolve that number to a deliverer interned later.
+ * Limits: fewer than 2^32 (topic, route) pairs per call (BFQ_E_RANGE; split the batch), route ranks below 2^32, and at most
+ * 2^31 - 3 ids per handle (BFQ_E_RANGE). A receiver url without a subBrokerId or delivererKey makes the call fail with BFQ_E_INVALID.
  * The arrays live in the result's leased workspace: valid until bfq_device_result_release.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct {
