@@ -921,23 +921,22 @@ int32_t commit_full(bfq_index* h) {
         }
         if (i != flat.tenants.size()) return fail(BFQ_E_STATE, "internal error: staged tenants and built tenants disagree");
     }
-    // the host keeps only what it needs after the upload; the rest is handed to the janitor thread
+    // the host keeps only what it needs after the upload (the tag bytes too, about 2 B per wide edge: delta commits place
+    // rebuilt tenants' wide edges into a copy of them); the rest is handed to the janitor thread
     {
         struct Garbage {
             SlotVec slots;
-            std::vector<uint8_t> tags, rkind;
+            std::vector<uint8_t> rkind;
             std::vector<Slot> roots;
             std::vector<uint32_t> pfxP, pfxG;
         };
         auto* g = new Garbage();
         g->slots = std::move(flat.slots);
-        g->tags = std::move(flat.tags);
         g->rkind = std::move(flat.rkind);
         g->roots = std::move(flat.roots);
         g->pfxP = std::move(flat.pfx_persistent);
         g->pfxG = std::move(flat.pfx_group);
         flat.slots = SlotVec();
-        flat.tags = std::vector<uint8_t>();
         flat.rkind = std::vector<uint8_t>();
         flat.roots = std::vector<Slot>();
         flat.pfx_persistent = std::vector<uint32_t>();
@@ -974,7 +973,21 @@ void shift_seg_slice(std::vector<uint32_t>& segs, uint64_t base, uint64_t words,
 //   * ranks stay dense positions in KV order, so the tenants behind a tenant that grew or shrank have the ranks in their
 //     records moved by the difference (one streaming kernel over their regions) and their per-rank arrays copied to the
 //     shifted position.
-// The kernels see exactly the layout a full build would have produced, up to the placement of the regions.
+// The shared tag table (the children of wide nodes) is patched in place of being rebuilt. A tag-table slot IS the child's
+// record and its id is the child's node id, which its own children carry as their parent key; so a tenant's wide edges are
+// placed on the host, into a copy of the snapshot's tag bytes, while the tenant is built (its records are emitted knowing
+// every node id). In this order:
+//   1. the tag slots of every replaced or removed tenant are freed (EdgeTable::release): a rebuilt tenant keeps its ordinal,
+//      so its root-level edges come back with the same keys, and a stale entry must not be found before the new one;
+//   2. the rebuilt tenants are placed (build_tenant_image, the full build's EdgeTable::claim probe order);
+//   3. on the device, their tag-table records are scattered to their slots;
+//   4. the records of the untouched tenants whose ranks moved are shifted: their regions, and their listed tag slots;
+//   5. the new tag bytes are uploaded and the snapshot is published.
+// The tag table cannot grow without a full build (home_block depends on n_blocks), and freed slots leave their blocks'
+// overflow bytes set (only a full build clears them); so the commit is a full build instead when, after it,
+//   * more than 3/4 of the table's usable slots would be claimed, or
+//   * more than 1/4 of its blocks would have their overflow byte set (longer probes for every lookup that lands there).
+// The kernels see exactly the layout a full build would have produced, up to the placement of the regions and tag slots.
 int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const std::vector<std::string>& dirty) {
     const FlatIndex& of = old->flat;
     const bool trace = getenv("BFQ_COMMIT_TRACE") != nullptr;
@@ -985,7 +998,6 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
         fprintf(stderr, "[bfq delta commit] %-34s %9.3f ms\n", what, std::chrono::duration<double, std::milli>(now - t_prev).count());
         t_prev = now;
     };
-    if (of.n_big_edges > 0) return BFQ_NEED_FULL;   // the shared tag table cannot be patched per tenant
     if (old->garbage_slots > (uint64_t) of.n_slots / 4 + 4096) return BFQ_NEED_FULL;   // reclaim the replaced regions
     // ---- merge the touched tenants' KV (copy-on-write: the old blobs stay with the old snapshot)
     for (auto& p : dirty) h->staging.merge_tenant(p);
@@ -1011,6 +1023,21 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
     }
     if (plans.empty()) return BFQ_OK;   // nothing changed
     lap("merge touched tenants' KV");
+    // ---- the tag table: a copy of the snapshot's tag bytes (the snapshot's own stay as they are if this commit fails), with
+    // the slots of the replaced and removed tenants freed
+    EdgeTable table;
+    table.tags = of.tags;
+    table.n_blocks = of.n_blocks;
+    table.overflowed_blocks = of.overflowed_blocks;
+    uint64_t tag_live = of.n_big_edges;
+    const uint64_t tag_max = (uint64_t) of.n_blocks * BLOCK_USABLE * 3 / 4;
+    if (table.tags.size() != (size_t) of.n_blocks * 16) return BFQ_NEED_FULL;
+    for (auto& pl : plans) {
+        if (pl.old_index < 0) continue;
+        const TenantMeta& om = of.tenants[(size_t) pl.old_index];
+        for (uint32_t s : om.tag_slots) table.release(s);
+        tag_live -= om.big_edges;
+    }
     // ---- the new tenant list in key order: old tenants (untouched or replaced) merged with the new ones
     struct Entry {
         int old_index;   // -1: new tenant
@@ -1043,8 +1070,6 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
     nf.host_roots = of.host_roots;
     nf.segs = of.segs;
     nf.n_blocks = of.n_blocks;
-    nf.n_big_edges = 0;
-    nf.overflowed_blocks = of.overflowed_blocks;
     nf.max_nodes_per_depth = of.max_nodes_per_depth;
     nf.max_tenant_nodes = of.max_tenant_nodes;
     for (int k = 0; k < 5; k++) nf.child_hist[k] = of.child_hist[k];
@@ -1083,8 +1108,11 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
             nf.host_roots.emplace_back();
             nf.tenant_ordinal[id] = ordinal;
         }
-        if (!build_tenant_image(*pl.kv, sv(id), ordinal, rank, slot_cursor, seg_cursor, ppb, pgb, &pl.img, &err)) return fail(BFQ_E_INVALID, err);
-        if (pl.img.meta.big_edges > 0) return BFQ_NEED_FULL;
+        const uint64_t tag_room = tag_max > tag_live ? tag_max - tag_live : 0;
+        if (!build_tenant_image(*pl.kv, sv(id), ordinal, rank, slot_cursor, seg_cursor, ppb, pgb, &table, tag_room, &pl.img, &err))
+            return fail(BFQ_E_INVALID, err);
+        if (!pl.img.placed) return BFQ_NEED_FULL;   // its wide edges would fill the tag table past 3/4
+        tag_live += pl.img.meta.big_edges;
         slot_cursor += pl.img.meta.csr_slots;
         seg_cursor += pl.img.meta.seg_words;
         rank += pl.img.meta.n_routes;
@@ -1103,6 +1131,10 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
     for (auto& pl : plans)
         if (!pl.kv) nf.tenant_ordinal.erase(pl.prefix.substr(3));   // its root record stays behind, unreachable
     if (slot_cursor >= 0x7FFFFFF0ull || rank >= (int64_t) 0x7FFFFFFF) return BFQ_NEED_FULL;
+    if ((uint64_t) table.overflowed_blocks * 4 > (uint64_t) table.n_blocks) return BFQ_NEED_FULL;   // probes got too long
+    nf.tags = std::move(table.tags);
+    nf.n_big_edges = tag_live;
+    nf.overflowed_blocks = table.overflowed_blocks;
     nf.n_routes = rank;
     nf.n_slots = (uint32_t) slot_cursor;
     nf.n_nodes = 0;
@@ -1127,7 +1159,7 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
     } guard{st};
     const size_t n_new = (size_t) rank, n_old = (size_t) of.n_routes;
     CUDA_TRY(sn->d_slots.reserve((size_t) slot_cursor));
-    CUDA_TRY(sn->d_tags.reserve(std::max<size_t>(old->d_tags.cap, 1)));
+    CUDA_TRY(sn->d_tags.reserve(std::max<size_t>(nf.tags.size(), 1)));
     CUDA_TRY(sn->d_roots.reserve(std::max<size_t>(nf.host_roots.size(), 1)));
     CUDA_TRY(sn->d_segs.reserve(std::max<size_t>(nf.segs.size(), 2)));
     CUDA_TRY(sn->d_rkind.reserve(std::max<size_t>(n_new, 1)));
@@ -1135,14 +1167,21 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
     CUDA_TRY(sn->d_pfxG.reserve(n_new + 1));
     lap("device allocations");
     CUDA_TRY(cudaMemcpyAsync(sn->d_slots.p, old->d_slots.p, (size_t) of.n_slots * sizeof(Slot), cudaMemcpyDeviceToDevice, st));
-    if (old->d_tags.cap) CUDA_TRY(cudaMemcpyAsync(sn->d_tags.p, old->d_tags.p, old->d_tags.cap, cudaMemcpyDeviceToDevice, st));
-    // untouched tenants: slot regions whose ranks move, and the pieces of the per-rank arrays
+    // the whole tag array (16 B per block, ~2 B per wide edge): one small upload
+    if (!nf.tags.empty()) CUDA_TRY(cudaMemcpyAsync(sn->d_tags.p, nf.tags.data(), nf.tags.size(), cudaMemcpyHostToDevice, st));
+    // untouched tenants: slot regions and tag slots whose ranks move, and the pieces of the per-rank arrays; rebuilt tenants:
+    // their tag-table records
     std::vector<RankShiftRegion> regions;
+    std::vector<RankShiftSlot> shift_slots;
+    std::vector<uint32_t> scatter_ids;
+    std::vector<Slot> scatter_recs;
     for (size_t i = 0; i < nf.tenants.size(); i++) {
         const Entry& e = entries[i];
         const TenantMeta& m = nf.tenants[i];
         if (e.plan >= 0) {
             const TenantImage& img = plans[(size_t) e.plan].img;
+            scatter_ids.insert(scatter_ids.end(), m.tag_slots.begin(), m.tag_slots.end());
+            scatter_recs.insert(scatter_recs.end(), img.tag_recs.begin(), img.tag_recs.end());
             if (m.csr_slots) CUDA_TRY(cudaMemcpyAsync(sn->d_slots.p + m.region_base, img.slots.data(), (size_t) m.csr_slots * sizeof(Slot), cudaMemcpyHostToDevice, st));
             if (m.n_routes) {
                 CUDA_TRY(cudaMemcpyAsync(sn->d_rkind.p + m.lo, img.rkind.data(), (size_t) m.n_routes, cudaMemcpyHostToDevice, st));
@@ -1155,6 +1194,7 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
         const int64_t d = m.lo - om.lo;
         if (d != 0) {
             if (m.csr_slots) regions.push_back(RankShiftRegion{m.region_base, m.csr_slots, (int32_t) d});
+            for (uint32_t s : m.tag_slots) shift_slots.push_back(RankShiftSlot{s, (int32_t) d});
             Slot& r = nf.host_roots[m.ordinal];
             if (r.w[W_OWN_COUNT] > 0 && !(r.w[W_META] & FLAG_OWN_MULTI)) r.w[W_OWN_FIRST] = (uint32_t) ((int64_t) r.w[W_OWN_FIRST] + d);
             if (r.w[W_HASH_COUNT] > 0 && !(r.w[W_META] & FLAG_HASH_MULTI)) r.w[W_HASH_FIRST] = (uint32_t) ((int64_t) r.w[W_HASH_FIRST] + d);
@@ -1194,6 +1234,18 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
         CUDA_TRY(cudaStreamSynchronize(st));   // `tail` is on the stack
     }
     (void) n_old;
+    if (!scatter_ids.empty()) {
+        DevBuf<uint32_t> d_ids;
+        DevBuf<Slot> d_recs;
+        CUDA_TRY(d_ids.reserve(scatter_ids.size()));
+        CUDA_TRY(d_recs.reserve(scatter_recs.size()));
+        CUDA_TRY(cudaMemcpyAsync(d_ids.p, scatter_ids.data(), scatter_ids.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(d_recs.p, scatter_recs.data(), scatter_recs.size() * sizeof(Slot), cudaMemcpyHostToDevice, st));
+        launch_scatter_records(sn->d_slots.p, d_ids.p, d_recs.p, (int64_t) scatter_ids.size(), st);
+        CUDA_TRY(cudaStreamSynchronize(st));
+        d_ids.release();
+        d_recs.release();
+    }
     if (!regions.empty()) {
         DevBuf<RankShiftRegion> d_regions;
         CUDA_TRY(d_regions.reserve(regions.size()));
@@ -1202,12 +1254,20 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
         CUDA_TRY(cudaStreamSynchronize(st));
         d_regions.release();
     }
+    if (!shift_slots.empty()) {
+        DevBuf<RankShiftSlot> d_list;
+        CUDA_TRY(d_list.reserve(shift_slots.size()));
+        CUDA_TRY(cudaMemcpyAsync(d_list.p, shift_slots.data(), shift_slots.size() * sizeof(RankShiftSlot), cudaMemcpyHostToDevice, st));
+        launch_rank_shift_listed(sn->d_slots.p, d_list.p, (int64_t) shift_slots.size(), st);
+        CUDA_TRY(cudaStreamSynchronize(st));
+        d_list.release();
+    }
     CUDA_TRY(cudaMemcpyAsync(sn->d_roots.p, nf.host_roots.data(), nf.host_roots.size() * sizeof(Slot), cudaMemcpyHostToDevice, st));
     if (!nf.segs.empty()) CUDA_TRY(cudaMemcpyAsync(sn->d_segs.p, nf.segs.data(), nf.segs.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     CUDA_TRY(cudaGetLastError());
     lap("device copy + patch + rank shift");
-    sn->l2_window_bytes = 0;
+    set_l2_window(h, sn.get());
     publish(h, std::move(sn));
     lap("publish (drops the old snapshot)");
     return BFQ_OK;
@@ -1279,12 +1339,13 @@ int32_t bfq_index_stats(bfq_index* h, int64_t* stats, int32_t n) {
     std::lock_guard<std::mutex> g(h->mu);
     static const FlatIndex empty;
     const FlatIndex& f = h->snap ? h->snap->flat : empty;
-    const int64_t v[18] = {f.n_routes, (int64_t) f.tenant_ordinal.size(), f.n_nodes, (int64_t) f.n_slots,
+    const int64_t v[21] = {f.n_routes, (int64_t) f.tenant_ordinal.size(), f.n_nodes, (int64_t) f.n_slots,
                            h->snap ? h->snap->device_bytes() : 0, f.max_nodes_per_depth, h->launches, h->overflow_topics,
                            h->flagged_topics, f.n_multi, f.n_cont_chunks, h->deferred_topics, h->duplicate_topics,
                            h->full_commits, h->delta_commits, h->snap ? (int64_t) h->snap->garbage_slots : 0,
-                           h->buffer_retries, h->global_fanouts};
-    for (int32_t i = 0; i < n && i < 18; i++) stats[i] = v[i];
+                           h->buffer_retries, h->global_fanouts,
+                           h->snap ? (int64_t) f.n_blocks * BLOCK_USABLE : 0, (int64_t) f.n_big_edges, f.overflowed_blocks};
+    for (int32_t i = 0; i < n && i < 21; i++) stats[i] = v[i];
     return BFQ_OK;
 }
 
@@ -1368,6 +1429,65 @@ int32_t bfq_host_build_stats(const uint8_t* keys, const int64_t* key_off, const 
             ti++;
         }
     }
+    // The lookup rules of the kernels, on the host: is the node record `sl` at slot s found again from its parent's record
+    // `pr`? (nullptr = yes, else what is wrong). Wide nodes' children through the tag table `t`, the rest through the CSR rules.
+    auto lookup_error = [](const Slot& sl, uint32_t s, const Slot& pr, const EdgeTable& t) -> const char* {
+        if (sl.w[W_LEN] == LEN_PLUS) return pr.w[W_PLUS] == s ? nullptr : "'+' child is not linked from its parent";
+        const uint32_t meta = pr.w[W_META];
+        if (!(meta & FLAG_HAS_EXACT)) return "parent of an exact child lacks HAS_EXACT";
+        uint32_t found;
+        if (meta & FLAG_BIG) {
+            found = t.find(sl.w[W_PARENT], sl.w[W_LEN], &sl.w[W_TOK]);
+        } else {
+            const uint32_t lg = meta_log2size(meta), sd = meta >> 16, t32 = fold32(token_hash(sl.w[W_LEN], &sl.w[W_TOK]));
+            if (lg == 0 && (t32 & 0xFFFFu) != sd) return "single-child fingerprint mismatch";
+            found = pr.w[W_CHILD_BASE] + (lg ? child_index(t32, sd, lg) : 0u);
+        }
+        return found == s ? nullptr : "child lookup does not find a placed node";
+    };
+    // stats[19]: tenants with wide edges whose delta rebuild, simulated here, is found again node for node by those rules.
+    // The simulation is what bfq_index_commit's delta path does to the tenant: its tag slots are freed in a copy of the
+    // image's tag table, it is rebuilt into a fresh region behind the image and its wide edges are placed into that table
+    // (with the same key for its root-level edges: it keeps its ordinal), then its new tag-table records are written.
+    int64_t wide_rebuilds_found = 0;
+    if (n_stats > 19) {
+        const size_t tag_region = (size_t) flat.n_blocks * BLOCK_SLOTS;
+        size_t ti = 0;
+        for (auto& kvp : st.tenants()) {
+            if (ti >= flat.tenants.size()) break;
+            const TenantMeta& m = flat.tenants[ti++];
+            if (m.big_edges == 0) continue;
+            EdgeTable sim;
+            sim.n_blocks = flat.n_blocks;
+            sim.tags = flat.tags;
+            sim.overflowed_blocks = flat.overflowed_blocks;
+            sim.slots.assign(flat.slots.begin(), flat.slots.begin() + (ptrdiff_t) tag_region);
+            for (uint32_t s : m.tag_slots) sim.release(s);
+            const uint64_t base = flat.n_slots;
+            TenantImage img;
+            if (!build_tenant_image(*kvp.second.base, sv(m.tenant), m.ordinal, m.lo, base, flat.segs.size(), m.pp_base, m.pg_base, &sim,
+                                    ~0ull, &img, &err))
+                return fail(BFQ_E_INVALID, err);
+            if (!img.placed || img.meta.tag_slots.size() != m.big_edges) continue;
+            for (size_t k = 0; k < img.tag_recs.size(); k++) sim.slots[img.meta.tag_slots[k]] = img.tag_recs[k];
+            auto record_of = [&](uint32_t id) -> const Slot* {
+                if (id >= ROOT_BASE) return id == ROOT_BASE + m.ordinal ? &img.root : nullptr;
+                if (id < tag_region) return &sim.slots[id];
+                return id >= base && id - base < img.slots.size() ? &img.slots[id - base] : nullptr;
+            };
+            int64_t found = 0;
+            bool ok = true;
+            auto check = [&](uint32_t s, const Slot& sl) {
+                const Slot* pr = record_of(sl.w[W_PARENT]);
+                ok = ok && pr && lookup_error(sl, s, *pr, sim) == nullptr;
+                found++;
+            };
+            for (size_t i = 0; i < img.slots.size(); i++)
+                if (img.slots[i].w[W_PARENT] != EMPTY_PARENT) check((uint32_t) (base + i), img.slots[i]);
+            for (uint32_t s : img.meta.tag_slots) check(s, sim.slots[s]);
+            if (ok && found + 1 == img.meta.tenant_nodes) wide_rebuilds_found++;
+        }
+    }
     // self-check: every placed node is found again from its parent's record the way the kernels look it up
     {
         EdgeTable t;
@@ -1381,21 +1501,7 @@ int32_t bfq_host_build_stats(const uint8_t* keys, const int64_t* key_off, const 
             used++;
             const uint32_t pid = sl.w[W_PARENT];
             const Slot& pr = pid >= ROOT_BASE ? flat.roots[pid - ROOT_BASE] : t.slots[pid];
-            if (sl.w[W_LEN] == LEN_PLUS) {
-                if (pr.w[W_PLUS] != s) return fail(BFQ_E_STATE, "'+' child is not linked from its parent");
-                continue;
-            }
-            const uint32_t meta = pr.w[W_META];
-            if (!(meta & FLAG_HAS_EXACT)) return fail(BFQ_E_STATE, "parent of an exact child lacks HAS_EXACT");
-            uint32_t found;
-            if (meta & FLAG_BIG) {
-                found = t.find(pid, sl.w[W_LEN], &sl.w[W_TOK]);
-            } else {
-                const uint32_t lg = meta_log2size(meta), sd = meta >> 16, t32 = fold32(token_hash(sl.w[W_LEN], &sl.w[W_TOK]));
-                if (lg == 0 && (t32 & 0xFFFFu) != sd) return fail(BFQ_E_STATE, "single-child fingerprint mismatch");
-                found = pr.w[W_CHILD_BASE] + (lg ? child_index(t32, sd, lg) : 0u);
-            }
-            if (found != s) return fail(BFQ_E_STATE, "child lookup does not find a placed node");
+            if (const char* e = lookup_error(sl, s, pr, t)) return fail(BFQ_E_STATE, e);
         }
         if (used + (int64_t) flat.roots.size() != flat.n_nodes) return fail(BFQ_E_STATE, "node count mismatch");
     }
@@ -1409,6 +1515,7 @@ int32_t bfq_host_build_stats(const uint8_t* keys, const int64_t* key_off, const 
     if (n_stats > 16) stats[16] = (int64_t) image_sum;
     if (n_stats > 17) stats[17] = same_as_concat;
     if (n_stats > 18) stats[18] = tenant_images_equal;
+    if (n_stats > 19) stats[19] = wide_rebuilds_found;
     return BFQ_OK;
 }
 

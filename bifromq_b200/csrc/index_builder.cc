@@ -371,6 +371,8 @@ struct TenantBuild {
     Slot* root_rec = nullptr;
     uint32_t* segs = nullptr;     // word w of the segment table lives at segs[w - seg_origin]
     uint64_t seg_origin = 0;
+    std::vector<uint32_t> tag_slots;        // phase D: the tag-table slots its wide nodes' children claimed, in placement order
+    std::vector<Slot>* tag_recs = nullptr;  // delta build: the records of those children go here (tag_slots order), not to `slots`
 };
 
 // phase B, first half: decode the tenant's keys and build its trie. Returns false if the sorted-order construction met a level
@@ -764,8 +766,11 @@ inline uint32_t sat8(uint32_t v) { return v > 255u ? 255u : v; }
 void place_tenant(TenantBuild& tb, EdgeTable& table) {
     Builder& b = tb.b;
     const size_t N = b.nodes.size();
-    std::vector<uint32_t> id_of(N, NONE), child_base(N, 0), order;
+    std::vector<uint32_t> id_of(N, NONE), child_base(N, 0), order, tag_pos;
     order.reserve(N);
+    tb.tag_slots.clear();
+    tb.tag_slots.reserve((size_t) tb.big_edges);
+    if (tb.tag_recs) tag_pos.assign(N, NONE);   // node -> its index in tag_slots / tag_recs
     id_of[0] = ROOT_BASE + tb.ordinal;
     order.push_back(0);
     uint64_t cursor = tb.region_base;
@@ -782,7 +787,10 @@ void place_tenant(TenantBuild& tb, EdgeTable& table) {
         if (pl.big) {
             for (uint32_t j = c0; j < c1; j++) {
                 const BNode& ch = b.nodes[tb.child_list[j]];
-                id_of[tb.child_list[j]] = table.place(id_of[pi], ch.lenw, ch.tok);
+                const uint32_t s = table.claim(id_of[pi], ch.lenw, ch.tok);   // the record (key included) is emitted below
+                id_of[tb.child_list[j]] = s;
+                if (tb.tag_recs) tag_pos[tb.child_list[j]] = (uint32_t) tb.tag_slots.size();
+                tb.tag_slots.push_back(s);
                 order.push_back(tb.child_list[j]);
             }
         } else {
@@ -796,10 +804,11 @@ void place_tenant(TenantBuild& tb, EdgeTable& table) {
             cursor += 1ull << pl.lg;
         }
     }
-    if (order.size() != N || cursor != tb.region_base + tb.csr_slots) {
+    if (order.size() != N || cursor != tb.region_base + tb.csr_slots || tb.tag_slots.size() != tb.big_edges) {
         tb.err = "internal error: BFS placement did not cover the trie";
         return;
     }
+    if (tb.tag_recs) tb.tag_recs->assign(tb.tag_slots.size(), Slot());
     // segment-table offsets of the multi-segment targets, in node order (a sequential pass over the few that exist), so that
     // the records themselves can be written by several threads
     std::vector<uint64_t> seg_at(b.multi_lists.size(), 0);
@@ -843,7 +852,7 @@ void place_tenant(TenantBuild& tb, EdgeTable& table) {
             memset(rec->w, 0, sizeof(rec->w));
             rec->w[W_PARENT] = NONE;
         } else {
-            rec = &tb.slots[id_of[i] - tb.slot_origin];
+            rec = !tag_pos.empty() && tag_pos[i] != NONE ? &(*tb.tag_recs)[tag_pos[i]] : &tb.slots[id_of[i] - tb.slot_origin];
             rec->w[W_PARENT] = id_of[nd.parent];
             rec->w[W_LEN] = nd.lenw;
             for (uint32_t k = 0; k < TOKEN_WORDS; k++) rec->w[W_TOK + k] = nd.tok[k];
@@ -1131,6 +1140,7 @@ bool build_from_tenants(std::vector<TenantBuild>& tenants, int64_t n, FlatIndex*
         m.n_multi = tb.n_multi;
         m.n_cont = tb.b.n_cont;
         m.big_edges = tb.big_edges;
+        m.tag_slots = std::move(tb.tag_slots);
         out->tenants.push_back(std::move(m));
     }
     out->n_big_edges = n_big_edges;
@@ -1155,7 +1165,7 @@ bool build_from_tenants(std::vector<TenantBuild>& tenants, int64_t n, FlatIndex*
 }  // namespace
 
 bool build_tenant_image(const KVBlob& tkv, sv tenant, uint32_t ordinal, int64_t rank_lo, uint64_t region_base, uint64_t seg_base,
-                        uint32_t pp_base, uint32_t pg_base, TenantImage* out, std::string* err) {
+                        uint32_t pp_base, uint32_t pg_base, EdgeTable* tags, uint64_t tag_room, TenantImage* out, std::string* err) {
     *out = TenantImage();
     const int64_t n = tkv.n();
     TenantBuild tb;
@@ -1194,7 +1204,7 @@ bool build_tenant_image(const KVBlob& tkv, sv tenant, uint32_t ordinal, int64_t 
     m.walk_nodes = tb.tenant_nodes;
     m.n_cont = tb.b.n_cont;
     m.big_edges = tb.big_edges;
-    if (tb.big_edges > 0) return true;   // needs the shared tag table: the caller falls back to a full rebuild
+    if (tb.big_edges > 0 && (!tags || tb.big_edges > tag_room)) return true;   // not placed: the caller decides
     tb.region_base = region_base;
     tb.seg_base = seg_base;
     tb.pp_base = pp_base;
@@ -1222,8 +1232,9 @@ bool build_tenant_image(const KVBlob& tkv, sv tenant, uint32_t ordinal, int64_t 
     tb.root_rec = &out->root;
     tb.segs = out->segs.data();
     tb.seg_origin = seg_base;
+    tb.tag_recs = &out->tag_recs;
     EdgeTable unused;
-    place_tenant(tb, unused);
+    place_tenant(tb, tags ? *tags : unused);
     if (!tb.err.empty()) {
         if (err) *err = tb.err;
         return false;
@@ -1231,6 +1242,8 @@ bool build_tenant_image(const KVBlob& tkv, sv tenant, uint32_t ordinal, int64_t 
     out->pfxP[(size_t) n] = pp_base + tb.pp;
     out->pfxG[(size_t) n] = pg_base + tb.pg;
     m.n_multi = tb.n_multi;
+    m.tag_slots = std::move(tb.tag_slots);
+    out->placed = true;
     return true;
 }
 

@@ -40,25 +40,38 @@ struct TenantMeta {
     uint32_t pp = 0, pg = 0;               // persistent / group routes
     uint32_t pp_base = 0, pg_base = 0;     // value of the prefix-count arrays at its first rank
     int64_t tenant_nodes = 0, max_depth_nodes = 0, walk_nodes = 0, n_multi = 0, n_cont = 0;
-    uint64_t big_edges = 0;                // edges in the shared tag table (such a tenant is only rebuilt with the whole index)
+    uint64_t big_edges = 0;                // edges in the shared tag table (children of its wide nodes)
+    std::vector<uint32_t> tag_slots;       // their slot ids, in placement order (big_edges of them): what a delta commit frees
+                                           //   when it replaces or removes the tenant, and rank-shifts when the tenant moves
 };
 
 // One tenant built on its own (bfq_index_commit's delta path): records carry absolute slot ids / ranks for the given bases.
 struct TenantImage {
     TenantMeta meta;
+    bool placed = false;                   // false: built (meta is valid) but not placed, see build_tenant_image
     SlotVec slots;                         // csr_slots records, slot region_base + i at [i]
+    std::vector<Slot> tag_recs;            // records of the nodes placed in the tag table, slot meta.tag_slots[i] at [i]
     Slot root;
     std::vector<uint32_t> segs;            // seg_words
     std::vector<uint8_t> rkind;            // n
     std::vector<uint32_t> pfxP, pfxG;      // n + 1, already offset by the given bases
 };
+// Builds one tenant and places it at the given bases. The children of its wide nodes claim slots in `tags` (the live tag table
+// of the index, whose slot array stays on the device: only the tag bytes are touched) exactly as the full build's placement
+// does; their records come back in tag_recs instead of the region buffer. A tenant with wide edges is left unplaced
+// (placed = false, nothing claimed) when `tags` is null or when it has more than `tag_room` of them.
 bool build_tenant_image(const KVBlob& tenant_kv, sv tenant, uint32_t ordinal, int64_t rank_lo, uint64_t region_base, uint64_t seg_base,
-                        uint32_t pp_base, uint32_t pg_base, TenantImage* out, std::string* err);
+                        uint32_t pp_base, uint32_t pg_base, EdgeTable* tags, uint64_t tag_room, TenantImage* out, std::string* err);
+// the same without a tag table: a tenant with wide edges is built but not placed
+inline bool build_tenant_image(const KVBlob& tenant_kv, sv tenant, uint32_t ordinal, int64_t rank_lo, uint64_t region_base, uint64_t seg_base,
+                               uint32_t pp_base, uint32_t pg_base, TenantImage* out, std::string* err) {
+    return build_tenant_image(tenant_kv, tenant, ordinal, rank_lo, region_base, seg_base, pp_base, pg_base, nullptr, 0, out, err);
+}
 
 // Everything the device needs, in host memory, plus build statistics.
 struct FlatIndex {
     SlotVec slots;                            // blocked hash table (n_blocks * BLOCK_SLOTS)
-    std::vector<uint8_t> tags;                // 16 tag bytes per block
+    std::vector<uint8_t> tags;                // 16 tag bytes per block (kept on the host: delta commits place into a copy)
     std::vector<Slot> roots;                  // one record per tenant (key words unused)
     std::vector<uint32_t> segs;               // segment table (pairs), see trie_layout.h
     std::vector<uint8_t> rkind;               // per rank RouteKind
@@ -67,7 +80,7 @@ struct FlatIndex {
     std::unordered_map<std::string, uint32_t> tenant_ordinal;
     std::vector<TenantMeta> tenants;          // in key order
     std::vector<Slot> host_roots;             // kept on the host (roots is dropped after the upload)
-    uint64_t n_big_edges = 0;
+    uint64_t n_big_edges = 0;                 // claimed tag-table slots (the tenants' big_edges summed)
     int64_t n_routes = 0, n_nodes = 0, max_nodes_per_depth = 0, max_tenant_nodes = 0, n_multi = 0, n_cont_chunks = 0;
     uint32_t n_slots = 0, n_blocks = 0;
     int64_t overflowed_blocks = 0;

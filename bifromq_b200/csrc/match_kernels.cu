@@ -1019,19 +1019,37 @@ __global__ void __launch_bounds__(CAPS_THREADS) expand_flagged_kernel(const Expa
 }  // namespace
 
 namespace {
+// moves the ranks of one node record by d: its own / '#' first-rank words, unless the slot is free, the target is empty, or
+// the word indexes the segment table (a MULTI target; its ranks are shifted on the host)
+__device__ __forceinline__ void shift_record_ranks(uint32_t* w, uint32_t d) {
+    if (w[W_PARENT] == EMPTY_PARENT) return;
+    const uint32_t meta = w[W_META];
+    if (w[W_OWN_COUNT] > 0 && !(meta & FLAG_OWN_MULTI)) w[W_OWN_FIRST] += d;
+    if (w[W_HASH_COUNT] > 0 && !(meta & FLAG_HASH_MULTI)) w[W_HASH_FIRST] += d;
+}
 __global__ void __launch_bounds__(256) rank_shift_kernel(Slot* slots, const RankShiftRegion* regions, int n_regions) {
     // a CTA takes a region at a time; regions differ in size by orders of magnitude, so big ones are cut into pieces of 8192
     // slots that all CTAs pick up (piece index = blockIdx, striding)
     for (int r = 0; r < n_regions; r++) {
         const RankShiftRegion rg = regions[r];
         const uint32_t d = (uint32_t) rg.delta;
-        for (uint64_t s = (uint64_t) blockIdx.x * blockDim.x + threadIdx.x; s < rg.len; s += (uint64_t) gridDim.x * blockDim.x) {
-            uint32_t* w = slots[rg.base + s].w;
-            if (w[W_PARENT] == EMPTY_PARENT) continue;
-            const uint32_t meta = w[W_META];
-            if (w[W_OWN_COUNT] > 0 && !(meta & FLAG_OWN_MULTI)) w[W_OWN_FIRST] += d;
-            if (w[W_HASH_COUNT] > 0 && !(meta & FLAG_HASH_MULTI)) w[W_HASH_FIRST] += d;
-        }
+        for (uint64_t s = (uint64_t) blockIdx.x * blockDim.x + threadIdx.x; s < rg.len; s += (uint64_t) gridDim.x * blockDim.x)
+            shift_record_ranks(slots[rg.base + s].w, d);
+    }
+}
+// the tag-table records of the tenants whose ranks moved: one thread per listed slot (they are scattered over the table)
+__global__ void __launch_bounds__(256) rank_shift_listed_kernel(Slot* slots, const RankShiftSlot* list, int64_t n) {
+    for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x) {
+        const RankShiftSlot e = list[i];
+        shift_record_ranks(slots[e.slot].w, (uint32_t) e.delta);
+    }
+}
+// rebuilt tenants' tag-table records to their slots: 16 threads per record, one word each (coalesced 64-byte stores)
+__global__ void __launch_bounds__(256) scatter_records_kernel(Slot* slots, const uint32_t* ids, const Slot* recs, int64_t n) {
+    for (int64_t t = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; t < n * 16; t += (int64_t) gridDim.x * blockDim.x) {
+        const int64_t i = t >> 4;
+        const uint32_t k = (uint32_t) t & 15u;
+        slots[ids[i]].w[k] = recs[i].w[k];
     }
 }
 __global__ void __launch_bounds__(256) copy_add_kernel(uint32_t* dst, const uint32_t* src, int64_t n, uint32_t add) {
@@ -1053,6 +1071,14 @@ int device_sm_count() {
 void launch_rank_shift(Slot* slots, const RankShiftRegion* d_regions, int n_regions, cudaStream_t stream) {
     if (n_regions <= 0) return;
     rank_shift_kernel<<<device_sm_count() * 8, 256, 0, stream>>>(slots, d_regions, n_regions);
+}
+void launch_rank_shift_listed(Slot* slots, const RankShiftSlot* d_list, int64_t n, cudaStream_t stream) {
+    if (n <= 0) return;
+    rank_shift_listed_kernel<<<(unsigned) std::min<int64_t>((n + 255) / 256, (int64_t) device_sm_count() * 16), 256, 0, stream>>>(slots, d_list, n);
+}
+void launch_scatter_records(Slot* slots, const uint32_t* d_ids, const Slot* d_recs, int64_t n, cudaStream_t stream) {
+    if (n <= 0) return;
+    scatter_records_kernel<<<(unsigned) std::min<int64_t>((n * 16 + 255) / 256, (int64_t) device_sm_count() * 16), 256, 0, stream>>>(slots, d_ids, d_recs, n);
 }
 void launch_copy_add(uint32_t* dst, const uint32_t* src, int64_t n, uint32_t add, cudaStream_t stream) {
     if (n <= 0) return;

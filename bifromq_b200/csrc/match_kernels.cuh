@@ -200,6 +200,14 @@ struct RankShiftRegion {
     int32_t delta;
 };
 void launch_rank_shift(Slot* slots, const RankShiftRegion* d_regions, int n_regions, cudaStream_t stream);
+// the same rule for single slots: the tag-table records (children of wide nodes) of those tenants
+struct RankShiftSlot {
+    uint32_t slot;
+    int32_t delta;
+};
+void launch_rank_shift_listed(Slot* slots, const RankShiftSlot* d_list, int64_t n, cudaStream_t stream);
+// slots[ids[i]] = recs[i]: the tag-table records of the tenants a delta commit rebuilt
+void launch_scatter_records(Slot* slots, const uint32_t* d_ids, const Slot* d_recs, int64_t n, cudaStream_t stream);
 // dst[i] = src[i] + add (the prefix-count arrays of those tenants, copied to their shifted position)
 void launch_copy_add(uint32_t* dst, const uint32_t* src, int64_t n, uint32_t add, cudaStream_t stream);
 

@@ -154,8 +154,9 @@ struct EdgeTable {
         slots.resize((size_t) n_blocks * BLOCK_SLOTS);
         fill_empty_slots(slots.data(), slots.size());
     }
-    // claims a slot for the edge key and returns its index (the caller fills the payload)
-    uint32_t place(uint32_t parent, uint32_t lenw, const uint32_t* tok) {
+    // claims a tag for the edge key and returns its slot index; only the tag array is touched (the caller writes the whole
+    // record). The table must have a free usable slot somewhere, or this never returns.
+    uint32_t claim(uint32_t parent, uint32_t lenw, const uint32_t* tok) {
         const uint64_t h = edge_hash(token_hash(lenw, tok), parent);
         uint32_t b = home_block(h, n_blocks);
         const uint8_t fp = (uint8_t) fingerprint(h);
@@ -164,19 +165,34 @@ struct EdgeTable {
             for (uint32_t j = 0; j < BLOCK_USABLE; j++) {
                 uint8_t expected = 0;   // claim a free tag atomically: tenants are placed by concurrent threads
                 if (__atomic_load_n(&tg[j], __ATOMIC_RELAXED) == 0 &&
-                    __atomic_compare_exchange_n(&tg[j], &expected, fp, false, __ATOMIC_ACQ_REL, __ATOMIC_RELAXED)) {
-                    const uint32_t s = b * BLOCK_SLOTS + j;
-                    slots[s].w[W_PARENT] = parent;
-                    slots[s].w[W_LEN] = lenw;
-                    for (uint32_t k = 0; k < TOKEN_WORDS; k++) slots[s].w[W_TOK + k] = tok[k];
-                    return s;
-                }
+                    __atomic_compare_exchange_n(&tg[j], &expected, fp, false, __ATOMIC_ACQ_REL, __ATOMIC_RELAXED))
+                    return b * BLOCK_SLOTS + j;
             }
             if (__atomic_exchange_n(&tg[TAG_CTRL], (uint8_t) 1, __ATOMIC_ACQ_REL) == 0)
                 __atomic_fetch_add(&overflowed_blocks, (int64_t) 1, __ATOMIC_RELAXED);
             b = b + 1 == n_blocks ? 0 : b + 1;
         }
     }
+    // claims a slot for the edge key and writes the key words (the caller fills the payload)
+    uint32_t place(uint32_t parent, uint32_t lenw, const uint32_t* tok) {
+        const uint32_t s = claim(parent, lenw, tok);
+        slots[s].w[W_PARENT] = parent;
+        slots[s].w[W_LEN] = lenw;
+        for (uint32_t k = 0; k < TOKEN_WORDS; k++) slots[s].w[W_TOK + k] = tok[k];
+        return s;
+    }
+    // Frees a claimed slot (a forward delta commit frees the slots of the tenants it replaces or removes, BEFORE it places
+    // their new edges). Only the fingerprint byte is cleared; the record behind it stays as it was, and lookups stay exact:
+    //   * the control byte of the slot's block is never cleared, so a key that was placed past this block (because the block
+    //     was full when it was placed) is still reached: the probe still walks on from here;
+    //   * a free tag (0) is never taken for a candidate. Fingerprints are 2..255. The device compares a block's tags four
+    //     bytes at a time (match_bytes in hash_probe.cuh: (y - 0x01010101) & ~y & 0x80808080 with y = tags ^ fp), which
+    //     flags a byte whose y is 0 (a true match) and, through the borrow of a true match below it, a byte whose y is 1.
+    //     For a free tag y = fp >= 2: neither. The host lookup (find) compares bytes exactly;
+    //   * so the stale record behind a freed slot is never loaded, even when a rebuilt tenant re-places the very same key (a
+    //     root-level edge keeps its key: the tenant keeps its ordinal) into another slot of the probe sequence.
+    // A later claim may reuse the slot; the caller then overwrites the whole record.
+    void release(uint32_t slot) { tags[slot] = 0; }
     // host-side lookup (self-check only): slot index or NONE
     uint32_t find(uint32_t parent, uint32_t lenw, const uint32_t* tok) const {
         const uint64_t h = edge_hash(token_hash(lenw, tok), parent);

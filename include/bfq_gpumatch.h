@@ -80,7 +80,20 @@ int32_t bfq_index_apply(bfq_index* h, const uint8_t* add_keys, const int64_t* ad
  * continue on the previous snapshot; the swap is atomic with respect to matches (they always see a whole snapshot).
  * Every snapshot has a generation (1, 2, ...); results report the generation they were produced from. The previous
  * snapshot is freed when the last match / result that pins it is gone. bfq_index_apply is all-or-nothing: an
- * undecodable key leaves the staging area untouched. */
+ * undecodable key leaves the staging area untouched.
+ * Delta path: a commit whose staged changes touch at most 64 tenants rebuilds only those tenants, whatever their shape.
+ * Each gets a fresh slot region behind the existing ones (the one it replaces stays behind as garbage); the children of its
+ * wide nodes (too many children for a private perfect-hash array, about a thousand) go into the shared tag table: its old
+ * tag slots are freed first, then its new edges are placed into the free ones. The rest of the snapshot is copied on the
+ * device and the ranks of the tenants behind a grown or shrunk tenant are moved. The commit is a full build instead when:
+ *   - there is no snapshot yet, or bfq_index_reset / bfq_index_load ran since the last commit, or more than 64 tenants changed;
+ *   - garbage slots would exceed a quarter of the slots plus 4096;
+ *   - claimed tag-table slots would exceed 3/4 of its usable slots (the table only grows with a full build);
+ *   - tag-table blocks with their overflow byte set would exceed a quarter of the blocks (freed slots do not clear it, so
+ *     churn lengthens probes until a full build resets them);
+ *   - a slot id or rank would run out of 31 bits.
+ * Both paths give the same answers as a handle fully built from the same KV. bfq_index_stats reports the path taken
+ * (13, 14) and the tag table's fill (18..20). */
 int32_t bfq_index_commit(bfq_index* h);
 int32_t bfq_index_generation(bfq_index* h, uint64_t* generation);   /* 0 before the first commit */
 /* Tuning knobs (defaults are the measured best for a handle that has the GPU to itself):
@@ -102,7 +115,8 @@ int32_t bfq_index_set_option(bfq_index* h, const char* name, int64_t value);
  * warp-per-topic tier so far, 12 duplicate (tenant, topic) pairs answered from their first occurrence so far,
  * 13 full commits, 14 delta commits, 15 garbage slots of the current snapshot, 16 match calls that found a range or
  * throttle buffer too small, grew it and re-ran the batch so far, 17 bfq_fanout_device calls that took the global-count
- * pass (rather than the shared-memory tile pass) so far */
+ * pass (rather than the shared-memory tile pass) so far, 18 usable tag-table slots (15 per block), 19 claimed tag-table
+ * slots (children of wide nodes), 20 tag-table blocks whose overflow byte is set (all three of the current snapshot) */
 int32_t bfq_index_stats(bfq_index* h, int64_t* stats, int32_t n);
 /* device time of the tier-0 (lane-per-topic) match kernel of the latest completed match call on this handle, measured with
  * CUDA events recorded on the launching stream around the launch (for roofline accounting) */
@@ -113,7 +127,9 @@ int32_t bfq_index_last_kernel_ms(bfq_index* h, double* ms);
  * multi-segment filters, long-token chunks, 8 = tag-table blocks that overflowed, 9..13 = nodes with 0/1/2/3/>=4
  * exact children, 14 = staging microseconds, 15 = flatten microseconds, 16 = a checksum of the whole image the build would
  * upload, 17 = 1 if building from one concatenated KV blob gives that same image, 18 = tenants whose stand-alone image (what a delta
- * commit builds for a touched tenant) equals their part of the full image (used by CPU tests and to time the build). */
+ * commit builds for a touched tenant) equals their part of the full image, 19 = tenants with wide edges whose delta rebuild,
+ * simulated on the image (their tag slots freed, the tenant rebuilt into a fresh region and its wide edges placed again), is
+ * found again node for node by the kernels' lookup rules (used by CPU tests and to time the build). */
 int32_t bfq_host_build_stats(const uint8_t* keys, const int64_t* key_off, const uint8_t* vals, const int64_t* val_off,
                              int64_t n, int64_t* stats, int32_t n_stats);
 
