@@ -263,6 +263,7 @@ struct bfq_index {
     int64_t launches = 0, overflow_topics = 0, flagged_topics = 0, deferred_topics = 0, duplicate_topics = 0, buffer_retries = 0;
     int64_t global_fanouts = 0;
     int64_t full_commits = 0, delta_commits = 0;
+    int64_t rebuilt_tenants = 0;         // tenants the last commit built (bfq_index_stats slot 21)
     // Releases the host image of a full build (2.3 GB of records at 10M filters: 0.4 s of page freeing) off the committing
     // thread. Touched under stage_mu only (commits are serialised); joined before the next one starts and at destroy.
     std::thread janitor;
@@ -965,21 +966,29 @@ void shift_seg_slice(std::vector<uint32_t>& segs, uint64_t base, uint64_t words,
     }
 }
 
-// The delta path (SURVEY.md 8f rank 1; DW/DistWorkerCoProc.java:304-513 applies one SUB / UNSUB at a time): only the touched
-// tenants are merged, rebuilt and uploaded. The new snapshot is a device-side copy of the previous one (a few milliseconds
-// for gigabytes at HBM speed; the previous snapshot stays untouched for the matches and results that pin it) in which
+// The delta path (SURVEY.md 8f rank 1; DW/DistWorkerCoProc.java:304-513 applies one batch of SUBs / UNSUBs, of any number of
+// tenants, per mutation): only the touched tenants are merged, rebuilt and uploaded. The new snapshot is a device-side copy of
+// the previous one (a few milliseconds for gigabytes at HBM speed; the previous snapshot stays untouched for the matches and
+// results that pin it) in which
 //   * every rebuilt tenant gets a fresh slot region appended behind the existing ones (its old region becomes garbage until
 //     the next full build) and a patched root record;
 //   * ranks stay dense positions in KV order, so the tenants behind a tenant that grew or shrank have the ranks in their
 //     records moved by the difference (one streaming kernel over their regions) and their per-rank arrays copied to the
 //     shifted position.
+// The host work runs on all cores, so k touched tenants cost about what the largest of them costs plus k times a small
+// fixed amount: the tenants are merged in parallel, built in parallel (build_tenant_image: trie, plans, sizes; largest
+// first), given their bases in key order by prefix sums, and placed (place_tenant_image) in parallel into one staging
+// buffer. The device work is a fixed number of copies and launches whatever k is: one upload of the rebuilt regions (they
+// sit back to back at [old n_slots, new n_slots)), one upload of their per-rank arrays packed with a run table, and one
+// kernel that assembles the new per-rank arrays from the old ones and the packed ones (assemble_rank_arrays_kernel).
 // The shared tag table (the children of wide nodes) is patched in place of being rebuilt. A tag-table slot IS the child's
 // record and its id is the child's node id, which its own children carry as their parent key; so a tenant's wide edges are
-// placed on the host, into a copy of the snapshot's tag bytes, while the tenant is built (its records are emitted knowing
-// every node id). In this order:
+// placed on the host, into a copy of the snapshot's tag bytes, while the tenant's records are emitted (knowing every node
+// id). In this order:
 //   1. the tag slots of every replaced or removed tenant are freed (EdgeTable::release): a rebuilt tenant keeps its ordinal,
 //      so its root-level edges come back with the same keys, and a stale entry must not be found before the new one;
-//   2. the rebuilt tenants are placed (build_tenant_image, the full build's EdgeTable::claim probe order);
+//   2. the rebuilt tenants with wide edges are placed one after another in key order (the full build's EdgeTable::claim
+//      probe order); tenants without wide edges touch no shared state and are placed in parallel before them;
 //   3. on the device, their tag-table records are scattered to their slots;
 //   4. the records of the untouched tenants whose ranks moved are shifted: their regions, and their listed tag slots;
 //   5. the new tag bytes are uploaded and the snapshot is published.
@@ -988,7 +997,8 @@ void shift_seg_slice(std::vector<uint32_t>& segs, uint64_t base, uint64_t words,
 //   * more than 3/4 of the table's usable slots would be claimed, or
 //   * more than 1/4 of its blocks would have their overflow byte set (longer probes for every lookup that lands there).
 // The kernels see exactly the layout a full build would have produced, up to the placement of the regions and tag slots.
-int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const std::vector<std::string>& dirty) {
+// *built is set to the number of tenants rebuilt.
+int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const std::vector<std::string>& dirty, int64_t* built) {
     const FlatIndex& of = old->flat;
     const bool trace = getenv("BFQ_COMMIT_TRACE") != nullptr;
     auto t_prev = std::chrono::steady_clock::now();
@@ -1000,11 +1010,13 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
     };
     if (old->garbage_slots > (uint64_t) of.n_slots / 4 + 4096) return BFQ_NEED_FULL;   // reclaim the replaced regions
     // ---- merge the touched tenants' KV (copy-on-write: the old blobs stay with the old snapshot)
-    for (auto& p : dirty) h->staging.merge_tenant(p);
+    h->staging.merge_tenants(dirty);
     struct Plan {
         std::string prefix;            // key prefix
         int old_index = -1;            // position in of.tenants, or -1 for a new tenant
         std::shared_ptr<const KVBlob> kv;   // null: the tenant is gone
+        uint32_t ordinal = 0;
+        int64_t pack_lo = 0;           // its first rank in the packed upload of the rebuilt tenants' per-rank arrays
         TenantImage img;
     };
     std::vector<Plan> plans;
@@ -1022,6 +1034,7 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
         plans.push_back(std::move(pl));
     }
     if (plans.empty()) return BFQ_OK;   // nothing changed
+    for (auto& pl : plans) *built += pl.kv ? 1 : 0;
     lap("merge touched tenants' KV");
     // ---- the tag table: a copy of the snapshot's tag bytes (the snapshot's own stay as they are if this commit fails), with
     // the slots of the replaced and removed tenants freed
@@ -1062,7 +1075,6 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
             entries.push_back({(int) i, pk});
         }
     }
-    // ---- bases: dense ranks, appended slot regions / segment slices, running prefix-count bases
     auto sn = std::make_shared<Snapshot>();
     sn->device = h->device;
     FlatIndex& nf = sn->flat;
@@ -1073,21 +1085,69 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
     nf.max_nodes_per_depth = of.max_nodes_per_depth;
     nf.max_tenant_nodes = of.max_tenant_nodes;
     for (int k = 0; k < 5; k++) nf.child_hist[k] = of.child_hist[k];
-    uint64_t slot_cursor = of.n_slots, seg_cursor = of.segs.size();
-    int64_t rank = 0;
-    uint32_t ppb = 0, pgb = 0;
-    std::string err;
-    nf.tenants.reserve(entries.size());
-    sn->th.reserve(entries.size());
-    // the old snapshot's per-tenant fan-out tables may be filled in by a concurrent bfq_fanout_device: copy them under its lock
-    std::vector<Snapshot::TenantHost> old_th;
+    // ---- ordinals and ranks (a tenant's ranks depend only on the sizes of the tenants before it), then the build step of
+    // every rebuilt tenant on all host cores, largest first
+    std::vector<uint32_t> by_size;
     {
-        std::lock_guard<std::mutex> gf(old->fan_mu);
-        old_th = old->th;
+        int64_t rank = 0;
+        for (auto& e : entries) {
+            if (e.plan < 0) {
+                rank += of.tenants[(size_t) e.old_index].n_routes;
+                continue;
+            }
+            Plan& pl = plans[(size_t) e.plan];
+            if (pl.old_index >= 0) {
+                pl.ordinal = of.tenants[(size_t) pl.old_index].ordinal;
+            } else {
+                pl.ordinal = (uint32_t) nf.host_roots.size();
+                nf.host_roots.emplace_back();
+                nf.tenant_ordinal[pl.prefix.substr(3)] = pl.ordinal;
+            }
+            pl.img.meta.lo = rank;
+            rank += pl.kv->n();
+            by_size.push_back((uint32_t) e.plan);
+        }
+        if (rank >= (int64_t) 0x7FFFFFFF) return BFQ_NEED_FULL;
     }
+    std::sort(by_size.begin(), by_size.end(), [&](uint32_t a, uint32_t b) { return plans[a].kv->n() > plans[b].kv->n(); });
+    std::vector<std::string> errs(plans.size());
+    parallel_for_each(by_size, [&](uint32_t k) {
+        Plan& pl = plans[k];
+        const std::string id = pl.prefix.substr(3);
+        build_tenant_image(*pl.kv, sv(id), pl.ordinal, pl.img.meta.lo, &pl.img, &errs[k]);
+    });
+    for (auto& e : errs)
+        if (!e.empty()) return fail(BFQ_E_INVALID, e);
+    lap("build touched tenants (host, all cores)");
+    // the tag-table fill bound: placing the wide tenants one by one fails at the first that passes 3/4, i.e. exactly when
+    // their wide edges together pass it
+    {
+        uint64_t added = 0;
+        for (uint32_t k : by_size) added += plans[k].img.meta.big_edges;
+        if (added > 0 && tag_live + added > tag_max) return BFQ_NEED_FULL;
+    }
+    // ---- bases in key order: dense ranks, appended slot regions / segment slices, running prefix-count bases; the runs of the
+    // per-rank arrays (untouched tenants: from the old snapshot, shifted; rebuilt ones: from the packed upload)
+    uint64_t slot_cursor = of.n_slots, seg_cursor = of.segs.size();
+    int64_t rank = 0, pack_n = 0;
+    uint32_t ppb = 0, pgb = 0;
+    nf.tenants.reserve(entries.size());
+    std::vector<RankRun> runs;
+    auto add_run = [&](int64_t new_lo, int64_t len, int64_t src_lo, uint32_t packed, uint32_t dP, uint32_t dG) {
+        if (len <= 0) return;
+        if (!runs.empty()) {
+            RankRun& r = runs.back();
+            if (r.packed == packed && (int64_t) r.src_lo + r.len == src_lo && r.dP == dP && r.dG == dG) {
+                r.len += (uint32_t) len;
+                return;
+            }
+        }
+        runs.push_back(RankRun{(uint32_t) new_lo, (uint32_t) len, (uint32_t) src_lo, packed, dP, dG});
+    };
     for (auto& e : entries) {
         if (e.plan < 0) {   // untouched: same region, ranks moved by the growth of the tenants before it
             TenantMeta m = of.tenants[(size_t) e.old_index];
+            add_run(rank, m.n_routes, m.lo, 0, ppb - m.pp_base, pgb - m.pg_base);
             m.lo = rank;
             m.pp_base = ppb;
             m.pg_base = pgb;
@@ -1095,43 +1155,88 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
             ppb += m.pp;
             pgb += m.pg;
             nf.tenants.push_back(std::move(m));
+            continue;
+        }
+        Plan& pl = plans[(size_t) e.plan];
+        TenantMeta& m = pl.img.meta;
+        m.region_base = slot_cursor;
+        m.seg_base = seg_cursor;
+        m.pp_base = ppb;
+        m.pg_base = pgb;
+        pl.pack_lo = pack_n;
+        add_run(rank, m.n_routes, pack_n, 1, 0, 0);
+        slot_cursor += m.csr_slots;
+        seg_cursor += m.seg_words;
+        rank += m.n_routes;
+        pack_n += m.n_routes;
+        ppb += m.pp;
+        pgb += m.pg;
+        nf.tenants.emplace_back();   // its placed meta, below
+    }
+    if (slot_cursor >= 0x7FFFFFF0ull) return BFQ_NEED_FULL;
+    // ---- the place step, into two staging buffers uploaded with one copy each: the rebuilt regions back to back (uninitialised;
+    // first touched by the placing threads), and [rkind | pfxP | pfxG | runs] of the rebuilt tenants. (Pageable: pinning
+    // gigabytes when a commit rebuilds most tenants costs more than the driver's staged copy.)
+    const uint64_t up_slots = slot_cursor - of.n_slots;
+    SlotVec regions_up((size_t) up_slots);
+    const size_t off_pfxP = ((size_t) pack_n + 15) & ~(size_t) 15, off_pfxG = off_pfxP + (size_t) pack_n * 4;
+    const size_t off_runs = (off_pfxG + (size_t) pack_n * 4 + 15) & ~(size_t) 15, pack_bytes = off_runs + runs.size() * sizeof(RankRun);
+    std::vector<uint8_t> pack(pack_bytes);
+    memcpy(pack.data() + off_runs, runs.data(), runs.size() * sizeof(RankRun));
+    lap("staging allocation");
+    auto place = [&](uint32_t k, EdgeTable* tags, uint64_t tag_room) {
+        Plan& pl = plans[k];
+        TenantImage& img = pl.img;
+        const TenantMeta& m = img.meta;
+        if (!place_tenant_image(&img, m.region_base, m.seg_base, m.pp_base, m.pg_base, tags, tag_room,
+                                regions_up.data() + (m.region_base - of.n_slots), &errs[k]))
+            return;
+        const size_t n = (size_t) m.n_routes, at = (size_t) pl.pack_lo;
+        memcpy(pack.data() + at, img.rkind.data(), n);
+        memcpy(pack.data() + off_pfxP + at * 4, img.pfxP.data(), n * 4);
+        memcpy(pack.data() + off_pfxG + at * 4, img.pfxG.data(), n * 4);
+    };
+    std::vector<uint32_t> narrow;
+    for (uint32_t k : by_size)
+        if (plans[k].img.meta.big_edges == 0) narrow.push_back(k);
+    parallel_for_each(narrow, [&](uint32_t k) { place(k, nullptr, 0); });
+    for (auto& e : entries) {   // the wide ones: one after another in key order, into the copy of the tag bytes
+        if (e.plan < 0 || plans[(size_t) e.plan].img.meta.big_edges == 0) continue;
+        place((uint32_t) e.plan, &table, tag_max > tag_live ? tag_max - tag_live : 0);
+        if (!errs[(size_t) e.plan].empty()) break;
+        if (!plans[(size_t) e.plan].img.placed) return BFQ_NEED_FULL;   // its wide edges would fill the tag table past 3/4
+        tag_live += plans[(size_t) e.plan].img.meta.big_edges;
+    }
+    for (auto& e : errs)
+        if (!e.empty()) return fail(BFQ_E_INVALID, e);
+    if ((uint64_t) table.overflowed_blocks * 4 > (uint64_t) table.n_blocks) return BFQ_NEED_FULL;   // probes got too long
+    lap("place touched tenants (host, all cores)");
+    sn->th.reserve(entries.size());
+    // the old snapshot's per-tenant fan-out tables may be filled in by a concurrent bfq_fanout_device: copy them under its lock
+    std::vector<Snapshot::TenantHost> old_th;
+    {
+        std::lock_guard<std::mutex> gf(old->fan_mu);
+        old_th = old->th;
+    }
+    for (size_t i = 0; i < entries.size(); i++) {
+        const Entry& e = entries[i];
+        if (e.plan < 0) {
             sn->th.push_back(old_th[(size_t) e.old_index]);
             continue;
         }
         Plan& pl = plans[(size_t) e.plan];
-        uint32_t ordinal;
-        const std::string id = pl.prefix.substr(3);
-        if (pl.old_index >= 0) {
-            ordinal = of.tenants[(size_t) pl.old_index].ordinal;
-        } else {
-            ordinal = (uint32_t) nf.host_roots.size();
-            nf.host_roots.emplace_back();
-            nf.tenant_ordinal[id] = ordinal;
-        }
-        const uint64_t tag_room = tag_max > tag_live ? tag_max - tag_live : 0;
-        if (!build_tenant_image(*pl.kv, sv(id), ordinal, rank, slot_cursor, seg_cursor, ppb, pgb, &table, tag_room, &pl.img, &err))
-            return fail(BFQ_E_INVALID, err);
-        if (!pl.img.placed) return BFQ_NEED_FULL;   // its wide edges would fill the tag table past 3/4
-        tag_live += pl.img.meta.big_edges;
-        slot_cursor += pl.img.meta.csr_slots;
-        seg_cursor += pl.img.meta.seg_words;
-        rank += pl.img.meta.n_routes;
-        ppb += pl.img.meta.pp;
-        pgb += pl.img.meta.pg;
-        nf.host_roots[ordinal] = pl.img.root;
+        nf.host_roots[pl.ordinal] = pl.img.root;
         nf.segs.insert(nf.segs.end(), pl.img.segs.begin(), pl.img.segs.end());
         nf.max_nodes_per_depth = std::max(nf.max_nodes_per_depth, pl.img.meta.max_depth_nodes);
         nf.max_tenant_nodes = std::max(nf.max_tenant_nodes, pl.img.meta.walk_nodes);
-        nf.tenants.push_back(pl.img.meta);
+        nf.tenants[i] = pl.img.meta;
         Snapshot::TenantHost thh;
         thh.kv = pl.kv;
-        thh.rkind = std::make_shared<const std::vector<uint8_t>>(pl.img.rkind);
+        thh.rkind = std::make_shared<const std::vector<uint8_t>>(std::move(pl.img.rkind));
         sn->th.push_back(std::move(thh));
     }
     for (auto& pl : plans)
         if (!pl.kv) nf.tenant_ordinal.erase(pl.prefix.substr(3));   // its root record stays behind, unreachable
-    if (slot_cursor >= 0x7FFFFFF0ull || rank >= (int64_t) 0x7FFFFFFF) return BFQ_NEED_FULL;
-    if ((uint64_t) table.overflowed_blocks * 4 > (uint64_t) table.n_blocks) return BFQ_NEED_FULL;   // probes got too long
     nf.tags = std::move(table.tags);
     nf.n_big_edges = tag_live;
     nf.overflowed_blocks = table.overflowed_blocks;
@@ -1149,15 +1254,17 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
     for (auto& pl : plans)
         if (pl.old_index >= 0) sn->garbage_slots += of.tenants[(size_t) pl.old_index].csr_slots;
     sn->delta_commits = old->delta_commits + 1;
-    lap("rebuild touched tenants (host)");
-    // ---- device: copy, patch, shift
+    lap("host bookkeeping");
+    // ---- device: copy, upload, assemble, patch, shift
     cudaStream_t st = nullptr;
     CUDA_TRY(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    DevBuf<uint8_t> d_pack;   // the packed per-rank arrays and the run table
     struct StreamGuard {
         cudaStream_t s;
-        ~StreamGuard() { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
-    } guard{st};
-    const size_t n_new = (size_t) rank, n_old = (size_t) of.n_routes;
+        DevBuf<uint8_t>& pack;
+        ~StreamGuard() { cudaStreamSynchronize(s); cudaStreamDestroy(s); pack.release(); }
+    } guard{st, d_pack};
+    const size_t n_new = (size_t) rank;
     CUDA_TRY(sn->d_slots.reserve((size_t) slot_cursor));
     CUDA_TRY(sn->d_tags.reserve(std::max<size_t>(nf.tags.size(), 1)));
     CUDA_TRY(sn->d_roots.reserve(std::max<size_t>(nf.host_roots.size(), 1)));
@@ -1165,12 +1272,32 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
     CUDA_TRY(sn->d_rkind.reserve(std::max<size_t>(n_new, 1)));
     CUDA_TRY(sn->d_pfxP.reserve(n_new + 1));
     CUDA_TRY(sn->d_pfxG.reserve(n_new + 1));
+    CUDA_TRY(d_pack.reserve(pack_bytes));
     lap("device allocations");
     CUDA_TRY(cudaMemcpyAsync(sn->d_slots.p, old->d_slots.p, (size_t) of.n_slots * sizeof(Slot), cudaMemcpyDeviceToDevice, st));
+    if (up_slots) CUDA_TRY(cudaMemcpyAsync(sn->d_slots.p + of.n_slots, regions_up.data(), (size_t) up_slots * sizeof(Slot), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(d_pack.p, pack.data(), pack_bytes, cudaMemcpyHostToDevice, st));
     // the whole tag array (16 B per block, ~2 B per wide edge): one small upload
     if (!nf.tags.empty()) CUDA_TRY(cudaMemcpyAsync(sn->d_tags.p, nf.tags.data(), nf.tags.size(), cudaMemcpyHostToDevice, st));
-    // untouched tenants: slot regions and tag slots whose ranks move, and the pieces of the per-rank arrays; rebuilt tenants:
-    // their tag-table records
+    {
+        AssembleRankParams ap;
+        ap.rkind = sn->d_rkind.p;
+        ap.pfxP = sn->d_pfxP.p;
+        ap.pfxG = sn->d_pfxG.p;
+        ap.old_rkind = old->d_rkind.p;
+        ap.old_pfxP = old->d_pfxP.p;
+        ap.old_pfxG = old->d_pfxG.p;
+        ap.up_rkind = d_pack.p;
+        ap.up_pfxP = (const uint32_t*) (d_pack.p + off_pfxP);
+        ap.up_pfxG = (const uint32_t*) (d_pack.p + off_pfxG);
+        ap.runs = (const RankRun*) (d_pack.p + off_runs);
+        ap.n_runs = (int32_t) runs.size();
+        ap.n = (int64_t) n_new;
+        ap.tailP = ppb;
+        ap.tailG = pgb;
+        launch_assemble_rank_arrays(ap, st);
+    }
+    // untouched tenants whose ranks move: slot regions and tag slots; rebuilt tenants: their tag-table records
     std::vector<RankShiftRegion> regions;
     std::vector<RankShiftSlot> shift_slots;
     std::vector<uint32_t> scatter_ids;
@@ -1182,12 +1309,6 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
             const TenantImage& img = plans[(size_t) e.plan].img;
             scatter_ids.insert(scatter_ids.end(), m.tag_slots.begin(), m.tag_slots.end());
             scatter_recs.insert(scatter_recs.end(), img.tag_recs.begin(), img.tag_recs.end());
-            if (m.csr_slots) CUDA_TRY(cudaMemcpyAsync(sn->d_slots.p + m.region_base, img.slots.data(), (size_t) m.csr_slots * sizeof(Slot), cudaMemcpyHostToDevice, st));
-            if (m.n_routes) {
-                CUDA_TRY(cudaMemcpyAsync(sn->d_rkind.p + m.lo, img.rkind.data(), (size_t) m.n_routes, cudaMemcpyHostToDevice, st));
-                CUDA_TRY(cudaMemcpyAsync(sn->d_pfxP.p + m.lo, img.pfxP.data(), (size_t) m.n_routes * 4, cudaMemcpyHostToDevice, st));
-                CUDA_TRY(cudaMemcpyAsync(sn->d_pfxG.p + m.lo, img.pfxG.data(), (size_t) m.n_routes * 4, cudaMemcpyHostToDevice, st));
-            }
             continue;
         }
         const TenantMeta& om = of.tenants[(size_t) e.old_index];
@@ -1201,39 +1322,6 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
             if (m.seg_words) shift_seg_slice(nf.segs, m.seg_base, m.seg_words, d);
         }
     }
-    // per-rank arrays of the untouched tenants: maximal runs with one rank shift and one pair of prefix-count shifts
-    for (size_t i = 0; i < nf.tenants.size();) {
-        if (entries[i].plan >= 0) {
-            i++;
-            continue;
-        }
-        const TenantMeta& m0 = nf.tenants[i];
-        const TenantMeta& o0 = of.tenants[(size_t) entries[i].old_index];
-        const int64_t d = m0.lo - o0.lo;
-        const uint32_t dP = m0.pp_base - o0.pp_base, dG = m0.pg_base - o0.pg_base;
-        size_t j = i;
-        int64_t len = 0;
-        while (j < nf.tenants.size() && entries[j].plan < 0) {
-            const TenantMeta& m = nf.tenants[j];
-            const TenantMeta& om = of.tenants[(size_t) entries[j].old_index];
-            if (m.lo - om.lo != d || m.pp_base - om.pp_base != dP || m.pg_base - om.pg_base != dG || om.lo != o0.lo + len) break;
-            len += m.n_routes;
-            j++;
-        }
-        if (len > 0) {
-            CUDA_TRY(cudaMemcpyAsync(sn->d_rkind.p + m0.lo, old->d_rkind.p + o0.lo, (size_t) len, cudaMemcpyDeviceToDevice, st));
-            launch_copy_add(sn->d_pfxP.p + m0.lo, old->d_pfxP.p + o0.lo, len, dP, st);
-            launch_copy_add(sn->d_pfxG.p + m0.lo, old->d_pfxG.p + o0.lo, len, dG, st);
-        }
-        i = j;
-    }
-    {
-        const uint32_t tail[2] = {ppb, pgb};
-        CUDA_TRY(cudaMemcpyAsync(sn->d_pfxP.p + n_new, &tail[0], 4, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(sn->d_pfxG.p + n_new, &tail[1], 4, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaStreamSynchronize(st));   // `tail` is on the stack
-    }
-    (void) n_old;
     if (!scatter_ids.empty()) {
         DevBuf<uint32_t> d_ids;
         DevBuf<Slot> d_recs;
@@ -1292,22 +1380,27 @@ int32_t bfq_index_commit(bfq_index* h) {
     }();
     if (old && delta_enabled && !h->staging.bulk_changed()) {
         const std::vector<std::string> dirty = h->staging.dirty_tenants();
-        if (dirty.empty()) return BFQ_OK;   // nothing staged since the last commit
-        if (dirty.size() <= 64) {
-            const int32_t rc = commit_delta(h, old, dirty);
-            if (rc != BFQ_NEED_FULL) {
-                if (rc == BFQ_OK) {
-                    std::lock_guard<std::mutex> g(h->mu);
-                    h->delta_commits++;
-                }
-                return rc;
+        if (dirty.empty()) {   // nothing staged since the last commit
+            std::lock_guard<std::mutex> g(h->mu);
+            h->rebuilt_tenants = 0;
+            return BFQ_OK;
+        }
+        int64_t built = 0;
+        const int32_t rc = commit_delta(h, old, dirty, &built);
+        if (rc != BFQ_NEED_FULL) {
+            if (rc == BFQ_OK) {
+                std::lock_guard<std::mutex> g(h->mu);
+                h->delta_commits++;
+                h->rebuilt_tenants = built;
             }
+            return rc;
         }
     }
     const int32_t rc = commit_full(h);
     if (rc == BFQ_OK) {
         std::lock_guard<std::mutex> g(h->mu);
         h->full_commits++;
+        h->rebuilt_tenants = (int64_t) h->snap->flat.tenants.size();
     }
     return rc;
 }
@@ -1339,13 +1432,14 @@ int32_t bfq_index_stats(bfq_index* h, int64_t* stats, int32_t n) {
     std::lock_guard<std::mutex> g(h->mu);
     static const FlatIndex empty;
     const FlatIndex& f = h->snap ? h->snap->flat : empty;
-    const int64_t v[21] = {f.n_routes, (int64_t) f.tenant_ordinal.size(), f.n_nodes, (int64_t) f.n_slots,
+    const int64_t v[22] = {f.n_routes, (int64_t) f.tenant_ordinal.size(), f.n_nodes, (int64_t) f.n_slots,
                            h->snap ? h->snap->device_bytes() : 0, f.max_nodes_per_depth, h->launches, h->overflow_topics,
                            h->flagged_topics, f.n_multi, f.n_cont_chunks, h->deferred_topics, h->duplicate_topics,
                            h->full_commits, h->delta_commits, h->snap ? (int64_t) h->snap->garbage_slots : 0,
                            h->buffer_retries, h->global_fanouts,
-                           h->snap ? (int64_t) f.n_blocks * BLOCK_USABLE : 0, (int64_t) f.n_big_edges, f.overflowed_blocks};
-    for (int32_t i = 0; i < n && i < 21; i++) stats[i] = v[i];
+                           h->snap ? (int64_t) f.n_blocks * BLOCK_USABLE : 0, (int64_t) f.n_big_edges, f.overflowed_blocks,
+                           h->rebuilt_tenants};
+    for (int32_t i = 0; i < n && i < 22; i++) stats[i] = v[i];
     return BFQ_OK;
 }
 
@@ -1399,8 +1493,9 @@ int32_t bfq_host_build_stats(const uint8_t* keys, const int64_t* key_off, const 
         if (!build_flat_index(snapshot, &flat2, &err)) return fail(BFQ_E_INVALID, err);
         same_as_concat = image_sum_of(flat2) == image_sum && flat2.n_nodes == flat.n_nodes && flat2.tenants.size() == flat.tenants.size();
     }
-    // stats[18]: tenants whose stand-alone image (build_tenant_image with the full build's bases — what a delta commit
-    // uploads for a touched tenant) equals their part of the full image byte for byte; -1 - index of the first that differs
+    // stats[18]: tenants whose stand-alone image (build_tenant_image + place_tenant_image with the full build's bases — what a
+    // delta commit uploads for a touched tenant) equals their part of the full image byte for byte; -1 - index of the first
+    // that differs
     int64_t tenant_images_equal = 0;
     if (n_stats > 18) {
         size_t ti = 0;
@@ -1465,8 +1560,8 @@ int32_t bfq_host_build_stats(const uint8_t* keys, const int64_t* key_off, const 
             for (uint32_t s : m.tag_slots) sim.release(s);
             const uint64_t base = flat.n_slots;
             TenantImage img;
-            if (!build_tenant_image(*kvp.second.base, sv(m.tenant), m.ordinal, m.lo, base, flat.segs.size(), m.pp_base, m.pg_base, &sim,
-                                    ~0ull, &img, &err))
+            if (!build_tenant_image(*kvp.second.base, sv(m.tenant), m.ordinal, m.lo, &img, &err) ||
+                !place_tenant_image(&img, base, flat.segs.size(), m.pp_base, m.pg_base, &sim, ~0ull, nullptr, &err))
                 return fail(BFQ_E_INVALID, err);
             if (!img.placed || img.meta.tag_slots.size() != m.big_edges) continue;
             for (size_t k = 0; k < img.tag_recs.size(); k++) sim.slots[img.meta.tag_slots[k]] = img.tag_recs[k];

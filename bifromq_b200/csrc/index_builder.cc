@@ -93,10 +93,8 @@ std::vector<std::string> Staging::dirty_tenants() const {
     return out;
 }
 
-void Staging::merge_tenant(const std::string& prefix) {
-    auto it = tenants_.find(prefix);
-    if (it == tenants_.end()) return;
-    TenantStage& ts = it->second;
+namespace {
+void merge_stage(TenantStage& ts) {
     if (!ts.delta.empty()) {
         const KVBlob& base = *ts.base;
         auto merged = std::make_shared<KVBlob>();
@@ -135,12 +133,34 @@ void Staging::merge_tenant(const std::string& prefix) {
         ts.base = std::move(merged);
         ts.delta.clear();
     }
-    if (ts.base->n() == 0) tenants_.erase(it);
+}
+}  // namespace
+
+void Staging::merge_tenant(const std::string& prefix) {
+    auto it = tenants_.find(prefix);
+    if (it == tenants_.end()) return;
+    merge_stage(it->second);
+    if (it->second.base->n() == 0) tenants_.erase(it);
+}
+void Staging::merge_tenants(const std::vector<std::string>& prefixes) {
+    std::vector<TenantStage*> stages;
+    std::vector<uint32_t> order;
+    for (auto& p : prefixes) {
+        auto it = tenants_.find(p);
+        if (it == tenants_.end()) continue;
+        order.push_back((uint32_t) stages.size());
+        stages.push_back(&it->second);
+    }
+    parallel_for_each(order, [&](uint32_t i) { merge_stage(*stages[i]); });
+    for (auto& p : prefixes) {   // erasing from the map is not thread-safe
+        auto it = tenants_.find(p);
+        if (it != tenants_.end() && it->second.base->n() == 0) tenants_.erase(it);
+    }
 }
 void Staging::merge_all() {
     std::vector<std::string> names;
     for (auto& kv : tenants_) names.push_back(kv.first);
-    for (auto& nme : names) merge_tenant(nme);
+    merge_tenants(names);
 }
 
 KVBlob Staging::concat() const {
@@ -893,16 +913,22 @@ void place_tenant(TenantBuild& tb, EdgeTable& table) {
 
 template <typename F>
 void parallel_for_tenants(std::vector<TenantBuild>& tenants, const std::vector<uint32_t>& by_size, F&& f) {
+    parallel_for_each(by_size, [&](uint32_t i) { f(tenants[i]); });
+}
+
+}  // namespace
+
+void parallel_for_each(const std::vector<uint32_t>& order, const std::function<void(uint32_t)>& f) {
     unsigned nthreads = std::thread::hardware_concurrency();
     if (nthreads == 0) nthreads = 1;
     nthreads = std::min<unsigned>(nthreads, 64);
-    nthreads = (unsigned) std::min<size_t>(nthreads, std::max<size_t>(tenants.size(), 1));
+    nthreads = (unsigned) std::min<size_t>(nthreads, std::max<size_t>(order.size(), 1));
     std::atomic<size_t> cursor{0};
     auto worker = [&]() {
         while (true) {
             const size_t i = cursor.fetch_add(1);
-            if (i >= by_size.size()) break;
-            f(tenants[by_size[i]]);
+            if (i >= order.size()) break;
+            f(order[i]);
         }
     };
     if (nthreads <= 1) {
@@ -913,8 +939,6 @@ void parallel_for_tenants(std::vector<TenantBuild>& tenants, const std::vector<u
     for (unsigned t = 0; t < nthreads; t++) th.emplace_back(worker);
     for (auto& t : th) t.join();
 }
-
-}  // namespace
 
 namespace {
 
@@ -1164,61 +1188,87 @@ bool build_from_tenants(std::vector<TenantBuild>& tenants, int64_t n, FlatIndex*
 
 }  // namespace
 
-bool build_tenant_image(const KVBlob& tkv, sv tenant, uint32_t ordinal, int64_t rank_lo, uint64_t region_base, uint64_t seg_base,
-                        uint32_t pp_base, uint32_t pg_base, EdgeTable* tags, uint64_t tag_room, TenantImage* out, std::string* err) {
-    *out = TenantImage();
-    const int64_t n = tkv.n();
+// the trie and plans of one tenant between build_tenant_image and place_tenant_image
+struct TenantBuildState {
+    std::string tenant;   // tb.tenant views it
     TenantBuild tb;
-    tb.tenant = tenant;
+};
+
+bool build_tenant_image(const KVBlob& tkv, sv tenant, uint32_t ordinal, int64_t rank_lo, TenantImage* img, std::string* err) {
+    *img = TenantImage();
+    auto state = std::make_shared<TenantBuildState>();
+    state->tenant = std::string(tenant);
+    TenantBuild& tb = state->tb;
+    const int64_t n = tkv.n();
+    tb.tenant = state->tenant;
     tb.lo = 0;
     tb.hi = n;
     tb.ordinal = ordinal;
     tb.rank_off = rank_lo;
     tb.index_off = 0;
-    out->rkind.assign((size_t) n, 0);
-    out->pfxP.assign((size_t) n + 1, 0);
-    out->pfxG.assign((size_t) n + 1, 0);
-    tb.rkind = out->rkind.data();
-    tb.pfxP = out->pfxP.data();
-    tb.pfxG = out->pfxG.data();
+    img->rkind.assign((size_t) n, 0);
+    img->pfxP.assign((size_t) n + 1, 0);
+    img->pfxG.assign((size_t) n + 1, 0);
+    tb.rkind = img->rkind.data();
+    tb.pfxP = img->pfxP.data();
+    tb.pfxG = img->pfxG.data();
     build_tenant(tkv, tb);
     if (!tb.err.empty()) {
         if (err) *err = tb.err;
         return false;
     }
-    TenantMeta& m = out->meta;
-    m.tenant = std::string(tenant);
+    TenantMeta& m = img->meta;
+    m.tenant = state->tenant;
     m.ordinal = ordinal;
     m.lo = rank_lo;
     m.n_routes = n;
-    m.region_base = region_base;
     m.csr_slots = tb.csr_slots;
-    m.seg_base = seg_base;
     m.seg_words = tb.seg_words;
     m.pp = tb.pp;
     m.pg = tb.pg;
-    m.pp_base = pp_base;
-    m.pg_base = pg_base;
     m.tenant_nodes = (int64_t) tb.b.nodes.size();
     m.max_depth_nodes = tb.max_depth_nodes;
     m.walk_nodes = tb.tenant_nodes;
     m.n_cont = tb.b.n_cont;
     m.big_edges = tb.big_edges;
+    img->state = std::move(state);
+    return true;
+}
+
+bool place_tenant_image(TenantImage* img, uint64_t region_base, uint64_t seg_base, uint32_t pp_base, uint32_t pg_base, EdgeTable* tags,
+                        uint64_t tag_room, Slot* region, std::string* err) {
+    if (!img->state) {
+        if (err) *err = "internal error: a tenant image is placed that was not built, or twice";
+        return false;
+    }
+    TenantBuild& tb = img->state->tb;
+    TenantMeta& m = img->meta;
+    const int64_t n = m.n_routes;
+    m.region_base = region_base;
+    m.seg_base = seg_base;
+    m.pp_base = pp_base;
+    m.pg_base = pg_base;
     if (tb.big_edges > 0 && (!tags || tb.big_edges > tag_room)) return true;   // not placed: the caller decides
     tb.region_base = region_base;
     tb.seg_base = seg_base;
     tb.pp_base = pp_base;
     tb.pg_base = pg_base;
-    out->slots.resize((size_t) tb.csr_slots);
+    tb.rkind = img->rkind.data();
+    tb.pfxP = img->pfxP.data();
+    tb.pfxG = img->pfxG.data();
+    if (!region) {
+        img->slots.resize((size_t) tb.csr_slots);
+        region = img->slots.data();
+    }
     {   // uninitialised; filled (first-touched) by several threads when the tenant is large
-        const size_t total = out->slots.size(), piece = 1u << 16;
+        const size_t total = (size_t) tb.csr_slots, piece = 1u << 16;
         const unsigned nt = total >= (1u << 20) ? std::min<unsigned>(std::max(1u, std::thread::hardware_concurrency()), 16u) : 1u;
         std::atomic<size_t> next{0};
         auto worker = [&]() {
             while (true) {
                 const size_t at = next.fetch_add(piece);
                 if (at >= total) break;
-                fill_empty_slots(out->slots.data() + at, std::min(piece, total - at));
+                fill_empty_slots(region + at, std::min(piece, total - at));
             }
         };
         std::vector<std::thread> th;
@@ -1226,24 +1276,25 @@ bool build_tenant_image(const KVBlob& tkv, sv tenant, uint32_t ordinal, int64_t 
         worker();
         for (auto& t : th) t.join();
     }
-    out->segs.assign((size_t) tb.seg_words, 0);
-    tb.slots = out->slots.data();
+    img->segs.assign((size_t) tb.seg_words, 0);
+    tb.slots = region;
     tb.slot_origin = region_base;
-    tb.root_rec = &out->root;
-    tb.segs = out->segs.data();
+    tb.root_rec = &img->root;
+    tb.segs = img->segs.data();
     tb.seg_origin = seg_base;
-    tb.tag_recs = &out->tag_recs;
+    tb.tag_recs = &img->tag_recs;
     EdgeTable unused;
     place_tenant(tb, tags ? *tags : unused);
     if (!tb.err.empty()) {
         if (err) *err = tb.err;
         return false;
     }
-    out->pfxP[(size_t) n] = pp_base + tb.pp;
-    out->pfxG[(size_t) n] = pg_base + tb.pg;
+    img->pfxP[(size_t) n] = pp_base + tb.pp;
+    img->pfxG[(size_t) n] = pg_base + tb.pg;
     m.n_multi = tb.n_multi;
     m.tag_slots = std::move(tb.tag_slots);
-    out->placed = true;
+    img->placed = true;
+    img->state.reset();
     return true;
 }
 

@@ -2,6 +2,7 @@
 // all tenants' filter tries into the hash-table layout of trie_layout.h.
 #pragma once
 #include <cstdint>
+#include <functional>
 #include <map>
 #include <memory>
 #include <string>
@@ -46,27 +47,41 @@ struct TenantMeta {
 };
 
 // One tenant built on its own (bfq_index_commit's delta path): records carry absolute slot ids / ranks for the given bases.
+// It is made in two steps, so that a commit can build many tenants in parallel before it knows where each one goes:
+// build_tenant_image (trie, child-array plans, sizes) and place_tenant_image (placement and records at given bases).
+struct TenantBuildState;                   // the trie and plans between the two steps (index_builder.cc)
 struct TenantImage {
-    TenantMeta meta;
-    bool placed = false;                   // false: built (meta is valid) but not placed, see build_tenant_image
-    SlotVec slots;                         // csr_slots records, slot region_base + i at [i]
+    TenantMeta meta;                       // after the build step: every size and count; after placing: the bases too
+    bool placed = false;                   // false: not placed (yet), see place_tenant_image
+    SlotVec slots;                         // csr_slots records, slot region_base + i at [i] (unless placed into a caller's buffer)
     std::vector<Slot> tag_recs;            // records of the nodes placed in the tag table, slot meta.tag_slots[i] at [i]
     Slot root;
     std::vector<uint32_t> segs;            // seg_words
     std::vector<uint8_t> rkind;            // n
-    std::vector<uint32_t> pfxP, pfxG;      // n + 1, already offset by the given bases
+    std::vector<uint32_t> pfxP, pfxG;      // n + 1: tenant-local after the build step, offset by the given bases after placing
+    std::shared_ptr<TenantBuildState> state;   // released by place_tenant_image
 };
-// Builds one tenant and places it at the given bases. The children of its wide nodes claim slots in `tags` (the live tag table
-// of the index, whose slot array stays on the device: only the tag bytes are touched) exactly as the full build's placement
-// does; their records come back in tag_recs instead of the region buffer. A tenant with wide edges is left unplaced
-// (placed = false, nothing claimed) when `tags` is null or when it has more than `tag_room` of them.
-bool build_tenant_image(const KVBlob& tenant_kv, sv tenant, uint32_t ordinal, int64_t rank_lo, uint64_t region_base, uint64_t seg_base,
-                        uint32_t pp_base, uint32_t pg_base, EdgeTable* tags, uint64_t tag_room, TenantImage* out, std::string* err);
-// the same without a tag table: a tenant with wide edges is built but not placed
+// The build step: decodes the tenant's keys, builds its trie and plans its child arrays. Its routes get the ranks
+// [rank_lo, rank_lo + n): a tenant's ranks depend only on the sizes of the tenants before it. Fills meta's sizes and counts
+// (n_routes, csr_slots, seg_words, pp, pg, big_edges, node counts), rkind and the tenant-local prefix counts. Thread-safe for
+// distinct images.
+bool build_tenant_image(const KVBlob& tenant_kv, sv tenant, uint32_t ordinal, int64_t rank_lo, TenantImage* img, std::string* err);
+// The place step: places a built tenant at the given bases and emits its records, into `region` (csr_slots records) or, when
+// it is null, into img->slots. The children of its wide nodes claim slots in `tags` (the live tag table of the index, whose
+// slot array stays on the device: only the tag bytes are touched) exactly as the full build's placement does; their records
+// come back in tag_recs instead of the region. A tenant with wide edges is left unplaced (placed = false, nothing claimed)
+// when `tags` is null or when it has more than `tag_room` of them. Tenants without wide edges touch no shared state, so they
+// can be placed in parallel; tenants with wide edges claim from `tags` and are placed one after another.
+bool place_tenant_image(TenantImage* img, uint64_t region_base, uint64_t seg_base, uint32_t pp_base, uint32_t pg_base, EdgeTable* tags,
+                        uint64_t tag_room, Slot* region, std::string* err);
+// Both steps at once, without a tag table: a tenant with wide edges is built but not placed
 inline bool build_tenant_image(const KVBlob& tenant_kv, sv tenant, uint32_t ordinal, int64_t rank_lo, uint64_t region_base, uint64_t seg_base,
                                uint32_t pp_base, uint32_t pg_base, TenantImage* out, std::string* err) {
-    return build_tenant_image(tenant_kv, tenant, ordinal, rank_lo, region_base, seg_base, pp_base, pg_base, nullptr, 0, out, err);
+    return build_tenant_image(tenant_kv, tenant, ordinal, rank_lo, out, err) &&
+           place_tenant_image(out, region_base, seg_base, pp_base, pg_base, nullptr, 0, nullptr, err);
 }
+// Runs f(i) for every i of `order` on all host cores, taking them in that order (largest task first keeps the cores busy)
+void parallel_for_each(const std::vector<uint32_t>& order, const std::function<void(uint32_t)>& f);
 
 // Everything the device needs, in host memory, plus build statistics.
 struct FlatIndex {
@@ -117,6 +132,9 @@ public:
     std::vector<std::string> dirty_tenants() const;
     // merges one tenant's delta into a NEW base blob (the old one may be pinned by a snapshot); erases the tenant if it ends empty
     void merge_tenant(const std::string& prefix);
+    // the same for many tenants, merged on all host cores (each merge rewrites only its own TenantStage); the tenants that end
+    // empty are erased afterwards, on the calling thread
+    void merge_tenants(const std::vector<std::string>& prefixes);
     void merge_all();
     const std::map<std::string, TenantStage>& tenants() const { return tenants_; }
     KVBlob concat() const;     // every tenant's base, in key order (the input of a full build)

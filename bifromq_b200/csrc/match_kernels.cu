@@ -1052,8 +1052,30 @@ __global__ void __launch_bounds__(256) scatter_records_kernel(Slot* slots, const
         slots[ids[i]].w[k] = recs[i].w[k];
     }
 }
-__global__ void __launch_bounds__(256) copy_add_kernel(uint32_t* dst, const uint32_t* src, int64_t n, uint32_t add) {
-    for (int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t) gridDim.x * blockDim.x) dst[i] = src[i] + add;
+// one thread per rank (striding); a thread finds its run by binary search over the run starts (a warp's lanes almost always
+// land in the same run, so the probes are broadcasts from L1)
+__global__ void __launch_bounds__(256) assemble_rank_arrays_kernel(const AssembleRankParams p) {
+    for (int64_t r = (int64_t) blockIdx.x * blockDim.x + threadIdx.x; r <= p.n; r += (int64_t) gridDim.x * blockDim.x) {
+        if (r == p.n) {
+            p.pfxP[r] = p.tailP;
+            p.pfxG[r] = p.tailG;
+            continue;
+        }
+        int lo = 0, hi = p.n_runs - 1;   // the last run with new_lo <= r
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if ((int64_t) p.runs[mid].new_lo <= r) lo = mid;
+            else hi = mid - 1;
+        }
+        const RankRun run = p.runs[lo];
+        const uint32_t s = run.src_lo + (uint32_t) (r - run.new_lo);
+        const uint8_t* rk = run.packed ? p.up_rkind : p.old_rkind;
+        const uint32_t* pP = run.packed ? p.up_pfxP : p.old_pfxP;
+        const uint32_t* pG = run.packed ? p.up_pfxG : p.old_pfxG;
+        p.rkind[r] = rk[s];
+        p.pfxP[r] = pP[s] + run.dP;
+        p.pfxG[r] = pG[s] + run.dG;
+    }
 }
 }  // namespace
 
@@ -1080,9 +1102,8 @@ void launch_scatter_records(Slot* slots, const uint32_t* d_ids, const Slot* d_re
     if (n <= 0) return;
     scatter_records_kernel<<<(unsigned) std::min<int64_t>((n * 16 + 255) / 256, (int64_t) device_sm_count() * 16), 256, 0, stream>>>(slots, d_ids, d_recs, n);
 }
-void launch_copy_add(uint32_t* dst, const uint32_t* src, int64_t n, uint32_t add, cudaStream_t stream) {
-    if (n <= 0) return;
-    copy_add_kernel<<<(unsigned) std::min<int64_t>((n + 255) / 256, (int64_t) device_sm_count() * 16), 256, 0, stream>>>(dst, src, n, add);
+void launch_assemble_rank_arrays(const AssembleRankParams& p, cudaStream_t stream) {
+    assemble_rank_arrays_kernel<<<(unsigned) std::min<int64_t>((p.n + 1 + 255) / 256, (int64_t) device_sm_count() * 16), 256, 0, stream>>>(p);
 }
 
 int match_kernel_smem_bytes() { return (int) sizeof(WarpSmem) * WARPS_PER_CTA; }

@@ -208,7 +208,27 @@ struct RankShiftSlot {
 void launch_rank_shift_listed(Slot* slots, const RankShiftSlot* d_list, int64_t n, cudaStream_t stream);
 // slots[ids[i]] = recs[i]: the tag-table records of the tenants a delta commit rebuilt
 void launch_scatter_records(Slot* slots, const uint32_t* d_ids, const Slot* d_recs, int64_t n, cudaStream_t stream);
-// dst[i] = src[i] + add (the prefix-count arrays of those tenants, copied to their shifted position)
-void launch_copy_add(uint32_t* dst, const uint32_t* src, int64_t n, uint32_t add, cudaStream_t stream);
+// The per-rank arrays (rkind and the two prefix counts) of a delta commit's new snapshot, all ranks in one launch. The ranks
+// are cut into runs sorted by new rank that tile [0, n): a run of untouched tenants is read from the old snapshot's arrays, a
+// run of rebuilt tenants from the packed upload; the prefix counts of a run move by (dP, dG) (mod 2^32, like the counts).
+struct RankRun {
+    uint32_t new_lo, len;   // new ranks [new_lo, new_lo + len)
+    uint32_t src_lo;        // first rank of the run in its source
+    uint32_t packed;        // 1: the packed upload, 0: the old snapshot
+    uint32_t dP, dG;
+};
+struct AssembleRankParams {
+    uint8_t* rkind;                                 // out [n]
+    uint32_t *pfxP, *pfxG;                          // out [n + 1]
+    const uint8_t* old_rkind;                       // the old snapshot's arrays
+    const uint32_t *old_pfxP, *old_pfxG;
+    const uint8_t* up_rkind;                        // the rebuilt tenants' arrays, packed in new-rank order
+    const uint32_t *up_pfxP, *up_pfxG;
+    const RankRun* runs;
+    int32_t n_runs;
+    int64_t n;
+    uint32_t tailP, tailG;                          // pfxP[n], pfxG[n]: the totals
+};
+void launch_assemble_rank_arrays(const AssembleRankParams& p, cudaStream_t stream);
 
 }  // namespace bfq

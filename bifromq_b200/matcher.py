@@ -177,12 +177,12 @@ class GpuRouteIndex:
         N.check(N.lib.bfq_index_commit(self._h))
 
     def stats(self):
-        s = np.zeros(21, np.int64)
+        s = np.zeros(22, np.int64)
         N.check(N.lib.bfq_index_stats(self._h, s.ctypes.data, len(s)))
         names = ["routes", "tenants", "nodes", "slots", "device_bytes", "max_nodes_per_depth", "launches",
                  "overflow_topics", "flagged_topics", "multi_segment_filters", "long_token_chunks", "deferred_topics",
                  "duplicate_topics", "full_commits", "delta_commits", "garbage_slots", "buffer_retries", "global_fanouts",
-                 "tag_usable_slots", "tag_used_slots", "tag_overflowed_blocks"]
+                 "tag_usable_slots", "tag_used_slots", "tag_overflowed_blocks", "rebuilt_tenants"]
         return dict(zip(names, s.tolist()))
 
     def deliverer(self, deliverer_id):

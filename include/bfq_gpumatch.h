@@ -81,19 +81,21 @@ int32_t bfq_index_apply(bfq_index* h, const uint8_t* add_keys, const int64_t* ad
  * Every snapshot has a generation (1, 2, ...); results report the generation they were produced from. The previous
  * snapshot is freed when the last match / result that pins it is gone. bfq_index_apply is all-or-nothing: an
  * undecodable key leaves the staging area untouched.
- * Delta path: a commit whose staged changes touch at most 64 tenants rebuilds only those tenants, whatever their shape.
+ * Delta path: a commit rebuilds only the tenants its staged changes touch, however many and whatever their shape (one
+ * batchAddRoute / batchRemoveRoute batch may span every tenant of the range); the touched tenants are rebuilt on all host
+ * cores and the device work is a fixed number of copies and launches.
  * Each gets a fresh slot region behind the existing ones (the one it replaces stays behind as garbage); the children of its
  * wide nodes (too many children for a private perfect-hash array, about a thousand) go into the shared tag table: its old
  * tag slots are freed first, then its new edges are placed into the free ones. The rest of the snapshot is copied on the
  * device and the ranks of the tenants behind a grown or shrunk tenant are moved. The commit is a full build instead when:
- *   - there is no snapshot yet, or bfq_index_reset / bfq_index_load ran since the last commit, or more than 64 tenants changed;
+ *   - there is no snapshot yet, or bfq_index_reset / bfq_index_load ran since the last commit;
  *   - garbage slots would exceed a quarter of the slots plus 4096;
  *   - claimed tag-table slots would exceed 3/4 of its usable slots (the table only grows with a full build);
  *   - tag-table blocks with their overflow byte set would exceed a quarter of the blocks (freed slots do not clear it, so
  *     churn lengthens probes until a full build resets them);
  *   - a slot id or rank would run out of 31 bits.
  * Both paths give the same answers as a handle fully built from the same KV. bfq_index_stats reports the path taken
- * (13, 14) and the tag table's fill (18..20). */
+ * (13, 14), the tag table's fill (18..20) and how many tenants the commit built (21). */
 int32_t bfq_index_commit(bfq_index* h);
 int32_t bfq_index_generation(bfq_index* h, uint64_t* generation);   /* 0 before the first commit */
 /* Tuning knobs (defaults are the measured best for a handle that has the GPU to itself):
@@ -116,7 +118,8 @@ int32_t bfq_index_set_option(bfq_index* h, const char* name, int64_t value);
  * 13 full commits, 14 delta commits, 15 garbage slots of the current snapshot, 16 match calls that found a range or
  * throttle buffer too small, grew it and re-ran the batch so far, 17 bfq_fanout_device calls that took the global-count
  * pass (rather than the shared-memory tile pass) so far, 18 usable tag-table slots (15 per block), 19 claimed tag-table
- * slots (children of wide nodes), 20 tag-table blocks whose overflow byte is set (all three of the current snapshot) */
+ * slots (children of wide nodes), 20 tag-table blocks whose overflow byte is set (all three of the current snapshot), 21 tenants
+ * the last bfq_index_commit built (0 when nothing changed, every tenant after a full build) */
 int32_t bfq_index_stats(bfq_index* h, int64_t* stats, int32_t n);
 /* device time of the tier-0 (lane-per-topic) match kernel of the latest completed match call on this handle, measured with
  * CUDA events recorded on the launching stream around the launch (for roofline accounting) */
