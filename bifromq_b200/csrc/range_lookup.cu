@@ -13,8 +13,10 @@
 // level when t_1 starts with '$'), "+" and t_{i+1} (the last two only while i < n; "+" not for a '$' first level), and the
 // node with i == n is itself a filter. seek(B) = the least member >= B in level-wise String.compareTo order is a lower-bound
 // walk of that trie: follow B while it is a path, remember the deepest level that has a greater sibling, and complete
-// minimally ("#" as soon as it is the smallest child). No trie is materialised; a member is a bitmask of '+' choices plus
-// where it ends. UTF-8 byte order equals UTF-16 code-unit order on BMP text (what the MQTT edge admits).
+// minimally ("#" as soon as it is the smallest child). No trie is materialised and no level is stored: the walk reads the
+// topic and the bounds through cursors, and the member it finds is described by how far it follows the bound, the one greater
+// child it takes there and where its minimal completion starts, so neither a topic nor a bound has a level limit. UTF-8 byte
+// order equals UTF-16 code-unit order on BMP text (what the MQTT edge admits).
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -30,7 +32,7 @@ int32_t set_error(int32_t code, const std::string& msg);
 
 namespace {
 
-constexpr int RL_MAX_LEVELS = 34;   // levels of a topic / of a bound this kernel handles (MaxTopicLevels default is 16)
+__device__ const uint8_t kWild[2] = {'#', '+'};   // the level of kind 0 and of kind 1 below
 
 struct Str {
     const uint8_t* p;
@@ -42,146 +44,147 @@ __device__ __forceinline__ int cmp(Str a, Str b) {   // bytewise, shorter prefix
         if (a.p[i] != b.p[i]) return a.p[i] < b.p[i] ? -1 : 1;
     return a.n == b.n ? 0 : (a.n < b.n ? -1 : 1);
 }
-__device__ __forceinline__ int split(const uint8_t* s, int len, uint8_t sep, int* start, int* end) {
-    int n = 0, b = 0;
-    for (int i = 0; i <= len; i++)
-        if (i == len || s[i] == sep) {
-            if (n < RL_MAX_LEVELS) {
-                start[n] = b;
-                end[n] = i;
-            }
-            n++;
-            b = i + 1;
+__device__ __forceinline__ Str wild(int kind) { return Str{kWild + kind, 1}; }
+__device__ __forceinline__ bool below_hash(Str s) { return s.n == 0 || s.p[0] < '#'; }   // s < "#"
+
+// cursor over the levels of a topic ('/') or of a NUL-joined bound: `pos` is where the next level starts, past `len` once every
+// level has been read
+struct Levels {
+    const uint8_t* s;
+    int len, pos;
+    uint8_t sep;
+    __device__ bool more() const { return pos <= len; }
+    __device__ Str peek() const {
+        int e = pos;
+        while (e < len && s[e] != sep) e++;
+        return Str{s + pos, e - pos};
+    }
+    __device__ void skip(Str l) { pos += l.n + 1; }
+    __device__ Str next() {
+        const Str l = peek();
+        skip(l);
+        return l;
+    }
+};
+
+// children of the node behind i matched levels, smallest first; kinds: 0 = "#", 1 = "+", 2 = the topic's level i + 1 (tx; only
+// while has_t, i.e. i < n). wild = false under the tenant level of a '$' topic: no "#" / "+" there
+__device__ __forceinline__ int children(bool wild, bool has_t, Str tx, int* kind) {
+    int c = 0;
+    if (has_t) {
+        // order "#" < "+" always; place the topic level among them
+        const int ch = cmp(tx, Str{kWild, 1}), cp = cmp(tx, Str{kWild + 1, 1});
+        if (!wild) {
+            kind[c++] = 2;
+        } else if (ch < 0) {
+            kind[c++] = 2; kind[c++] = 0; kind[c++] = 1;
+        } else if (ch == 0) {            // the topic level is literally "#" (not a valid topic, but keep the order total)
+            kind[c++] = 0; kind[c++] = 1;
+        } else if (cp < 0) {
+            kind[c++] = 0; kind[c++] = 2; kind[c++] = 1;
+        } else if (cp == 0) {
+            kind[c++] = 0; kind[c++] = 1;
+        } else {
+            kind[c++] = 0; kind[c++] = 1; kind[c++] = 2;
         }
-    return n;
+    } else if (wild) {
+        kind[c++] = 0;   // "#" matches the parent level
+    }
+    return c;
 }
 
-// a member of the expansion set: levels 1..depth choose '+' where the bit is set, else the topic's level; `hash` = it ends with
-// a "#" level behind them (else it is the full-length filter: depth == n)
+// A member of the expansion set as seek finds it, after the tenant level: the bound's levels 1..pre, then at most one level
+// that leaves the bound (div: -1 = none, 0 = "#", which ends the member, 1 = "+", 2 = the topic level at dpos), then the minimal
+// completion from topic position `tail`. The smallest child of a node is "#" unless the topic level sorts below it, or no
+// wildcard exists (under the tenant level of a '$' topic); it is never "+". So the completion follows topic levels while that
+// holds and then ends in "#", or it ends with the topic.
 struct Member {
-    uint64_t plus;
-    int depth;
-    bool hash;
+    int pre, div, dpos, tail;
 };
 
-struct Ctx {
-    const uint8_t* topic;
-    int ts[RL_MAX_LEVELS], te[RL_MAX_LEVELS], n;   // topic levels
-    bool sys;                                       // t_1 starts with '$'
-    __device__ Str t(int i) const { return Str{topic + ts[i - 1], te[i - 1] - ts[i - 1]}; }   // 1-based
-    // children of the node behind i matched levels, smallest first; kinds: 0 = "#", 1 = "+", 2 = t_{i+1}
-    __device__ int children(int i, int* kind) const {
-        const bool wild = !(i == 0 && sys);
-        int c = 0;
-        if (i < n) {
-            const uint8_t H = '#', P = '+';
-            const Str h{&H, 1}, pl{&P, 1};
-            const Str tx = t(i + 1);
-            // order "#" < "+" always; place t_{i+1} among them
-            const int ch = cmp(tx, h), cp = cmp(tx, pl);
-            if (!wild) {
-                kind[c++] = 2;
-            } else if (ch < 0) {
-                kind[c++] = 2; kind[c++] = 0; kind[c++] = 1;
-            } else if (ch == 0) {            // the topic level is literally "#" (not a valid topic, but keep the order total)
-                kind[c++] = 0; kind[c++] = 1;
-            } else if (cp < 0) {
-                kind[c++] = 0; kind[c++] = 2; kind[c++] = 1;
-            } else if (cp == 0) {
-                kind[c++] = 0; kind[c++] = 1;
+// yields the levels of a member after the tenant level, one per call; false once there are no more
+struct MemberLevels {
+    Levels bound, topic;   // the bound at its level 1, the topic at the completion's first level
+    int pre, div, dpos;
+    bool sys;
+    int i;                 // levels yielded so far
+    bool done;
+    __device__ bool next(Str* out) {
+        if (done) return false;
+        if (i < pre) {
+            *out = bound.next();
+        } else if (i == pre && div >= 0) {
+            *out = div == 2 ? Str{topic.s + dpos, topic.pos - 1 - dpos} : wild(div);
+            done = div == 0;
+        } else if (!topic.more()) {   // the full-length filter
+            done = true;
+            return false;
+        } else {
+            const Str tx = topic.peek();
+            if ((i == 0 && sys) || below_hash(tx)) {
+                topic.skip(tx);
+                *out = tx;
             } else {
-                kind[c++] = 0; kind[c++] = 1; kind[c++] = 2;
+                *out = wild(0);
+                done = true;
             }
-        } else if (wild) {
-            kind[c++] = 0;   // "#" matches the parent level
         }
-        return c;
+        i++;
+        return true;
     }
-    // smallest member in the subtree of the node behind i matched levels (path so far in m.plus)
-    __device__ Member complete(Member m, int i) const {
-        while (i < n) {
-            int kind[3];
-            const int c = children(i, kind);
-            (void) c;
-            if (kind[0] == 0) {
-                m.depth = i;
-                m.hash = true;
-                return m;
-            }
-            if (kind[0] == 1) m.plus |= 1ull << i;
-            i++;
-        }
-        m.depth = n;
-        m.hash = false;
-        return m;
-    }
-    __device__ Str level_of(const Member& m, int i, const uint8_t* H, const uint8_t* P) const {   // level i (1-based) of member m
-        if (m.hash && i == m.depth + 1) return Str{H, 1};
-        if ((m.plus >> (i - 1)) & 1ull) return Str{P, 1};
-        return t(i);
-    }
-    __device__ int levels_of(const Member& m) const { return m.depth + (m.hash ? 1 : 0); }
 };
 
-// least member >= bound (bound levels b[0..k) WITHOUT the tenant level); false: none
-__device__ bool seek(const Ctx& c, const uint8_t* bound, const int* bs, const int* be, int k, Member* out) {
-    const uint8_t H = '#', P = '+';
-    Member m{0ull, 0, false};
+// least member >= the bound whose level 1 `b` is at (the tenant levels are equal); false: none. *exact: the member is the bound
+__device__ bool seek(Levels t, Levels b, bool sys, Member* out, bool* exact) {
     int fb_depth = -1, fb_kind = 0;   // deepest level on the tight path with a child greater than the bound's level
-    uint64_t fb_plus = 0;
-    int i = 0;                         // matched levels so far (tight)
+    int fb_tpos = 0;                  // ... and the topic position of its level fb_depth + 1
+    int i = 0;                        // matched levels so far (tight)
+    *exact = false;
     while (true) {
-        if (i >= k) {                  // the bound is exhausted: everything below this node is >= it
-            *out = c.complete(m, i);
+        if (!b.more()) {              // the bound is exhausted: everything below this node is >= it
+            *out = Member{i, -1, 0, t.pos};
+            *exact = !t.more();       // the node itself is the full-length filter
             return true;
         }
-        const Str b{bound + bs[i], be[i] - bs[i]};
+        const Str bl = b.next();
+        const bool has_t = t.more();
+        const Str tx = has_t ? t.peek() : Str{t.s, 0};
         int kind[3];
-        const int nc = c.children(i, kind);
+        const int nc = children(!(i == 0 && sys), has_t, tx, kind);
         int eq = -1, gt = -1;
         for (int j = 0; j < nc; j++) {
-            const Str s = kind[j] == 0 ? Str{&H, 1} : kind[j] == 1 ? Str{&P, 1} : c.t(i + 1);
-            const int r = cmp(s, b);
+            const int r = cmp(kind[j] == 2 ? tx : wild(kind[j]), bl);
             if (r == 0) eq = kind[j];
             else if (r > 0 && gt < 0) gt = kind[j];
         }
         if (gt >= 0) {
             fb_depth = i;
             fb_kind = gt;
-            fb_plus = m.plus;
+            fb_tpos = t.pos;
         }
-        if (eq == 0) {                 // "#": terminal. Equal to the bound iff the bound ends here too, else it is a proper prefix (<)
-            if (i + 1 == k) {
-                m.depth = i;
-                m.hash = true;
-                *out = m;
+        if (eq == 0) {                // "#": terminal. Equal to the bound iff the bound ends here too, else it is a proper prefix (<)
+            if (!b.more()) {
+                *out = Member{i, 0, 0, 0};
+                *exact = true;
                 return true;
             }
             break;
         }
-        if (eq > 0) {
-            if (eq == 1) m.plus |= 1ull << i;
+        if (eq > 0) {                 // "+" or the topic level: both consume the topic level
+            t.skip(tx);
             i++;
-            if (i == c.n && i == k) {  // the full-length filter equals the bound
-                m.depth = c.n;
-                m.hash = false;
-                *out = m;
-                return true;
-            }
             continue;
         }
-        break;                         // no child equals the bound's level: leave the tight path
+        break;                        // no child equals the bound's level: leave the tight path
     }
     if (fb_depth < 0) return false;
-    m.plus = fb_plus;
     if (fb_kind == 0) {
-        m.depth = fb_depth;
-        m.hash = true;
-        *out = m;
+        *out = Member{fb_depth, 0, 0, 0};
         return true;
     }
-    if (fb_kind == 1) m.plus |= 1ull << fb_depth;
-    *out = c.complete(m, fb_depth + 1);
+    t.pos = fb_tpos;                  // "+" and the topic level exist only while the topic has a level fb_depth + 1
+    t.skip(t.peek());
+    *out = Member{fb_depth, fb_kind, fb_tpos, t.pos};
     return true;
 }
 
@@ -202,54 +205,38 @@ __global__ void __launch_bounds__(128) range_lookup_kernel(int64_t n_pairs, cons
     const int64_t ti = lo;
     const int tn = topic_tenant[ti];
     const int64_t cand = cand_off[tn] + (j - pair_off[ti]);
-    Ctx c;
-    c.topic = topics + topic_off[ti];
+    const uint8_t* topic = topics + topic_off[ti];
     const int tlen = (int) (topic_off[ti + 1] - topic_off[ti]);
-    c.n = split(c.topic, tlen, '/', c.ts, c.te);
-    c.sys = tlen > 0 && c.topic[0] == '$';
-    const uint8_t* fb = first_blob + first_off[cand];
-    const uint8_t* lb = last_blob + last_off[cand];
-    int fs[RL_MAX_LEVELS], fe[RL_MAX_LEVELS], ls[RL_MAX_LEVELS], le[RL_MAX_LEVELS];
-    const int fk = split(fb, (int) (first_off[cand + 1] - first_off[cand]), 0, fs, fe);
-    const int lk = split(lb, (int) (last_off[cand + 1] - last_off[cand]), 0, ls, le);
-    if (c.n > RL_MAX_LEVELS || fk > RL_MAX_LEVELS || lk > RL_MAX_LEVELS) {
-        out[j] = 3;   // unsupported depth: reported to the caller as an error
-        return;
-    }
+    const bool sys = tlen > 0 && topic[0] == '$';
+    const Levels t{topic, tlen, 0, '/'};
+    Levels f{first_blob + first_off[cand], (int) (first_off[cand + 1] - first_off[cand]), 0, 0};
+    Levels l{last_blob + last_off[cand], (int) (last_off[cand + 1] - last_off[cand]), 0, 0};
     const Str tenant{tenants + tenant_off[tn], (int) (tenant_off[tn + 1] - tenant_off[tn])};
     // level 0 is the tenant id: every member starts with it
-    Member m;
-    const int r0 = cmp(tenant, Str{fb + fs[0], fe[0] - fs[0]});
+    const int r0 = cmp(tenant, f.next());
     if (r0 < 0) {
         out[j] = 2;   // the bound's tenant sorts behind this tenant: nothing >= first
         return;
     }
-    bool found;
-    if (r0 > 0) {
-        m = c.complete(Member{0ull, 0, false}, 0);   // every member is greater: the smallest one
-        found = true;
-    } else {
-        found = seek(c, fb, fs + 1, fe + 1, fk - 1, &m);
-    }
-    if (!found) {
+    Member m{0, -1, 0, 0};   // r0 > 0: every member is greater, so the smallest one
+    bool exact = false;
+    if (r0 == 0 && !seek(t, f, sys, &m, &exact)) {
         out[j] = 2;
         return;
     }
     // found == first, or found <= last (level-wise)
-    const uint8_t H = '#', P = '+';
-    const int ml = c.levels_of(m);
-    bool equal_first = r0 == 0 && ml == fk - 1;
-    for (int i = 1; equal_first && i <= ml; i++) equal_first = cmp(c.level_of(m, i, &H, &P), Str{fb + fs[i], fe[i] - fs[i]}) == 0;
-    int r = cmp(tenant, Str{lb + ls[0], le[0] - ls[0]});
-    for (int i = 1; r == 0; i++) {
-        const bool me = i > ml, le_ = i > lk - 1;
+    int r = cmp(tenant, l.next());
+    MemberLevels g{f, Levels{topic, tlen, m.tail, '/'}, m.pre, m.div, m.dpos, sys, 0, false};
+    while (r == 0) {
+        Str ml;
+        const bool me = !g.next(&ml), le_ = !l.more();
         if (me || le_) {
             r = me && le_ ? 0 : (me ? -1 : 1);
             break;
         }
-        r = cmp(c.level_of(m, i, &H, &P), Str{lb + ls[i], le[i] - ls[i]});
+        r = cmp(ml, l.next());
     }
-    out[j] = (equal_first || r <= 0) ? 1 : 0;
+    out[j] = (exact || r <= 0) ? 1 : 0;
 }
 
 int32_t rl_fail(int32_t code, const std::string& msg) { return bfq::set_error(code, msg); }
@@ -323,7 +310,6 @@ extern "C" int32_t bfq_range_lookup(int32_t device_ordinal, const uint8_t* tenan
         for (int64_t k = 0; k < cand_off[t + 1] - cand_off[t]; k++) {
             uint8_t& cell = keep_out[keep_off_out[i] + k];
             const uint8_t fl = cand_flags[cand_off[t] + k];
-            if (cell == 3) return rl_fail(BFQ_E_RANGE, "a topic or a range bound has more levels than bfq_range_lookup handles");
             if (stopped) {
                 cell = 0;
             } else if (!(fl & 1)) {

@@ -251,6 +251,9 @@ int32_t bfq_expand_device(const bfq_device_result* res, int64_t* d_offsets, int6
  *                                     1 = the range is returned by the reference's lookup, 0 = it is not
  * Semantics are the reference's loop, literally: no Fact -> kept; a Fact without first or last -> empty range, skipped; the
  * first range whose seek runs past the end of the expansion set ends the scan. Stateless; needs a CUDA device.
+ * Depth: there is no level limit. A topic (up to MaxTopicLength) and a bound may have any number of levels; each thread reads
+ * them through cursors and keeps no per-level state, so a deep topic in a batch costs time in its own rows only.
+ * Errors: BFQ_E_INVALID for a NULL array the call needs, BFQ_E_RANGE for a topic_tenant outside [0, n_tenants).
  * ---------------------------------------------------------------------------------------------- */
 int32_t bfq_range_lookup(int32_t device_ordinal, const uint8_t* tenants, const int64_t* tenant_off, int32_t n_tenants,
                          const uint8_t* topics, const int64_t* topic_off, const int32_t* topic_tenant, int64_t n_topics,
