@@ -4,7 +4,8 @@ this package is the thin host-side mirror of the reference's Java interfaces use
 """
 from ._native import NativeError, lib, load_library  # noqa: F401
 from .matcher import (GpuRouteIndex, GpuTenantRouteMatcher, GroupFanoutThrottled, MatchedRoutes,  # noqa: F401
-                      PersistentFanoutThrottled)
+                      OutOfTenantResource, PersistentFanoutBytesThrottled, PersistentFanoutThrottled, budget_events)
 
 __all__ = ["GpuRouteIndex", "GpuTenantRouteMatcher", "MatchedRoutes", "PersistentFanoutThrottled",
-           "GroupFanoutThrottled", "NativeError", "load_library", "lib"]
+           "GroupFanoutThrottled", "PersistentFanoutBytesThrottled", "OutOfTenantResource", "budget_events",
+           "NativeError", "load_library", "lib"]

@@ -44,6 +44,13 @@ class BfqFanoutResult(C.Structure):
                 ("n_pairs", C.c_int64), ("n_deliverers", C.c_int32), ("ordered_share_id", C.c_int32), ("generation", C.c_uint64)]
 
 
+class BfqBudgetResult(C.Structure):
+    _fields_ = [("d_delivered_persistent", C.c_void_p), ("d_topic_flags", C.c_void_p), ("n_delivered", C.c_int64),
+                ("n_dropped_bytes", C.c_int64), ("n_dropped_persistent_bandwidth", C.c_int64),
+                ("n_dropped_transient_bandwidth", C.c_int64)]
+
+
+BUDGET_BYTES_THROTTLED, BUDGET_NO_PERSISTENT_BW, BUDGET_NO_TRANSIENT_BW, BUDGET_METERED = 1, 2, 4, 8
 EXCHANGE_ID_BYTES, EXCHANGE_COUNTS, EXCHANGE_RANGES = 128, 1, 2
 _vp, _i32, _i64 = C.c_void_p, C.c_int32, C.c_int64
 _SIGNATURES = {
@@ -80,6 +87,7 @@ _SIGNATURES = {
     "bfq_device_result_wait": (_i32, [C.POINTER(BfqDeviceResult)]),
     "bfq_device_result_release": (None, [C.POINTER(BfqDeviceResult)]),
     "bfq_expand_device": (_i32, [C.POINTER(BfqDeviceResult), _vp, _vp, _i64, _vp, C.POINTER(_i64)]),
+    "bfq_expand_device_budget": (_i32, [C.POINTER(BfqDeviceResult), _vp, _vp, _vp, _vp, _vp, _i64, _vp, C.POINTER(BfqBudgetResult)]),
     "bfq_range_lookup": (_i32, [_i32, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bfq_fanout_device": (_i32, [C.POINTER(BfqDeviceResult), _vp, _vp, _i64, _vp, C.POINTER(BfqFanoutResult)]),
     "bfq_fanout_deliverer": (_i32, [_vp, _i32, C.POINTER(_i32), _vp, _i64, C.POINTER(_i64)]),

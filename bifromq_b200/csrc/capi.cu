@@ -173,6 +173,11 @@ struct Workspace {
     DevBuf<unsigned long long> d_counters;
     PinBuf<unsigned long long> h_counters;
     DevBuf<unsigned long long> d_exp_counts;
+    // delivery budgets (bfq_expand_device_budget)
+    DevBuf<long long> d_bud_bytes;
+    DevBuf<uint8_t> d_bud_bw, d_bud_flags;
+    DevBuf<uint32_t> d_bud_dp, d_bud_list;
+    DevBuf<unsigned long long> d_bud_ctr;
     // fan-out expansion (fanout.cu)
     DevBuf<uint32_t> d_fo_counts, d_fo_base, d_pack_topic, d_pack_rank, d_pack_member;
     DevBuf<long long> d_pack_offsets;
@@ -207,6 +212,7 @@ struct Workspace {
         d_ranges.release(); d_scratch.release();
         d_throttled.release(); d_counters.release(); h_counters.release();
         d_ord_keys.release(); d_leader.release(); d_order.release(); d_hash_tab.release(); d_hist.release();
+        d_bud_bytes.release(); d_bud_bw.release(); d_bud_flags.release(); d_bud_dp.release(); d_bud_list.release(); d_bud_ctr.release();
         d_fo_counts.release(); d_fo_base.release(); d_pack_topic.release(); d_pack_rank.release(); d_pack_member.release();
         d_pack_offsets.release(); d_fo_tmp.release();
         h_span_begin.release(); h_span_count.release(); h_route_count.release(); h_ranges.release(); h_throttled.release();
@@ -2044,21 +2050,16 @@ int32_t bfq_match_device(bfq_index* h, const uint8_t* tenants, const int64_t* te
     return rc;
 }
 
-int32_t bfq_expand_device(const bfq_device_result* res, int64_t* d_offsets, int64_t* d_ranks, int64_t rank_cap, void* stream,
-                          int64_t* n_ranks) {
-    if (!res || !res->lease || !d_offsets) return fail(BFQ_E_INVALID, "bad argument");
-    auto* L = static_cast<DeviceLease*>(res->lease);
-    if (!L->done || L->rc != BFQ_OK) return fail(BFQ_E_STATE, "bfq_expand_device needs a completed match (bfq_device_result_wait)");
-    bfq_index* h = L->h;
-    Workspace* w = L->ws;
+}  // extern "C"
+
+namespace {
+// the expand's inputs for a completed device match (its workspace, snapshot and caps) and the caller's CSR outputs
+ExpandParams expand_params(const DeviceLease* L, int64_t* d_offsets, int64_t* d_ranks, int64_t rank_cap) {
+    const Workspace* w = L->ws;
     const Snapshot* s = L->snap.get();
-    const int64_t n_topics = L->n;
-    CUDA_TRY(cudaSetDevice(h->device));
-    cudaStream_t st = (cudaStream_t) stream;
     const size_t nt = (size_t) std::max(L->ctx.n_tenants, 1);
-    CUDA_TRY(w->d_exp_counts.reserve((size_t) n_topics + 1));
     ExpandParams p{};
-    p.n_topics = n_topics;
+    p.n_topics = L->n;
     p.span_begin = w->d_span_begin.p;
     p.span_count = w->d_span_count.p;
     p.route_count = w->d_route_count.p;
@@ -2077,6 +2078,24 @@ int32_t bfq_expand_device(const bfq_device_result* res, int64_t* d_offsets, int6
     p.rkind = s->d_rkind.p;
     p.pfx_persistent = s->d_pfxP.p;
     p.pfx_group = s->d_pfxG.p;
+    return p;
+}
+}  // namespace
+
+extern "C" {
+
+int32_t bfq_expand_device(const bfq_device_result* res, int64_t* d_offsets, int64_t* d_ranks, int64_t rank_cap, void* stream,
+                          int64_t* n_ranks) {
+    if (!res || !res->lease || !d_offsets) return fail(BFQ_E_INVALID, "bad argument");
+    auto* L = static_cast<DeviceLease*>(res->lease);
+    if (!L->done || L->rc != BFQ_OK) return fail(BFQ_E_STATE, "bfq_expand_device needs a completed match (bfq_device_result_wait)");
+    bfq_index* h = L->h;
+    Workspace* w = L->ws;
+    const int64_t n_topics = L->n;
+    CUDA_TRY(cudaSetDevice(h->device));
+    cudaStream_t st = (cudaStream_t) stream;
+    CUDA_TRY(w->d_exp_counts.reserve((size_t) n_topics + 1));
+    const ExpandParams p = expand_params(L, d_offsets, d_ranks, rank_cap);
     size_t tmp_bytes = 0;
     CUDA_TRY(launch_expand(p, nullptr, &tmp_bytes, st, 1));
     CUDA_TRY(w->d_scan_tmp.reserve(tmp_bytes + 256));
@@ -2092,6 +2111,77 @@ int32_t bfq_expand_device(const bfq_device_result* res, int64_t* d_offsets, int6
     }
     std::lock_guard<std::mutex> g(h->mu);
     h->launches += launches;
+    return BFQ_OK;
+}
+
+int32_t bfq_expand_device_budget(const bfq_device_result* res, const int32_t* d_msg_bytes, const int64_t* max_pfanout_bytes,
+                                 const uint8_t* tenant_bandwidth, int64_t* d_offsets, int64_t* d_ranks, int64_t rank_cap,
+                                 void* stream, bfq_budget_result* out) {
+    if (!res || !res->lease || !d_offsets || !out) return fail(BFQ_E_INVALID, "bad argument");
+    auto* L = static_cast<DeviceLease*>(res->lease);
+    if (!L->done || L->rc != BFQ_OK) return fail(BFQ_E_STATE, "bfq_expand_device_budget needs a completed match (bfq_device_result_wait)");
+    const int64_t n_topics = L->n;
+    const int32_t n_tenants = L->ctx.n_tenants;
+    if (n_topics > 0 && !d_msg_bytes) return fail(BFQ_E_INVALID, "NULL d_msg_bytes");
+    if (n_tenants > 0 && (!max_pfanout_bytes || !tenant_bandwidth)) return fail(BFQ_E_INVALID, "NULL per-tenant budget table");
+    for (int32_t i = 0; i < n_tenants; i++)
+        if (max_pfanout_bytes[i] <= 0)
+            return fail(BFQ_E_INVALID, "max_pfanout_bytes[" + std::to_string(i) + "] = " + std::to_string(max_pfanout_bytes[i]) +
+                                           ": MaxPersistentFanoutBytes must be > 0");
+    bfq_index* h = L->h;
+    Workspace* w = L->ws;
+    CUDA_TRY(cudaSetDevice(h->device));
+    cudaStream_t st = (cudaStream_t) stream;
+    const size_t nn = (size_t) std::max<int64_t>(n_topics, 1), nt = (size_t) std::max(n_tenants, 1);
+    CUDA_TRY(w->d_exp_counts.reserve(nn + 1));
+    CUDA_TRY(w->d_bud_bytes.reserve(nt));
+    CUDA_TRY(w->d_bud_bw.reserve(nt));
+    CUDA_TRY(w->d_bud_flags.reserve(nn));
+    CUDA_TRY(w->d_bud_dp.reserve(nn));
+    CUDA_TRY(w->d_bud_list.reserve(nn));
+    CUDA_TRY(w->d_bud_ctr.reserve(BUD_CTR_COUNT));
+    if (n_tenants > 0) {
+        CUDA_TRY(cudaMemcpyAsync(w->d_bud_bytes.p, max_pfanout_bytes, (size_t) n_tenants * sizeof(long long), cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(w->d_bud_bw.p, tenant_bandwidth, (size_t) n_tenants, cudaMemcpyHostToDevice, st));
+    }
+    CUDA_TRY(cudaMemsetAsync(w->d_bud_ctr.p, 0, BUD_CTR_COUNT * sizeof(unsigned long long), st));
+    BudgetParams q{};
+    q.e = expand_params(L, d_offsets, d_ranks, rank_cap);
+    q.n_tenants = n_tenants;
+    q.msg_bytes = d_msg_bytes;
+    q.max_bytes = w->d_bud_bytes.p;
+    q.bandwidth = w->d_bud_bw.p;
+    q.delivered_p = w->d_bud_dp.p;
+    q.flags = w->d_bud_flags.p;
+    q.list = w->d_bud_list.p;
+    q.ctr = w->d_bud_ctr.p;
+    size_t tmp_bytes = 0;
+    CUDA_TRY(launch_budget(q, nullptr, &tmp_bytes, st, 1));
+    CUDA_TRY(w->d_scan_tmp.reserve(tmp_bytes + 256));
+    CUDA_TRY(launch_budget(q, w->d_scan_tmp.p, &tmp_bytes, st, 1));
+    long long total = 0;
+    unsigned long long ctr[BUD_CTR_COUNT];
+    CUDA_TRY(cudaMemcpyAsync(&total, d_offsets + n_topics, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(ctr, w->d_bud_ctr.p, sizeof(ctr), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    int64_t launches = 2;
+    const bool ok = ctr[BUD_BAD_SIZE] == 0;
+    if (ok && d_ranks && total <= rank_cap) {
+        q.n_listed = (int64_t) ctr[BUD_LISTED];
+        CUDA_TRY(launch_budget(q, w->d_scan_tmp.p, &tmp_bytes, st, 2));
+        launches += 2;
+    }
+    {
+        std::lock_guard<std::mutex> g(h->mu);
+        h->launches += launches;
+    }
+    if (!ok) return fail(BFQ_E_INVALID, std::to_string(ctr[BUD_BAD_SIZE]) + " negative d_msg_bytes entries");
+    out->d_delivered_persistent = w->d_bud_dp.p;
+    out->d_topic_flags = w->d_bud_flags.p;
+    out->n_delivered = (int64_t) total;
+    out->n_dropped_bytes = (int64_t) ctr[BUD_DROP_BYTES];
+    out->n_dropped_persistent_bandwidth = (int64_t) ctr[BUD_DROP_PBW];
+    out->n_dropped_transient_bandwidth = (int64_t) ctr[BUD_DROP_TBW];
     return BFQ_OK;
 }
 

@@ -983,11 +983,16 @@ __global__ void __launch_bounds__(256) expand_plain_kernel(const ExpandParams p)
             pos += count;
         });
 }
+// Writes topic t's ranks that survive a persistent cap maxP and a group cap maxG (KV order, the classification of
+// caps_kernel), dropping transient routes too if drop_t. One CTA of CAPS_THREADS per topic.
+__device__ __forceinline__ void copy_capped(const ExpandParams& p, uint32_t t, uint64_t maxP, uint64_t maxG, bool drop_t);
 // one CTA per cap-flagged topic: same classification as caps_kernel, the survivors are written
 __global__ void __launch_bounds__(CAPS_THREADS) expand_flagged_kernel(const ExpandParams p) {
     const uint32_t t = p.flagged_list[blockIdx.x];
     const int tenant = p.topic_tenant[t];
-    const uint64_t maxP = (uint64_t) max(p.max_pfanout[tenant], 0), maxG = (uint64_t) max(p.max_gfanout[tenant], 0);
+    copy_capped(p, t, (uint64_t) max(p.max_pfanout[tenant], 0), (uint64_t) max(p.max_gfanout[tenant], 0), false);
+}
+__device__ __forceinline__ void copy_capped(const ExpandParams& p, uint32_t t, uint64_t maxP, uint64_t maxG, bool drop_t) {
     SegIter it{p.ranges + p.span_begin[t], p.segs, p.span_count[t] & SPAN_COUNT_MASK};
     __shared__ unsigned long long cursor;
     if (threadIdx.x == 0) cursor = 0;
@@ -1006,7 +1011,8 @@ __global__ void __launch_bounds__(CAPS_THREADS) expand_flagged_kernel(const Expa
             for (uint32_t r = first; r < first + count; r++) {
                 const uint8_t kind = p.rkind[r];
                 const bool drop = (kind == 1 && baseP + (p.pfx_persistent[r] - p.pfx_persistent[first]) >= maxP) ||
-                                  (kind == 2 && baseG + (p.pfx_group[r] - p.pfx_group[first]) >= maxG);
+                                  (kind == 2 && baseG + (p.pfx_group[r] - p.pfx_group[first]) >= maxG) ||
+                                  (kind == 0 && drop_t);
                 if (!drop) {
                     const unsigned long long k = atomicAdd(&cursor, 1ull);
                     if (base + (int64_t) k < p.rank_cap) p.ranks[base + k] = (int64_t) r;
@@ -1014,6 +1020,108 @@ __global__ void __launch_bounds__(CAPS_THREADS) expand_flagged_kernel(const Expa
             }
         });
     }
+}
+
+// ------------------------------------------------------------------------------------------------ delivery budgets
+// DeliverExecutorGroup.submit (bifromq-dist-worker .../DeliverExecutorGroup.java:112-231) over a topic's surviving routes R
+// (the match's caps applied): |R| <= 1 is delivered as is; otherwise groups are delivered, transient routes only with
+// transient bandwidth, and persistent routes only with persistent bandwidth and while sent * s < MaxPersistentFanoutBytes:
+// the first k = min(P, ceil(B / s)) of them in KV order (all P when s == 0).
+// One warp per topic: |R|, P and G from the prefix counts over the topic's ranges, then k, the flags and the delivered count.
+__global__ void __launch_bounds__(256) budget_pass_kernel(const BudgetParams q) {
+    const ExpandParams& p = q.e;
+    const int lane = threadIdx.x & 31;
+    const int64_t t = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (t >= p.n_topics) {
+        if (t == p.n_topics && lane == 0) p.counts[t] = 0;
+        return;
+    }
+    const uint32_t sc = p.span_count[t];
+    SegIter it{p.ranges + p.span_begin[t], p.segs, sc & SPAN_COUNT_MASK};
+    uint64_t n = 0, np = 0, ng = 0;
+    for (uint32_t j = lane; j < it.n; j += 32)
+        it.for_range(j, [&](uint32_t first, uint32_t count) {
+            n += count;
+            np += p.pfx_persistent[first + count] - p.pfx_persistent[first];
+            ng += p.pfx_group[first + count] - p.pfx_group[first];
+        });
+    for (int o = 16; o > 0; o >>= 1) {
+        n += __shfl_xor_sync(0xFFFFFFFFu, n, o);
+        np += __shfl_xor_sync(0xFFFFFFFFu, np, o);
+        ng += __shfl_xor_sync(0xFFFFFFFFu, ng, o);
+    }
+    if (lane != 0) return;
+    const int32_t s = q.msg_bytes[t];
+    if (s < 0) atomicAdd(&q.ctr[BUD_BAD_SIZE], 1ull);
+    const int tenant = p.topic_tenant[t];
+    const bool known = tenant >= 0 && tenant < q.n_tenants;   // an unknown tenant matches nothing
+    uint64_t P = np, G = ng;
+    if ((sc & SPAN_FLAGGED) && known) {
+        P = min(P, (uint64_t) max(p.max_pfanout[tenant], 0));
+        G = min(G, (uint64_t) max(p.max_gfanout[tenant], 0));
+    }
+    const uint64_t T = n - np - ng, R = T + P + G;
+    uint64_t k = P, tdel = T;
+    uint8_t f = (R > 1 || P == 1) ? BUDGET_METERED : 0;
+    if (R > 1 && known) {
+        const uint8_t bw = q.bandwidth[tenant];
+        if (!(bw & 2) && T > 0) {
+            tdel = 0;
+            f |= BUDGET_NO_TRANSIENT_BW;
+            atomicAdd(&q.ctr[BUD_DROP_TBW], (unsigned long long) T);
+        }
+        if (!(bw & 1)) {
+            if (P > 0) {
+                k = 0;
+                f |= BUDGET_NO_PERSISTENT_BW;
+                atomicAdd(&q.ctr[BUD_DROP_PBW], (unsigned long long) P);
+            }
+        } else if (s > 0) {
+            // ceil(B / s) without overflow (B >= 1): the number of sends for which sent * s < B still held
+            const uint64_t m = ((uint64_t) q.max_bytes[tenant] - 1) / (uint64_t) s + 1;
+            if (m < P) {
+                k = m;
+                f |= BUDGET_BYTES_THROTTLED;
+                atomicAdd(&q.ctr[BUD_DROP_BYTES], (unsigned long long) (P - m));
+            }
+        }
+        if (f & BUDGET_DROPS) q.list[atomicAdd(&q.ctr[BUD_LISTED], 1ull)] = (uint32_t) t;
+    }
+    p.counts[t] = tdel + k + G;
+    q.delivered_p[t] = (uint32_t) k;
+    q.flags[t] = f;
+}
+// one warp per topic the budget and the caps leave whole
+__global__ void __launch_bounds__(256) budget_plain_kernel(const BudgetParams q) {
+    const ExpandParams& p = q.e;
+    const int lane = threadIdx.x & 31;
+    const int64_t t = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (t >= p.n_topics || (p.span_count[t] & SPAN_FLAGGED) || (q.flags[t] & BUDGET_DROPS)) return;
+    SegIter it{p.ranges + p.span_begin[t], p.segs, p.span_count[t] & SPAN_COUNT_MASK};
+    int64_t pos = p.offsets[t];
+    for (uint32_t j = 0; j < it.n; j++)
+        it.for_range(j, [&](uint32_t first, uint32_t count) {
+            for (uint32_t x = lane; x < count; x += 32)
+                if (pos + x < p.rank_cap) p.ranks[pos + x] = (int64_t) first + x;
+            pos += count;
+        });
+}
+// one CTA per cap-flagged topic (blocks [0, n_flagged)) and per budget-listed topic (the rest). A topic on both lists is
+// copied by its listed block only, under min(maxP, k): the match's cap and the budget keep KV-order prefixes of the same
+// persistent routes, so together they keep the shorter one.
+__global__ void __launch_bounds__(CAPS_THREADS) budget_capped_kernel(const BudgetParams q) {
+    const ExpandParams& p = q.e;
+    const bool listed = blockIdx.x >= p.n_flagged;
+    const uint32_t t = listed ? q.list[blockIdx.x - p.n_flagged] : p.flagged_list[blockIdx.x];
+    const uint8_t f = q.flags[t];
+    if (!listed && (f & BUDGET_DROPS)) return;
+    uint64_t maxP = listed ? q.delivered_p[t] : ~0ull, maxG = ~0ull;
+    if (p.span_count[t] & SPAN_FLAGGED) {
+        const int tenant = p.topic_tenant[t];
+        maxP = min(maxP, (uint64_t) max(p.max_pfanout[tenant], 0));
+        maxG = (uint64_t) max(p.max_gfanout[tenant], 0);
+    }
+    copy_capped(p, t, maxP, maxG, (f & BUDGET_NO_TRANSIENT_BW) != 0);
 }
 
 }  // namespace
@@ -1263,6 +1371,19 @@ cudaError_t launch_expand(const ExpandParams& p, void* d_scan_tmp, size_t* tmp_b
     }
     if (p.n_topics > 0) expand_plain_kernel<<<(unsigned) ((p.n_topics * 32 + 255) / 256), 256, 0, stream>>>(p);
     if (p.n_flagged > 0) expand_flagged_kernel<<<(unsigned) p.n_flagged, CAPS_THREADS, 0, stream>>>(p);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_budget(const BudgetParams& q, void* d_scan_tmp, size_t* tmp_bytes, cudaStream_t stream, int phase) {
+    const ExpandParams& p = q.e;
+    const int n1 = (int) p.n_topics + 1;
+    if (!d_scan_tmp) return cub::DeviceScan::ExclusiveSum(nullptr, *tmp_bytes, p.counts, reinterpret_cast<unsigned long long*>(p.offsets), n1, stream);
+    if (phase == 1) {
+        budget_pass_kernel<<<(unsigned) (((p.n_topics + 1) * 32 + 255) / 256), 256, 0, stream>>>(q);
+        return cub::DeviceScan::ExclusiveSum(d_scan_tmp, *tmp_bytes, p.counts, reinterpret_cast<unsigned long long*>(p.offsets), n1, stream);
+    }
+    if (p.n_topics > 0) budget_plain_kernel<<<(unsigned) ((p.n_topics * 32 + 255) / 256), 256, 0, stream>>>(q);
+    if (p.n_flagged + q.n_listed > 0) budget_capped_kernel<<<(unsigned) (p.n_flagged + q.n_listed), CAPS_THREADS, 0, stream>>>(q);
     return cudaGetLastError();
 }
 

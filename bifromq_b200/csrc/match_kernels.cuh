@@ -114,6 +114,38 @@ struct ExpandParams {
 // phase 2 = write the ranks (unordered within a topic). tmp as for launch_compact.
 cudaError_t launch_expand(const ExpandParams& p, void* d_scan_tmp, size_t* tmp_bytes, cudaStream_t stream, int phase);
 
+// Delivery budgets of DeliverExecutorGroup.submit on top of the expand (bfq_expand_device_budget): per topic a tighter
+// persistent cap k (MaxPersistentFanoutBytes, persistent bandwidth) and an on/off switch for transient routes.
+enum : uint8_t {
+    BUDGET_BYTES_THROTTLED = 1,      // k < P persistent routes delivered: PersistentFanoutBytesThrottled
+    BUDGET_NO_PERSISTENT_BW = 2,     // persistent routes dropped: OutOfTenantResource(TotalPersistentFanOutBytesPerSeconds)
+    BUDGET_NO_TRANSIENT_BW = 4,      // transient routes dropped: OutOfTenantResource(TotalTransientFanOutBytesPerSeconds)
+    BUDGET_METERED = 8,              // the topic records MqttPersistentFanOutBytes (|R| > 1, or one persistent route)
+    BUDGET_DROPS = 7,                // any of the first three: the topic's survivors are copied rank by rank
+};
+enum : int {
+    BUD_LISTED = 0,                  // topics in BudgetParams::list
+    BUD_BAD_SIZE = 1,                // topics with a negative message size
+    BUD_DROP_BYTES = 2,              // persistent routes dropped by the bytes budget
+    BUD_DROP_PBW = 3,                // ... by the persistent bandwidth switch
+    BUD_DROP_TBW = 4,                // transient routes dropped by the transient bandwidth switch
+    BUD_CTR_COUNT = 8,
+};
+struct BudgetParams {
+    ExpandParams e;                  // the match's CSR inputs and the expand's outputs (e.counts / e.offsets / e.ranks)
+    int32_t n_tenants;
+    const int32_t* msg_bytes;        // [n_topics] message size of each topic position
+    const long long* max_bytes;      // [n_tenants] MaxPersistentFanoutBytes (> 0)
+    const uint8_t* bandwidth;        // [n_tenants] bit 0: persistent bandwidth, bit 1: transient bandwidth
+    uint32_t* delivered_p;           // out [n_topics] persistent routes delivered (k)
+    uint8_t* flags;                  // out [n_topics] BUDGET_* bits
+    uint32_t* list;                  // out: topics with a BUDGET_DROPS bit
+    int64_t n_listed;                // phase 2: entries of list (read back after phase 1)
+    unsigned long long* ctr;         // [BUD_CTR_COUNT], zeroed before phase 1
+};
+// phase 1 = budget pass (counts, flags, list) + exclusive scan into e.offsets; phase 2 = write the delivered ranks
+cudaError_t launch_budget(const BudgetParams& q, void* d_scan_tmp, size_t* tmp_bytes, cudaStream_t stream, int phase);
+
 // Locality ordering + de-duplication for tier 0, all own kernels (no library sort):
 //   prep     one thread per topic: 64-bit hash of (tenant, topic bytes) -> insert into an open-addressing table; the first
 //            inserter of a (tenant, topic) pair is its LEADER, later identical ones (verified byte by byte) are followers that

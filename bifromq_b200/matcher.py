@@ -27,6 +27,34 @@ RANGE_MULTI = 0x80000000
 
 PersistentFanoutThrottled = namedtuple("PersistentFanoutThrottled", "tenant_id topic mqtt_topic_filter max_count")
 GroupFanoutThrottled = namedtuple("GroupFanoutThrottled", "tenant_id topic mqtt_topic_filter max_count")
+PersistentFanoutBytesThrottled = namedtuple("PersistentFanoutBytesThrottled", "tenant_id topic max_bytes")
+OutOfTenantResource = namedtuple("OutOfTenantResource", "reason tenant_id topic")
+PERSISTENT_BANDWIDTH = "TotalPersistentFanOutBytesPerSeconds"   # TenantResourceType names, the reason OutOfTenantResource carries
+TRANSIENT_BANDWIDTH = "TotalTransientFanOutBytesPerSeconds"
+
+
+def budget_events(tenants, topics, topic_tenant, flags, delivered_persistent, msg_bytes, max_pfanout_bytes):
+    """The events and meter values of a bfq_expand_device_budget result, as DeliverExecutorGroup.submit reports them.
+    flags / delivered_persistent: the result's per-topic arrays copied to the host; msg_bytes: the sizes passed to the call.
+    -> (events, meter): events in topic order, for each topic PersistentFanoutBytesThrottled, then OutOfTenantResource for
+    persistent, then for transient bandwidth; meter = [(topic position, MqttPersistentFanOutBytes value)] for every topic
+    the reference records it for (zero values included). The reference reports OutOfTenantResource once per publisher of
+    the message pack (with its ClientInfo): repeating each one per publisher is the caller's job."""
+    events, meter = [], []
+    flags = np.asarray(flags)
+    for t in np.flatnonzero(flags).tolist():
+        f = int(flags[t])
+        tenant = int(topic_tenant[t])
+        tid = tenants[tenant]
+        if f & N.BUDGET_BYTES_THROTTLED:
+            events.append(PersistentFanoutBytesThrottled(tid, topics[t], int(max_pfanout_bytes[tenant])))
+        if f & N.BUDGET_NO_PERSISTENT_BW:
+            events.append(OutOfTenantResource(PERSISTENT_BANDWIDTH, tid, topics[t]))
+        if f & N.BUDGET_NO_TRANSIENT_BW:
+            events.append(OutOfTenantResource(TRANSIENT_BANDWIDTH, tid, topics[t]))
+        if f & N.BUDGET_METERED:
+            meter.append((t, int(delivered_persistent[t]) * int(msg_bytes[t])))
+    return events, meter
 
 
 class BatchResult:
@@ -112,6 +140,19 @@ class DeviceResult:
         total = C.c_int64(0)
         N.check(N.lib.bfq_expand_device(C.byref(self.raw), d_offsets_ptr, d_ranks_ptr, rank_cap, stream, C.byref(total)))
         return total.value
+
+    def expand_budget(self, d_msg_bytes_ptr, max_pfanout_bytes, tenant_bandwidth, d_offsets_ptr, d_ranks_ptr, rank_cap, stream=0):
+        """bfq_expand_device_budget: device CSR of the routes DeliverExecutorGroup.submit delivers. d_msg_bytes_ptr: int32
+        message size per topic position (device); max_pfanout_bytes (MaxPersistentFanoutBytes) and tenant_bandwidth (bit 0
+        persistent, bit 1 transient bandwidth) per tenant of the match's tenant list. -> BfqBudgetResult; its per-topic
+        device arrays stay valid until release() or the next budget call on this result"""
+        mb = np.ascontiguousarray(max_pfanout_bytes, dtype=np.int64)
+        bw = np.ascontiguousarray(tenant_bandwidth, dtype=np.uint8)
+        out = N.BfqBudgetResult()
+        N.check(N.lib.bfq_expand_device_budget(C.byref(self.raw), d_msg_bytes_ptr, N.ptr(mb) if mb.size else None,
+                                               N.ptr(bw) if bw.size else None, d_offsets_ptr, d_ranks_ptr, rank_cap, stream,
+                                               C.byref(out)))
+        return out
 
     def fanout(self, d_offsets_ptr, d_ranks_ptr, n_pairs, stream=0):
         """bfq_fanout_device: the (topic, route) pairs of this result's device CSR grouped by deliverer id -> BfqFanoutResult

@@ -236,6 +236,50 @@ void bfq_device_result_release(bfq_device_result* res);
 int32_t bfq_expand_device(const bfq_device_result* res, int64_t* d_offsets, int64_t* d_ranks, int64_t rank_cap,
                           void* stream, int64_t* n_ranks);
 
+/* Delivery budgets of DeliverExecutorGroup.submit (DW/DeliverExecutorGroup.java:112-231) applied to a completed device match:
+ * the same device CSR as bfq_expand_device, holding only the routes that are actually DELIVERED. It goes unchanged into
+ * bfq_fanout_device. Per tenant i of the match's tenant list the host supplies max_pfanout_bytes[i]
+ * (Setting.MaxPersistentFanoutBytes, > 0) and tenant_bandwidth[i] (bit 0: resourceThrottler.hasResource(tenant,
+ * TotalPersistentFanOutBytesPerSeconds), bit 1: the same for TotalTransientFanOutBytesPerSeconds); per topic position t,
+ * d_msg_bytes[t] (device, SizeUtil.estSizeOf of the topic's TopicMessagePack, >= 0). Repeated topics may carry different sizes.
+ * For topic t with surviving routes R (the match's caps applied), kinds as in bfq_route_kind, P of them persistent:
+ *   |R| <= 1       delivered whatever the budgets say (the reference's single-route branch)
+ *   |R| > 1        groups: all delivered, no budget applies (a group of persistent members does not count toward the bytes)
+ *                  transient: all delivered with transient bandwidth, else none (flag BFQ_BUDGET_NO_TRANSIENT_BW if any)
+ *                  persistent: without persistent bandwidth none (flag BFQ_BUDGET_NO_PERSISTENT_BW if P > 0); with it the
+ *                  first k = min(P, ceil(B / s)) in KV (rank) order, k = P if s == 0: the sends for which sent * s < B held
+ *                  (flag BFQ_BUDGET_BYTES_THROTTLED iff k < P). Computed without overflow for any B <= 2^63 - 1, s <= 2^31 - 1.
+ * The reference iterates a hash set, so WHICH k persistent routes it sends is unspecified; this call fixes it to KV order,
+ * the rule of the match's own caps, so results are reproducible. With the match's caps applied first, submit's count checks
+ * (MaxPersistentFanout, MaxGroupFanout) never drop a route or fire an event, so the call takes no count inputs.
+ * What the host does with the result (the reference's events and meter):
+ *   BFQ_BUDGET_BYTES_THROTTLED    report PersistentFanoutBytesThrottled(tenantId, topic, maxBytes) once for the topic
+ *   BFQ_BUDGET_NO_*_BW            report OutOfTenantResource(reason) once per PUBLISHER of the topic's message pack
+ *   BFQ_BUDGET_METERED            record MqttPersistentFanOutBytes = d_delivered_persistent[t] * s (zero included); set for
+ *                                 |R| > 1 and for a single persistent route
+ * The match result is not touched: route_count, throttled and the BatchDistReply fan-out count stay the match's.
+ * Sizing and writing follow bfq_expand_device: d_offsets[n_topics + 1] is always written, d_ranks only if the total fits
+ * rank_cap (d_ranks = NULL only sizes), ranks are unordered within a topic and resolve against the result's own snapshot.
+ * The per-topic arrays live in the result's leased workspace until bfq_device_result_release (the next budget call on the
+ * same result overwrites them). The call synchronises `stream` once (to read the total and the size check).
+ * Errors: BFQ_E_INVALID for a NULL array the call needs, a max_pfanout_bytes[i] <= 0, or a negative d_msg_bytes entry (checked
+ * on the device; offsets are written, ranks are not); BFQ_E_STATE for a match that has not completed. */
+#define BFQ_BUDGET_BYTES_THROTTLED 1
+#define BFQ_BUDGET_NO_PERSISTENT_BW 2
+#define BFQ_BUDGET_NO_TRANSIENT_BW 4
+#define BFQ_BUDGET_METERED 8
+typedef struct {
+    const uint32_t* d_delivered_persistent;  /* [n_topics] persistent routes delivered (k; 1 or 0 when |R| <= 1) */
+    const uint8_t* d_topic_flags;            /* [n_topics] BFQ_BUDGET_* bits */
+    int64_t n_delivered;                     /* routes delivered = d_offsets[n_topics] */
+    int64_t n_dropped_bytes;                 /* persistent routes dropped by MaxPersistentFanoutBytes */
+    int64_t n_dropped_persistent_bandwidth;  /* persistent routes dropped for lack of persistent bandwidth */
+    int64_t n_dropped_transient_bandwidth;   /* transient routes dropped for lack of transient bandwidth */
+} bfq_budget_result;
+int32_t bfq_expand_device_budget(const bfq_device_result* res, const int32_t* d_msg_bytes, const int64_t* max_pfanout_bytes,
+                                 const uint8_t* tenant_bandwidth, int64_t* d_offsets, int64_t* d_ranks, int64_t rank_cap,
+                                 void* stream, bfq_budget_result* out);
+
 /* ------------------------------------------------------------------------------------------------
  * Batched range pruning on the dist-server side (SURVEY.md 8f): TenantRangeLookupCache.lookup
  * (bifromq-dist/bifromq-dist-server/src/main/java/org/apache/bifromq/dist/server/scheduler/TenantRangeLookupCache.java:70-106)
