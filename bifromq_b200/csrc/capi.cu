@@ -15,72 +15,12 @@
 
 #include "../../include/bfq_gpumatch.h"
 #include "codec.h"
+#include "cuda_buf.h"
 #include "index_builder.h"
 #include "fanout.h"
 #include "match_kernels.cuh"
 
 using namespace bfq;
-
-namespace bfq {
-thread_local std::string g_last_error;
-int32_t set_error(int32_t code, const std::string& msg) {
-    g_last_error = msg;
-    return code;
-}
-}  // namespace bfq
-
-namespace {
-
-int32_t fail(int32_t code, const std::string& msg) { return bfq::set_error(code, msg); }
-#define CUDA_TRY(expr)                                                                          \
-    do {                                                                                        \
-        cudaError_t _e = (expr);                                                                \
-        if (_e != cudaSuccess)                                                                  \
-            return fail(BFQ_E_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e));        \
-    } while (0)
-
-// growable device / pinned-host buffers
-template <typename T>
-struct DevBuf {
-    T* p = nullptr;
-    size_t cap = 0;
-    cudaError_t reserve(size_t n) {
-        if (n <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        cudaError_t e = cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T));
-        if (e == cudaSuccess) cap = n;
-        return e;
-    }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
-    size_t bytes() const { return cap * sizeof(T); }
-};
-template <typename T>
-struct PinBuf {
-    T* p = nullptr;
-    size_t cap = 0;
-    cudaError_t reserve(size_t n) {
-        if (n <= cap) return cudaSuccess;
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        cap = 0;
-        cudaError_t e = cudaMallocHost(&p, std::max<size_t>(n, 1) * sizeof(T));
-        if (e == cudaSuccess) cap = n;
-        return e;
-    }
-    void release() {
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        cap = 0;
-    }
-};
-
-}  // namespace
 
 // ------------------------------------------------------------------------------------------------ snapshots
 // One committed state of the index: device arrays + the host-side tables results are resolved against (segment table,
@@ -89,9 +29,9 @@ struct PinBuf {
 struct Snapshot {
     int device = 0;
     uint64_t generation = 0;
-    DevBuf<Slot> d_slots, d_roots;
-    DevBuf<uint32_t> d_segs, d_pfxP, d_pfxG;
-    DevBuf<uint8_t> d_rkind, d_tags;
+    DeviceBuf<Slot> d_slots, d_roots;
+    DeviceBuf<uint32_t> d_segs, d_pfxP, d_pfxG;
+    DeviceBuf<uint8_t> d_rkind, d_tags;
     FlatIndex flat;          // host copy (segs / tenant map / tenant table / statistics; the uploaded arrays are dropped)
     // per tenant, aligned with flat.tenants (key order): the committed KV (route lookups; shared with the staging area and
     // with the neighbouring snapshots, a delta commit replaces only the touched tenants') and the route kinds
@@ -102,10 +42,9 @@ struct Snapshot {
     };
     // fan-out tables of the whole snapshot (device), assembled from the tenants' on first use
     struct FanTable {
-        DevBuf<uint32_t> d_rdeliv, d_gmem_off, d_gmem_deliv;
-        DevBuf<uint8_t> d_gordered;
+        DeviceBuf<uint32_t> d_rdeliv, d_gmem_off, d_gmem_deliv;
+        DeviceBuf<uint8_t> d_gordered;
         uint32_t n_deliverers = 0;   // incl. the reserved last id (ordered shared subscriptions)
-        ~FanTable() { d_rdeliv.release(); d_gmem_off.release(); d_gmem_deliv.release(); d_gordered.release(); }
     };
     std::mutex fan_mu;
     std::shared_ptr<FanTable> fan;
@@ -129,10 +68,7 @@ struct Snapshot {
     int64_t device_bytes() const {
         return (int64_t) (d_slots.bytes() + d_tags.bytes() + d_roots.bytes() + d_segs.bytes() + d_rkind.bytes() + d_pfxP.bytes() + d_pfxG.bytes());
     }
-    ~Snapshot() {
-        cudaSetDevice(device);
-        d_slots.release(); d_roots.release(); d_segs.release(); d_pfxP.release(); d_pfxG.release(); d_rkind.release(); d_tags.release();
-    }
+    ~Snapshot() { cudaSetDevice(device); }   // runs before the members are destroyed: the buffers are freed on this device
 };
 
 constexpr int MAX_CHUNKS = 8;
@@ -154,38 +90,38 @@ struct Workspace {
     std::vector<int32_t> tab_caps;
     int32_t tab_n = -1;
     bool any_cap = true;
-    DevBuf<int32_t> d_tenant_tab;   // root | maxP | maxG, 3 x n_tenants
-    PinBuf<int32_t> h_tenant_tab;
+    DeviceBuf<int32_t> d_tenant_tab;   // root | maxP | maxG, 3 x n_tenants
+    PinnedBuf<int32_t> h_tenant_tab;
     // per-call device buffers
-    DevBuf<uint8_t> d_topics;
-    DevBuf<int64_t> d_topic_off;
-    DevBuf<int32_t> d_topic_tenant;
-    DevBuf<uint32_t> d_span_begin, d_span_count, d_route_count, d_overflow, d_flagged, d_kept, d_defer;
-    DevBuf<uint2> d_ranges, d_scratch, d_ranges_c;
-    DevBuf<uint8_t> d_scan_tmp;
-    DevBuf<uint32_t> d_cnt, d_new_begin, d_final_begin, d_final_count;
+    DeviceBuf<uint8_t> d_topics;
+    DeviceBuf<int64_t> d_topic_off;
+    DeviceBuf<int32_t> d_topic_tenant;
+    DeviceBuf<uint32_t> d_span_begin, d_span_count, d_route_count, d_overflow, d_flagged, d_kept, d_defer;
+    DeviceBuf<uint2> d_ranges, d_scratch, d_ranges_c;
+    DeviceBuf<uint8_t> d_scan_tmp;
+    DeviceBuf<uint32_t> d_cnt, d_new_begin, d_final_begin, d_final_count;
     // locality order + dedup (launch_order): per compute-stream slot (two sub-batches can be in flight)
-    DevBuf<uint32_t> d_ord_keys, d_leader, d_order;
-    DevBuf<unsigned long long> d_hash_tab;   // 2 x hash_stride
-    DevBuf<uint32_t> d_hist;                 // 2 x hist_stride (histogram + block totals/prefixes + ticket)
+    DeviceBuf<uint32_t> d_ord_keys, d_leader, d_order;
+    DeviceBuf<unsigned long long> d_hash_tab;   // 2 x hash_stride
+    DeviceBuf<uint32_t> d_hist;                 // 2 x hist_stride (launch_order's scratch)
     size_t hash_stride = 0, hist_stride = 0;
-    DevBuf<uint3> d_throttled;
-    DevBuf<unsigned long long> d_counters;
-    PinBuf<unsigned long long> h_counters;
-    DevBuf<unsigned long long> d_exp_counts;
+    DeviceBuf<uint3> d_throttled;
+    DeviceBuf<unsigned long long> d_counters;
+    PinnedBuf<unsigned long long> h_counters;
+    DeviceBuf<unsigned long long> d_exp_counts;
     // delivery budgets (bfq_expand_device_budget)
-    DevBuf<long long> d_bud_bytes;
-    DevBuf<uint8_t> d_bud_bw, d_bud_flags;
-    DevBuf<uint32_t> d_bud_dp, d_bud_list;
-    DevBuf<unsigned long long> d_bud_ctr;
+    DeviceBuf<long long> d_bud_bytes;
+    DeviceBuf<uint8_t> d_bud_bw, d_bud_flags;
+    DeviceBuf<uint32_t> d_bud_dp, d_bud_list;
+    DeviceBuf<unsigned long long> d_bud_ctr;
     // fan-out expansion (fanout.cu)
-    DevBuf<uint32_t> d_fo_counts, d_fo_base, d_pack_topic, d_pack_rank, d_pack_member;
-    DevBuf<long long> d_pack_offsets;
-    DevBuf<uint8_t> d_fo_tmp;
+    DeviceBuf<uint32_t> d_fo_counts, d_fo_base, d_pack_topic, d_pack_rank, d_pack_member;
+    DeviceBuf<long long> d_pack_offsets;
+    DeviceBuf<uint8_t> d_fo_tmp;
     // pinned result buffers
-    PinBuf<uint32_t> h_span_begin, h_span_count, h_route_count;
-    PinBuf<uint2> h_ranges;
-    PinBuf<uint3> h_throttled;
+    PinnedBuf<uint32_t> h_span_begin, h_span_count, h_route_count;
+    PinnedBuf<uint2> h_ranges;
+    PinnedBuf<uint3> h_throttled;
 
     cudaError_t init(int dev) {
         device = dev;
@@ -203,19 +139,7 @@ struct Workspace {
         return e;
     }
     ~Workspace() {
-        cudaSetDevice(device);
-        d_tenant_tab.release(); h_tenant_tab.release();
-        d_topics.release(); d_topic_off.release(); d_topic_tenant.release();
-        d_span_begin.release(); d_span_count.release(); d_route_count.release(); d_overflow.release();
-        d_flagged.release(); d_kept.release(); d_defer.release(); d_exp_counts.release(); d_ranges_c.release();
-        d_scan_tmp.release(); d_cnt.release(); d_new_begin.release(); d_final_begin.release(); d_final_count.release();
-        d_ranges.release(); d_scratch.release();
-        d_throttled.release(); d_counters.release(); h_counters.release();
-        d_ord_keys.release(); d_leader.release(); d_order.release(); d_hash_tab.release(); d_hist.release();
-        d_bud_bytes.release(); d_bud_bw.release(); d_bud_flags.release(); d_bud_dp.release(); d_bud_list.release(); d_bud_ctr.release();
-        d_fo_counts.release(); d_fo_base.release(); d_pack_topic.release(); d_pack_rank.release(); d_pack_member.release();
-        d_pack_offsets.release(); d_fo_tmp.release();
-        h_span_begin.release(); h_span_count.release(); h_route_count.release(); h_ranges.release(); h_throttled.release();
+        cudaSetDevice(device);   // the buffers are freed after this body, on this device
         for (auto& e : ev) if (e) cudaEventDestroy(e);
         for (auto& e : evk) if (e) cudaEventDestroy(e);
         for (auto& e : ev_h2d) if (e) cudaEventDestroy(e);
@@ -352,8 +276,8 @@ int32_t resolve_tenants(Workspace* w, const Snapshot* s, const uint8_t* tenants,
             same = w->tab_caps[i] == (max_p ? max_p[i] : 0x7FFFFFFF) && w->tab_caps[nt + i] == (max_g ? max_g[i] : 0x7FFFFFFF);
     }
     if (same) return BFQ_OK;
-    CUDA_TRY(w->h_tenant_tab.reserve(3 * nt));
-    CUDA_TRY(w->d_tenant_tab.reserve(3 * nt));
+    BFQ_CUDA_TRY(w->h_tenant_tab.reserve(3 * nt));
+    BFQ_CUDA_TRY(w->d_tenant_tab.reserve(3 * nt));
     w->tab_blob.assign(tenants ? tenants + (n_tenants ? tenant_off[0] : 0) : nullptr, tenants ? tenants + (n_tenants ? tenant_off[0] : 0) + blob_n : nullptr);
     w->tab_off.resize(nt + 1);
     w->tab_caps.assign(2 * nt, 0x7FFFFFFF);
@@ -373,7 +297,7 @@ int32_t resolve_tenants(Workspace* w, const Snapshot* s, const uint8_t* tenants,
     if (n_tenants > 0) w->tab_off[n_tenants] = tenant_off[n_tenants] - tenant_off[0];
     // the workspace is idle between calls, so nothing reads the pinned staging table while it is rewritten; the streams
     // that read the device table are ordered behind this copy (same stream, or through the H2D events of the host path)
-    CUDA_TRY(cudaMemcpyAsync(w->d_tenant_tab.p, w->h_tenant_tab.p, 3 * nt * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_tenant_tab.p, w->h_tenant_tab.p, 3 * nt * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
     w->tab_generation = s->generation;
     w->tab_n = n_tenants;
     w->any_cap = any_cap;
@@ -389,45 +313,42 @@ struct SubBatch {
     uint64_t dyn_off = 0, dyn_cap = 0;     // slice of ranges[n_total * INLINE_RANGES ...) for tiers 1/2
     uint64_t thr_off = 0, thr_cap = 0;     // slice of the throttled list
 };
-constexpr int32_t BFQ_RETRY_GROW = -100;
-// words of one ordering scratch slot: histogram | block totals | block prefixes | ticket (kept 256-byte aligned)
-size_t hist_words(size_t buckets) { return (buckets + 2 * (buckets / 4096) + 64 + 63) / 64 * 64; }   // internal: a slice was too small, redo the batch un-chunked with bigger buffers
+constexpr int32_t BFQ_RETRY_GROW = -100;   // internal: a slice was too small, redo the batch un-chunked with bigger buffers
 
 int32_t prepare_workspace(bfq_index* h, Workspace* w, int64_t n, int n_chunks, int32_t n_tenants) {
     const size_t nn = (size_t) std::max<int64_t>(n, 1);
     if (n >= (int64_t) 0x3FFFFFFF) return fail(BFQ_E_INVALID, "too many topics in one batch");
-    CUDA_TRY(w->d_span_begin.reserve(nn));
-    CUDA_TRY(w->d_span_count.reserve(nn));
-    CUDA_TRY(w->d_route_count.reserve(nn));
-    CUDA_TRY(w->d_overflow.reserve(nn));
-    CUDA_TRY(w->d_flagged.reserve(nn));
-    CUDA_TRY(w->d_kept.reserve(nn));
-    CUDA_TRY(w->d_defer.reserve(nn));
-    CUDA_TRY(w->d_counters.reserve(CTR_COUNT * MAX_CHUNKS));
-    CUDA_TRY(w->h_counters.reserve(CTR_COUNT * MAX_CHUNKS));
+    BFQ_CUDA_TRY(w->d_span_begin.reserve(nn));
+    BFQ_CUDA_TRY(w->d_span_count.reserve(nn));
+    BFQ_CUDA_TRY(w->d_route_count.reserve(nn));
+    BFQ_CUDA_TRY(w->d_overflow.reserve(nn));
+    BFQ_CUDA_TRY(w->d_flagged.reserve(nn));
+    BFQ_CUDA_TRY(w->d_kept.reserve(nn));
+    BFQ_CUDA_TRY(w->d_defer.reserve(nn));
+    BFQ_CUDA_TRY(w->d_counters.reserve(CTR_COUNT * MAX_CHUNKS));
+    BFQ_CUDA_TRY(w->h_counters.reserve(CTR_COUNT * MAX_CHUNKS));
     // ranges[0, n * INLINE_RANGES): tier-0 inline slots; the rest: cursor-allocated region of tiers 1 and 2
     const uint64_t dyn_base = (uint64_t) n * INLINE_RANGES;
     if (dyn_base >= 0xF0000000ull) return fail(BFQ_E_RANGE, "batch too large for 32-bit range indices; split the batch");
     const size_t min_dyn = std::max<size_t>((size_t) n_chunks << 18, nn);
-    if (w->d_ranges.cap < dyn_base + min_dyn) CUDA_TRY(w->d_ranges.reserve((size_t) (dyn_base + std::max<size_t>(1 << 20, min_dyn))));
+    if (w->d_ranges.cap < dyn_base + min_dyn) BFQ_CUDA_TRY(w->d_ranges.reserve((size_t) (dyn_base + std::max<size_t>(1 << 20, min_dyn))));
     const int64_t per_chunk = (n + n_chunks - 1) / n_chunks + 1;
     if (per_chunk >= h->order_min) {
-        CUDA_TRY(w->d_ord_keys.reserve(nn));
-        CUDA_TRY(w->d_leader.reserve(nn));
-        CUDA_TRY(w->d_order.reserve(nn));
-        const size_t buckets = order_hist_buckets(per_chunk, n_tenants);
-        const size_t hist_stride = hist_words(buckets);
+        BFQ_CUDA_TRY(w->d_ord_keys.reserve(nn));
+        BFQ_CUDA_TRY(w->d_leader.reserve(nn));
+        BFQ_CUDA_TRY(w->d_order.reserve(nn));
+        const size_t hist_stride = order_scratch_words(per_chunk, n_tenants);
         const size_t hash_stride = order_hash_entries(per_chunk);
         if (hist_stride > w->hist_stride) {
-            CUDA_TRY(w->d_hist.reserve(2 * hist_stride));
+            BFQ_CUDA_TRY(w->d_hist.reserve(2 * hist_stride));
             w->hist_stride = hist_stride;
         }
         if (hash_stride > w->hash_stride) {
-            CUDA_TRY(w->d_hash_tab.reserve(2 * hash_stride));
+            BFQ_CUDA_TRY(w->d_hash_tab.reserve(2 * hash_stride));
             w->hash_stride = hash_stride;
         }
     }
-    if (w->d_throttled.cap < ((size_t) n_chunks << 14)) CUDA_TRY(w->d_throttled.reserve(std::max<size_t>(1 << 16, (size_t) n_chunks << 14)));
+    if (w->d_throttled.cap < ((size_t) n_chunks << 14)) BFQ_CUDA_TRY(w->d_throttled.reserve(std::max<size_t>(1 << 16, (size_t) n_chunks << 14)));
     return BFQ_OK;
 }
 
@@ -506,7 +427,7 @@ CapsParams caps_params(const CoreCtx& c, const SubBatch& sb, const MatchParams& 
 
 bool wants_order(const CoreCtx& c, const SubBatch& sb) {
     return sb.n >= c.h->order_min && c.w->d_order.cap >= (size_t) (sb.begin + sb.n) && c.w->hist_stride > 0 &&
-           c.w->hist_stride >= hist_words(order_hist_buckets(sb.n, c.n_tenants)) && c.w->hash_stride >= order_hash_entries(sb.n);
+           c.w->hist_stride >= order_scratch_words(sb.n, c.n_tenants) && c.w->hash_stride >= order_hash_entries(sb.n);
 }
 
 // Enqueues one sub-batch on c.stream WITHOUT synchronising: [dedup + locality order] -> tier 0 -> tier 1 -> [followers] ->
@@ -526,13 +447,12 @@ int32_t enqueue_core(const CoreCtx& c, const SubBatch& sb, CoreOut* out) {
         cudaStreamSetAttribute(stream, cudaStreamAttributeAccessPolicyWindow, &attr);
         cudaGetLastError();
     }
-    CUDA_TRY(cudaMemsetAsync(p.counters, 0, CTR_COUNT * sizeof(unsigned long long), stream));
+    BFQ_CUDA_TRY(cudaMemsetAsync(p.counters, 0, CTR_COUNT * sizeof(unsigned long long), stream));
     bool ordered = false, dedup = false;
     if (wants_order(c, sb)) {
         // group the topics by tenant and leading levels so that neighbouring lanes walk the same part of the trie, and
         // match every distinct (tenant, topic) pair once
         const int slot = sb.chunk & 1;
-        const size_t buckets = order_hist_buckets(n, c.n_tenants);
         OrderParams q{};
         q.n_topics = n;
         q.topics = c.d_topics;
@@ -545,17 +465,10 @@ int32_t enqueue_core(const CoreCtx& c, const SubBatch& sb, CoreOut* out) {
         q.hash_tab = w->d_hash_tab.p + (size_t) slot * w->hash_stride;
         q.hash_mask = order_hash_entries(n) - 1;
         q.hist = w->d_hist.p + (size_t) slot * w->hist_stride;
-        q.blk_tot = q.hist + buckets;
-        q.blk_pfx = q.blk_tot + buckets / 4096;
-        q.ticket = q.blk_pfx + buckets / 4096;
-        q.hist_bits = 0;
-        while (((size_t) 1 << q.hist_bits) < buckets) q.hist_bits++;
         q.dedup = c.h->dedup ? 1 : 0;
         q.dedup_hash_mask = c.h->dedup_hash_bits >= 64 ? ~0ull : (1ull << c.h->dedup_hash_bits) - 1;
         q.counters = p.counters;
-        CUDA_TRY(cudaMemsetAsync(q.hist, 0, hist_words(buckets) * sizeof(uint32_t), stream));
-        if (q.dedup) CUDA_TRY(cudaMemsetAsync(q.hash_tab, 0xFF, ((size_t) q.hash_mask + 1) * sizeof(unsigned long long), stream));
-        CUDA_TRY(launch_order(q, stream));
+        BFQ_CUDA_TRY(launch_order(q, stream));
         p.order = q.order;
         p.order_count = p.counters + CTR_NLEAD;
         out->n_launches += 3;
@@ -565,9 +478,9 @@ int32_t enqueue_core(const CoreCtx& c, const SubBatch& sb, CoreOut* out) {
     if (n > 0) {
         // tier 0 (one lane per topic), then tier 1 (one warp per topic) over whatever tier 0 deferred — its count is read
         // on the device, so both launches go out back to back
-        if (sb.chunk == 0) CUDA_TRY(cudaEventRecord(w->evk[0], stream));
+        if (sb.chunk == 0) BFQ_CUDA_TRY(cudaEventRecord(w->evk[0], stream));
         launch_match_lanes(p, stream);
-        if (sb.chunk == 0) CUDA_TRY(cudaEventRecord(w->evk[1], stream));
+        if (sb.chunk == 0) BFQ_CUDA_TRY(cudaEventRecord(w->evk[1], stream));
         p.work_list = p.defer_list;
         p.n_work = -1;
         launch_match(p, false, 0, stream);
@@ -592,12 +505,12 @@ int32_t enqueue_core(const CoreCtx& c, const SubBatch& sb, CoreOut* out) {
             out->n_launches += 2;
         }
     }
-    CUDA_TRY(cudaGetLastError());
+    BFQ_CUDA_TRY(cudaGetLastError());
     return BFQ_OK;
 }
 
 int32_t copy_counters(const CoreCtx& c, const SubBatch& sb) {
-    CUDA_TRY(cudaMemcpyAsync(c.w->h_counters.p + (size_t) sb.chunk * CTR_COUNT, c.w->d_counters.p + (size_t) sb.chunk * CTR_COUNT,
+    BFQ_CUDA_TRY(cudaMemcpyAsync(c.w->h_counters.p + (size_t) sb.chunk * CTR_COUNT, c.w->d_counters.p + (size_t) sb.chunk * CTR_COUNT,
                              CTR_COUNT * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c.stream));
     return BFQ_OK;
 }
@@ -611,8 +524,8 @@ int32_t finish_core(const CoreCtx& c, const SubBatch& sb, CoreOut* out, bool* re
     unsigned long long* hc = w->h_counters.p + (size_t) sb.chunk * CTR_COUNT;
     if (reran) *reran = false;
     // the device path waits for ITS match only (an event behind it): later matches may already be queued on the same stream
-    if (done) CUDA_TRY(cudaEventSynchronize(done));
-    else CUDA_TRY(cudaStreamSynchronize(stream));
+    if (done) BFQ_CUDA_TRY(cudaEventSynchronize(done));
+    else BFQ_CUDA_TRY(cudaStreamSynchronize(stream));
     out->n_overflow += (int64_t) hc[CTR_OVERFLOW];
     out->n_deferred += (int64_t) hc[CTR_DEFER];
     if (hc[CTR_OVERFLOW] > 0) {
@@ -624,8 +537,8 @@ int32_t finish_core(const CoreCtx& c, const SubBatch& sb, CoreOut* out, bool* re
         warps = std::min<uint64_t>(warps, (uint64_t) device_sm_count() * 8);
         warps = (warps + 7) / 8 * 8;
         if (w->d_scratch.cap < (size_t) (warps * per_warp)) {
-            CUDA_TRY(cudaDeviceSynchronize());   // the other compute stream of this workspace may be in tier 2 on the old scratch
-            CUDA_TRY(w->d_scratch.reserve((size_t) (warps * per_warp)));
+            BFQ_CUDA_TRY(cudaDeviceSynchronize());   // the other compute stream of this workspace may be in tier 2 on the old scratch
+            BFQ_CUDA_TRY(w->d_scratch.reserve((size_t) (warps * per_warp)));
         }
         p.scratch = w->d_scratch.p;
         p.scratch_frontier_cap = capF;
@@ -653,10 +566,10 @@ int32_t finish_core(const CoreCtx& c, const SubBatch& sb, CoreOut* out, bool* re
             launch_caps(q, stream);
             out->n_launches += 2;
         }
-        CUDA_TRY(cudaGetLastError());
+        BFQ_CUDA_TRY(cudaGetLastError());
         int32_t rc = copy_counters(c, sb);
         if (rc != BFQ_OK) return rc;
-        CUDA_TRY(cudaStreamSynchronize(stream));
+        BFQ_CUDA_TRY(cudaStreamSynchronize(stream));
         if (hc[CTR_ERROR] != 0) return fail(BFQ_E_STATE, "tier-2 scratch exhausted (index statistics inconsistent)");
         if (reran) *reran = true;
     }
@@ -696,9 +609,9 @@ int32_t grow_for_retry(Workspace* w, const CoreOut& co, int64_t n, int C) {
     if (co.want_dyn) {
         const size_t want = (size_t) ((uint64_t) n * INLINE_RANGES + (co.want_dyn + co.want_dyn / 4 + 1024) * (uint64_t) C);
         if (want >= 0xFFFFFFF0ull) return fail(BFQ_E_RANGE, "more than 2^32 matched ranges in one batch; split the batch");
-        CUDA_TRY(w->d_ranges.reserve(want));
+        BFQ_CUDA_TRY(w->d_ranges.reserve(want));
     }
-    if (co.want_thr) CUDA_TRY(w->d_throttled.reserve((size_t) ((co.want_thr + co.want_thr / 4 + 1024) * (uint64_t) C)));
+    if (co.want_thr) BFQ_CUDA_TRY(w->d_throttled.reserve((size_t) ((co.want_thr + co.want_thr / 4 + 1024) * (uint64_t) C)));
     return BFQ_OK;
 }
 
@@ -744,7 +657,7 @@ int32_t device_enqueue(DeviceLease* L) {
     if (rc != BFQ_OK) return rc;
     rc = copy_counters(L->ctx, sb);
     if (rc != BFQ_OK) return rc;
-    CUDA_TRY(cudaEventRecord(L->ws->ev_done, L->ctx.stream));
+    BFQ_CUDA_TRY(cudaEventRecord(L->ws->ev_done, L->ctx.stream));
     return BFQ_OK;
 }
 
@@ -780,8 +693,6 @@ int64_t emit_bytes(const std::string& s, uint8_t* out, int64_t cap) {
 
 extern "C" {
 
-const char* bfq_last_error(void) { return bfq::g_last_error.c_str(); }
-
 int32_t bfq_index_create(int32_t device_ordinal, bfq_index** out) {
     if (!out) return fail(BFQ_E_INVALID, "out is NULL");
     int count = 0;
@@ -789,7 +700,7 @@ int32_t bfq_index_create(int32_t device_ordinal, bfq_index** out) {
     if (e != cudaSuccess || count == 0)
         return fail(BFQ_E_CUDA, std::string("no usable CUDA device (there is no CPU fallback): ") + cudaGetErrorString(e));
     if (device_ordinal < 0 || device_ordinal >= count) return fail(BFQ_E_INVALID, "device ordinal out of range");
-    CUDA_TRY(cudaSetDevice(device_ordinal));
+    BFQ_CUDA_TRY(cudaSetDevice(device_ordinal));
     auto* h = new bfq_index();
     h->device = device_ordinal;
     h->pool->device = device_ordinal;
@@ -895,24 +806,24 @@ int32_t commit_full(bfq_index* h) {
     std::string err;
     if (!build_flat_index_parts(parts, &flat, &err)) return fail(BFQ_E_INVALID, err);
     lap("build (host, all cores)");
-    CUDA_TRY(sn->d_slots.reserve(flat.slots.size()));
-    CUDA_TRY(sn->d_tags.reserve(flat.tags.size()));
-    CUDA_TRY(sn->d_roots.reserve(std::max<size_t>(flat.roots.size(), 1)));
-    CUDA_TRY(sn->d_segs.reserve(flat.segs.size()));
-    CUDA_TRY(sn->d_rkind.reserve(std::max<size_t>(flat.rkind.size(), 1)));
-    CUDA_TRY(sn->d_pfxP.reserve(flat.pfx_persistent.size()));
-    CUDA_TRY(sn->d_pfxG.reserve(flat.pfx_group.size()));
+    BFQ_CUDA_TRY(sn->d_slots.reserve(flat.slots.size()));
+    BFQ_CUDA_TRY(sn->d_tags.reserve(flat.tags.size()));
+    BFQ_CUDA_TRY(sn->d_roots.reserve(std::max<size_t>(flat.roots.size(), 1)));
+    BFQ_CUDA_TRY(sn->d_segs.reserve(flat.segs.size()));
+    BFQ_CUDA_TRY(sn->d_rkind.reserve(std::max<size_t>(flat.rkind.size(), 1)));
+    BFQ_CUDA_TRY(sn->d_pfxP.reserve(flat.pfx_persistent.size()));
+    BFQ_CUDA_TRY(sn->d_pfxG.reserve(flat.pfx_group.size()));
     // (one pageable cudaMemcpy: a threaded upload through per-thread pinned bounce buffers pays more for the pinned
     // allocations than the driver's own staging loses)
-    CUDA_TRY(cudaMemcpy(sn->d_slots.p, flat.slots.data(), flat.slots.size() * sizeof(Slot), cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(sn->d_tags.p, flat.tags.data(), flat.tags.size(), cudaMemcpyHostToDevice));
+    BFQ_CUDA_TRY(cudaMemcpy(sn->d_slots.p, flat.slots.data(), flat.slots.size() * sizeof(Slot), cudaMemcpyHostToDevice));
+    BFQ_CUDA_TRY(cudaMemcpy(sn->d_tags.p, flat.tags.data(), flat.tags.size(), cudaMemcpyHostToDevice));
     if (!flat.roots.empty())
-        CUDA_TRY(cudaMemcpy(sn->d_roots.p, flat.roots.data(), flat.roots.size() * sizeof(Slot), cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(sn->d_segs.p, flat.segs.data(), flat.segs.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        BFQ_CUDA_TRY(cudaMemcpy(sn->d_roots.p, flat.roots.data(), flat.roots.size() * sizeof(Slot), cudaMemcpyHostToDevice));
+    BFQ_CUDA_TRY(cudaMemcpy(sn->d_segs.p, flat.segs.data(), flat.segs.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
     if (!flat.rkind.empty())
-        CUDA_TRY(cudaMemcpy(sn->d_rkind.p, flat.rkind.data(), flat.rkind.size(), cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(sn->d_pfxP.p, flat.pfx_persistent.data(), flat.pfx_persistent.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(sn->d_pfxG.p, flat.pfx_group.data(), flat.pfx_group.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+        BFQ_CUDA_TRY(cudaMemcpy(sn->d_rkind.p, flat.rkind.data(), flat.rkind.size(), cudaMemcpyHostToDevice));
+    BFQ_CUDA_TRY(cudaMemcpy(sn->d_pfxP.p, flat.pfx_persistent.data(), flat.pfx_persistent.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    BFQ_CUDA_TRY(cudaMemcpy(sn->d_pfxG.p, flat.pfx_group.data(), flat.pfx_group.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
     lap("device allocations + upload");
     // per-tenant host side: the staged blobs are shared (no second copy of the KV), the route kinds are sliced
     sn->th.resize(flat.tenants.size());
@@ -1263,28 +1174,32 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
     lap("host bookkeeping");
     // ---- device: copy, upload, assemble, patch, shift
     cudaStream_t st = nullptr;
-    CUDA_TRY(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    DevBuf<uint8_t> d_pack;   // the packed per-rank arrays and the run table
+    BFQ_CUDA_TRY(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    // temporaries the enqueued work reads: declared ahead of the guard, so they are freed after it has synchronised the stream
+    DeviceBuf<uint8_t> d_pack;   // the packed per-rank arrays and the run table
+    DeviceBuf<uint32_t> d_ids;
+    DeviceBuf<Slot> d_recs;
+    DeviceBuf<RankShiftRegion> d_regions;
+    DeviceBuf<RankShiftSlot> d_list;
     struct StreamGuard {
         cudaStream_t s;
-        DevBuf<uint8_t>& pack;
-        ~StreamGuard() { cudaStreamSynchronize(s); cudaStreamDestroy(s); pack.release(); }
-    } guard{st, d_pack};
+        ~StreamGuard() { cudaStreamSynchronize(s); cudaStreamDestroy(s); }
+    } guard{st};
     const size_t n_new = (size_t) rank;
-    CUDA_TRY(sn->d_slots.reserve((size_t) slot_cursor));
-    CUDA_TRY(sn->d_tags.reserve(std::max<size_t>(nf.tags.size(), 1)));
-    CUDA_TRY(sn->d_roots.reserve(std::max<size_t>(nf.host_roots.size(), 1)));
-    CUDA_TRY(sn->d_segs.reserve(std::max<size_t>(nf.segs.size(), 2)));
-    CUDA_TRY(sn->d_rkind.reserve(std::max<size_t>(n_new, 1)));
-    CUDA_TRY(sn->d_pfxP.reserve(n_new + 1));
-    CUDA_TRY(sn->d_pfxG.reserve(n_new + 1));
-    CUDA_TRY(d_pack.reserve(pack_bytes));
+    BFQ_CUDA_TRY(sn->d_slots.reserve((size_t) slot_cursor));
+    BFQ_CUDA_TRY(sn->d_tags.reserve(std::max<size_t>(nf.tags.size(), 1)));
+    BFQ_CUDA_TRY(sn->d_roots.reserve(std::max<size_t>(nf.host_roots.size(), 1)));
+    BFQ_CUDA_TRY(sn->d_segs.reserve(std::max<size_t>(nf.segs.size(), 2)));
+    BFQ_CUDA_TRY(sn->d_rkind.reserve(std::max<size_t>(n_new, 1)));
+    BFQ_CUDA_TRY(sn->d_pfxP.reserve(n_new + 1));
+    BFQ_CUDA_TRY(sn->d_pfxG.reserve(n_new + 1));
+    BFQ_CUDA_TRY(d_pack.reserve(pack_bytes));
     lap("device allocations");
-    CUDA_TRY(cudaMemcpyAsync(sn->d_slots.p, old->d_slots.p, (size_t) of.n_slots * sizeof(Slot), cudaMemcpyDeviceToDevice, st));
-    if (up_slots) CUDA_TRY(cudaMemcpyAsync(sn->d_slots.p + of.n_slots, regions_up.data(), (size_t) up_slots * sizeof(Slot), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaMemcpyAsync(d_pack.p, pack.data(), pack_bytes, cudaMemcpyHostToDevice, st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(sn->d_slots.p, old->d_slots.p, (size_t) of.n_slots * sizeof(Slot), cudaMemcpyDeviceToDevice, st));
+    if (up_slots) BFQ_CUDA_TRY(cudaMemcpyAsync(sn->d_slots.p + of.n_slots, regions_up.data(), (size_t) up_slots * sizeof(Slot), cudaMemcpyHostToDevice, st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(d_pack.p, pack.data(), pack_bytes, cudaMemcpyHostToDevice, st));
     // the whole tag array (16 B per block, ~2 B per wide edge): one small upload
-    if (!nf.tags.empty()) CUDA_TRY(cudaMemcpyAsync(sn->d_tags.p, nf.tags.data(), nf.tags.size(), cudaMemcpyHostToDevice, st));
+    if (!nf.tags.empty()) BFQ_CUDA_TRY(cudaMemcpyAsync(sn->d_tags.p, nf.tags.data(), nf.tags.size(), cudaMemcpyHostToDevice, st));
     {
         AssembleRankParams ap;
         ap.rkind = sn->d_rkind.p;
@@ -1329,37 +1244,26 @@ int32_t commit_delta(bfq_index* h, const std::shared_ptr<Snapshot>& old, const s
         }
     }
     if (!scatter_ids.empty()) {
-        DevBuf<uint32_t> d_ids;
-        DevBuf<Slot> d_recs;
-        CUDA_TRY(d_ids.reserve(scatter_ids.size()));
-        CUDA_TRY(d_recs.reserve(scatter_recs.size()));
-        CUDA_TRY(cudaMemcpyAsync(d_ids.p, scatter_ids.data(), scatter_ids.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(d_recs.p, scatter_recs.data(), scatter_recs.size() * sizeof(Slot), cudaMemcpyHostToDevice, st));
+        BFQ_CUDA_TRY(d_ids.reserve(scatter_ids.size()));
+        BFQ_CUDA_TRY(d_recs.reserve(scatter_recs.size()));
+        BFQ_CUDA_TRY(cudaMemcpyAsync(d_ids.p, scatter_ids.data(), scatter_ids.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+        BFQ_CUDA_TRY(cudaMemcpyAsync(d_recs.p, scatter_recs.data(), scatter_recs.size() * sizeof(Slot), cudaMemcpyHostToDevice, st));
         launch_scatter_records(sn->d_slots.p, d_ids.p, d_recs.p, (int64_t) scatter_ids.size(), st);
-        CUDA_TRY(cudaStreamSynchronize(st));
-        d_ids.release();
-        d_recs.release();
     }
     if (!regions.empty()) {
-        DevBuf<RankShiftRegion> d_regions;
-        CUDA_TRY(d_regions.reserve(regions.size()));
-        CUDA_TRY(cudaMemcpyAsync(d_regions.p, regions.data(), regions.size() * sizeof(RankShiftRegion), cudaMemcpyHostToDevice, st));
+        BFQ_CUDA_TRY(d_regions.reserve(regions.size()));
+        BFQ_CUDA_TRY(cudaMemcpyAsync(d_regions.p, regions.data(), regions.size() * sizeof(RankShiftRegion), cudaMemcpyHostToDevice, st));
         launch_rank_shift(sn->d_slots.p, d_regions.p, (int) regions.size(), st);
-        CUDA_TRY(cudaStreamSynchronize(st));
-        d_regions.release();
     }
     if (!shift_slots.empty()) {
-        DevBuf<RankShiftSlot> d_list;
-        CUDA_TRY(d_list.reserve(shift_slots.size()));
-        CUDA_TRY(cudaMemcpyAsync(d_list.p, shift_slots.data(), shift_slots.size() * sizeof(RankShiftSlot), cudaMemcpyHostToDevice, st));
+        BFQ_CUDA_TRY(d_list.reserve(shift_slots.size()));
+        BFQ_CUDA_TRY(cudaMemcpyAsync(d_list.p, shift_slots.data(), shift_slots.size() * sizeof(RankShiftSlot), cudaMemcpyHostToDevice, st));
         launch_rank_shift_listed(sn->d_slots.p, d_list.p, (int64_t) shift_slots.size(), st);
-        CUDA_TRY(cudaStreamSynchronize(st));
-        d_list.release();
     }
-    CUDA_TRY(cudaMemcpyAsync(sn->d_roots.p, nf.host_roots.data(), nf.host_roots.size() * sizeof(Slot), cudaMemcpyHostToDevice, st));
-    if (!nf.segs.empty()) CUDA_TRY(cudaMemcpyAsync(sn->d_segs.p, nf.segs.data(), nf.segs.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    CUDA_TRY(cudaGetLastError());
+    BFQ_CUDA_TRY(cudaMemcpyAsync(sn->d_roots.p, nf.host_roots.data(), nf.host_roots.size() * sizeof(Slot), cudaMemcpyHostToDevice, st));
+    if (!nf.segs.empty()) BFQ_CUDA_TRY(cudaMemcpyAsync(sn->d_segs.p, nf.segs.data(), nf.segs.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
+    BFQ_CUDA_TRY(cudaGetLastError());
     lap("device copy + patch + rank shift");
     set_l2_window(h, sn.get());
     publish(h, std::move(sn));
@@ -1374,7 +1278,7 @@ int32_t bfq_index_commit(bfq_index* h) {
     // The rebuild runs under the staging lock only: matches keep running on the previous snapshot meanwhile; the new one
     // is published by swapping one shared pointer. Matches and results in flight keep the old snapshot alive.
     std::lock_guard<std::mutex> gs(h->stage_mu);
-    CUDA_TRY(cudaSetDevice(h->device));
+    BFQ_CUDA_TRY(cudaSetDevice(h->device));
     std::shared_ptr<Snapshot> old;
     {
         std::lock_guard<std::mutex> g(h->mu);
@@ -1697,7 +1601,7 @@ int32_t bfq_match(bfq_index* h, const uint8_t* tenants, const int64_t* tenant_of
     if (!h || !out || n < 0 || n_tenants < 0) return fail(BFQ_E_INVALID, "bad argument");
     if (n > 0 && (!topics || !topic_off || !topic_tenant || !tenants || !tenant_off)) return fail(BFQ_E_INVALID, "NULL input");
     if (n_tenants > 0 && (!tenants || !tenant_off)) return fail(BFQ_E_INVALID, "NULL tenant list");
-    CUDA_TRY(cudaSetDevice(h->device));
+    BFQ_CUDA_TRY(cudaSetDevice(h->device));
     std::shared_ptr<Snapshot> snap;
     Workspace* w = nullptr;
     int32_t rc = acquire(h, &snap, &w, "bfq_match");
@@ -1712,16 +1616,16 @@ int32_t bfq_match(bfq_index* h, const uint8_t* tenants, const int64_t* tenant_of
     auto t0 = std::chrono::steady_clock::now();
     const size_t nn = (size_t) std::max<int64_t>(n, 1);
     const int64_t blob_e = n ? topic_off[n] : 0;
-    CUDA_TRY(w->d_topics.reserve((size_t) std::max<int64_t>(blob_e, 1) + 64));
-    CUDA_TRY(w->d_topic_off.reserve(nn + 1));
-    CUDA_TRY(w->d_topic_tenant.reserve(nn));
-    CUDA_TRY(w->d_cnt.reserve(nn));
-    CUDA_TRY(w->d_new_begin.reserve(nn));
-    CUDA_TRY(w->d_final_begin.reserve(nn));
-    CUDA_TRY(w->d_final_count.reserve(nn));
-    CUDA_TRY(w->h_span_begin.reserve(nn));
-    CUDA_TRY(w->h_span_count.reserve(nn));
-    CUDA_TRY(w->h_route_count.reserve(nn));
+    BFQ_CUDA_TRY(w->d_topics.reserve((size_t) std::max<int64_t>(blob_e, 1) + 64));
+    BFQ_CUDA_TRY(w->d_topic_off.reserve(nn + 1));
+    BFQ_CUDA_TRY(w->d_topic_tenant.reserve(nn));
+    BFQ_CUDA_TRY(w->d_cnt.reserve(nn));
+    BFQ_CUDA_TRY(w->d_new_begin.reserve(nn));
+    BFQ_CUDA_TRY(w->d_final_begin.reserve(nn));
+    BFQ_CUDA_TRY(w->d_final_count.reserve(nn));
+    BFQ_CUDA_TRY(w->h_span_begin.reserve(nn));
+    BFQ_CUDA_TRY(w->h_span_count.reserve(nn));
+    BFQ_CUDA_TRY(w->h_route_count.reserve(nn));
 
     // Large batches are cut into sub-batches that flow through three streams: all H2D copies on one, the kernels +
     // compaction + D2H of consecutive sub-batches alternating on two others, so the copy of sub-batch c+1 and the
@@ -1743,7 +1647,7 @@ int32_t bfq_match(bfq_index* h, const uint8_t* tenants, const int64_t* tenant_of
         if (attempt == 8) return fail(BFQ_E_STATE, "buffer sizing did not converge");
         rc = prepare_workspace(h, w, n, C, n_tenants);
         if (rc != BFQ_OK) return rc;
-        CUDA_TRY(w->d_ranges_c.reserve(w->d_ranges.cap));
+        BFQ_CUDA_TRY(w->d_ranges_c.reserve(w->d_ranges.cap));
         const uint64_t dyn_total = w->d_ranges.cap - (uint64_t) n * INLINE_RANGES;
         const uint64_t dyn_slice = dyn_total / (uint64_t) C, thr_slice = w->d_throttled.cap / (uint64_t) C;
         size_t tmp_bytes = 0;
@@ -1752,15 +1656,15 @@ int32_t bfq_match(bfq_index* h, const uint8_t* tenants, const int64_t* tenant_of
             q.n_topics = (n + C - 1) / C + 1;
             q.counts = w->d_cnt.p;
             q.new_begin = w->d_new_begin.p;
-            CUDA_TRY(launch_compact(q, nullptr, &tmp_bytes, w->stream, 1));
-            CUDA_TRY(w->d_scan_tmp.reserve(tmp_bytes * 2 + 512));   // one scratch per compute stream
+            BFQ_CUDA_TRY(launch_compact(q, nullptr, &tmp_bytes, w->stream, 1));
+            BFQ_CUDA_TRY(w->d_scan_tmp.reserve(tmp_bytes * 2 + 512));   // one scratch per compute stream
         }
         co = CoreOut();
         rbase = tbase = 0;
         // ---- H2D of every sub-batch, back to back on the copy stream
-        CUDA_TRY(cudaEventRecord(w->ev[0], w->copy_stream));
+        BFQ_CUDA_TRY(cudaEventRecord(w->ev[0], w->copy_stream));
         // the kernels read whole aligned 16-byte granules: define the bytes behind the blob's end (masked out, but read)
-        CUDA_TRY(cudaMemsetAsync(w->d_topics.p + blob_e, 0, 64, w->copy_stream));
+        BFQ_CUDA_TRY(cudaMemsetAsync(w->d_topics.p + blob_e, 0, 64, w->copy_stream));
         rc = resolve_tenants(w, snap.get(), tenants, tenant_off, n_tenants, max_pfanout, max_gfanout, w->copy_stream);
         if (rc != BFQ_OK) return rc;
         int64_t bounds[MAX_CHUNKS + 1];
@@ -1768,17 +1672,17 @@ int32_t bfq_match(bfq_index* h, const uint8_t* tenants, const int64_t* tenant_of
         for (int c = 0; c < C && n > 0; c++) {
             const int64_t b = bounds[c], e = bounds[c + 1];
             const int64_t ob = topic_off[b], oe = topic_off[e];
-            CUDA_TRY(cudaMemcpyAsync(w->d_topic_off.p + b, topic_off + b, (size_t) (e - b + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, w->copy_stream));
-            CUDA_TRY(cudaMemcpyAsync(w->d_topic_tenant.p + b, topic_tenant + b, (size_t) (e - b) * sizeof(int32_t), cudaMemcpyHostToDevice, w->copy_stream));
-            CUDA_TRY(cudaMemcpyAsync(w->d_topics.p + ob, topics + ob, (size_t) (oe - ob), cudaMemcpyHostToDevice, w->copy_stream));
-            CUDA_TRY(cudaEventRecord(w->ev_h2d[c], w->copy_stream));
+            BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_topic_off.p + b, topic_off + b, (size_t) (e - b + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, w->copy_stream));
+            BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_topic_tenant.p + b, topic_tenant + b, (size_t) (e - b) * sizeof(int32_t), cudaMemcpyHostToDevice, w->copy_stream));
+            BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_topics.p + ob, topics + ob, (size_t) (oe - ob), cudaMemcpyHostToDevice, w->copy_stream));
+            BFQ_CUDA_TRY(cudaEventRecord(w->ev_h2d[c], w->copy_stream));
         }
-        CUDA_TRY(cudaEventRecord(w->ev[1], w->copy_stream));
-        if (n == 0) CUDA_TRY(cudaStreamSynchronize(w->copy_stream));
+        BFQ_CUDA_TRY(cudaEventRecord(w->ev[1], w->copy_stream));
+        if (n == 0) BFQ_CUDA_TRY(cudaStreamSynchronize(w->copy_stream));
         bool retry = false;
         for (int c = 0; c < C && n > 0; c++) {
             cudaStream_t st = C == 1 ? w->stream : w->work_stream[c & 1];
-            CUDA_TRY(cudaStreamWaitEvent(st, w->ev_h2d[c], 0));
+            BFQ_CUDA_TRY(cudaStreamWaitEvent(st, w->ev_h2d[c], 0));
             SubBatch sb;
             sb.begin = bounds[c];
             sb.n = bounds[c + 1] - bounds[c];
@@ -1809,7 +1713,7 @@ int32_t bfq_match(bfq_index* h, const uint8_t* tenants, const int64_t* tenant_of
             cp.ranges_out_cap = (uint64_t) sb.n * INLINE_RANGES + sb.dyn_cap;
             cp.total_out = w->d_counters.p + (size_t) c * CTR_COUNT + CTR_ROUTES;
             uint8_t* scan_tmp = w->d_scan_tmp.p + (size_t) (c & 1) * ((tmp_bytes + 256) / 256 * 256);
-            CUDA_TRY(launch_compact(cp, scan_tmp, &tmp_bytes, st, 1));
+            BFQ_CUDA_TRY(launch_compact(cp, scan_tmp, &tmp_bytes, st, 1));
             rc = copy_counters(ctx, sb);
             if (rc != BFQ_OK) return rc;
             bool reran = false;
@@ -1820,10 +1724,10 @@ int32_t bfq_match(bfq_index* h, const uint8_t* tenants, const int64_t* tenant_of
             }
             if (rc != BFQ_OK) return rc;
             if (reran) {   // tier 2 changed spans: redo the counting pass
-                CUDA_TRY(launch_compact(cp, scan_tmp, &tmp_bytes, st, 1));
+                BFQ_CUDA_TRY(launch_compact(cp, scan_tmp, &tmp_bytes, st, 1));
                 rc = copy_counters(ctx, sb);
                 if (rc != BFQ_OK) return rc;
-                CUDA_TRY(cudaStreamSynchronize(st));
+                BFQ_CUDA_TRY(cudaStreamSynchronize(st));
                 co.n_launches += 3;
             }
             if (c == 0) {
@@ -1834,47 +1738,45 @@ int32_t bfq_match(bfq_index* h, const uint8_t* tenants, const int64_t* tenant_of
             const int64_t total_c = (int64_t) hc[CTR_ROUTES], thr_c = co.chunk_throttled[c];
             // host result buffers grow by reallocation: wait for the copies in flight before moving them
             if ((size_t) (rbase + total_c) > w->h_ranges.cap || (size_t) (tbase + thr_c) > w->h_throttled.cap) {
-                CUDA_TRY(cudaDeviceSynchronize());
+                BFQ_CUDA_TRY(cudaDeviceSynchronize());
                 if ((size_t) (rbase + total_c) > w->h_ranges.cap) {
-                    PinBuf<uint2> nb;
-                    CUDA_TRY(nb.reserve((size_t) ((rbase + total_c) * (C - c > 1 ? 2 : 1) + (1 << 16))));
+                    PinnedBuf<uint2> nb;
+                    BFQ_CUDA_TRY(nb.reserve((size_t) ((rbase + total_c) * (C - c > 1 ? 2 : 1) + (1 << 16))));
                     if (rbase) memcpy(nb.p, w->h_ranges.p, (size_t) rbase * sizeof(uint2));
-                    w->h_ranges.release();
-                    w->h_ranges = nb;
+                    w->h_ranges = std::move(nb);
                 }
                 if ((size_t) (tbase + thr_c) > w->h_throttled.cap) {
-                    PinBuf<uint3> nb;
-                    CUDA_TRY(nb.reserve((size_t) ((tbase + thr_c) * 2 + 1024)));
+                    PinnedBuf<uint3> nb;
+                    BFQ_CUDA_TRY(nb.reserve((size_t) ((tbase + thr_c) * 2 + 1024)));
                     if (tbase) memcpy(nb.p, w->h_throttled.p, (size_t) tbase * sizeof(uint3));
-                    w->h_throttled.release();
-                    w->h_throttled = nb;
+                    w->h_throttled = std::move(nb);
                 }
             }
             cp.out_base = (uint32_t) rbase;
-            CUDA_TRY(launch_compact(cp, scan_tmp, &tmp_bytes, st, 2));
+            BFQ_CUDA_TRY(launch_compact(cp, scan_tmp, &tmp_bytes, st, 2));
             co.n_launches += 4;
-            CUDA_TRY(cudaMemcpyAsync(w->h_span_begin.p + sb.begin, w->d_final_begin.p + sb.begin, (size_t) sb.n * 4, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(w->h_span_count.p + sb.begin, w->d_final_count.p + sb.begin, (size_t) sb.n * 4, cudaMemcpyDeviceToHost, st));
-            CUDA_TRY(cudaMemcpyAsync(w->h_route_count.p + sb.begin, w->d_route_count.p + sb.begin, (size_t) sb.n * 4, cudaMemcpyDeviceToHost, st));
+            BFQ_CUDA_TRY(cudaMemcpyAsync(w->h_span_begin.p + sb.begin, w->d_final_begin.p + sb.begin, (size_t) sb.n * 4, cudaMemcpyDeviceToHost, st));
+            BFQ_CUDA_TRY(cudaMemcpyAsync(w->h_span_count.p + sb.begin, w->d_final_count.p + sb.begin, (size_t) sb.n * 4, cudaMemcpyDeviceToHost, st));
+            BFQ_CUDA_TRY(cudaMemcpyAsync(w->h_route_count.p + sb.begin, w->d_route_count.p + sb.begin, (size_t) sb.n * 4, cudaMemcpyDeviceToHost, st));
             if (total_c > 0)
-                CUDA_TRY(cudaMemcpyAsync(w->h_ranges.p + rbase, w->d_ranges_c.p + region, (size_t) total_c * sizeof(uint2), cudaMemcpyDeviceToHost, st));
+                BFQ_CUDA_TRY(cudaMemcpyAsync(w->h_ranges.p + rbase, w->d_ranges_c.p + region, (size_t) total_c * sizeof(uint2), cudaMemcpyDeviceToHost, st));
             if (thr_c > 0)
-                CUDA_TRY(cudaMemcpyAsync(w->h_throttled.p + tbase, w->d_throttled.p + sb.thr_off, (size_t) thr_c * sizeof(uint3), cudaMemcpyDeviceToHost, st));
+                BFQ_CUDA_TRY(cudaMemcpyAsync(w->h_throttled.p + tbase, w->d_throttled.p + sb.thr_off, (size_t) thr_c * sizeof(uint3), cudaMemcpyDeviceToHost, st));
             rbase += total_c;
             tbase += thr_c;
         }
         if (!retry) break;
         // a slice of the range / throttled buffers was too small: grow them and redo the batch un-chunked
         count_retry(h);
-        CUDA_TRY(cudaDeviceSynchronize());
+        BFQ_CUDA_TRY(cudaDeviceSynchronize());
         rc = grow_for_retry(w, co, n, C);
         if (rc != BFQ_OK) return rc;
         C = 1;
     }
-    CUDA_TRY(cudaStreamSynchronize(w->work_stream[0]));
-    CUDA_TRY(cudaStreamSynchronize(w->work_stream[1]));
-    CUDA_TRY(cudaStreamSynchronize(w->stream));
-    CUDA_TRY(cudaStreamSynchronize(w->copy_stream));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(w->work_stream[0]));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(w->work_stream[1]));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(w->stream));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(w->copy_stream));
     add_stats(h, co, n, kernel_ms);
     co.n_ranges = rbase;
     co.n_throttled = tbase;
@@ -1995,7 +1897,7 @@ int32_t bfq_match_device_async(bfq_index* h, const uint8_t* tenants, const int64
     if (!h || !out || n < 0 || n_tenants < 0) return fail(BFQ_E_INVALID, "bad argument");
     if (n_tenants > 0 && (!tenants || !tenant_off)) return fail(BFQ_E_INVALID, "NULL tenant list");
     memset(out, 0, sizeof(*out));
-    CUDA_TRY(cudaSetDevice(h->device));
+    BFQ_CUDA_TRY(cudaSetDevice(h->device));
     auto* L = new DeviceLease();
     L->h = h;
     L->pool = h->pool;
@@ -2092,21 +1994,21 @@ int32_t bfq_expand_device(const bfq_device_result* res, int64_t* d_offsets, int6
     bfq_index* h = L->h;
     Workspace* w = L->ws;
     const int64_t n_topics = L->n;
-    CUDA_TRY(cudaSetDevice(h->device));
+    BFQ_CUDA_TRY(cudaSetDevice(h->device));
     cudaStream_t st = (cudaStream_t) stream;
-    CUDA_TRY(w->d_exp_counts.reserve((size_t) n_topics + 1));
+    BFQ_CUDA_TRY(w->d_exp_counts.reserve((size_t) n_topics + 1));
     const ExpandParams p = expand_params(L, d_offsets, d_ranks, rank_cap);
     size_t tmp_bytes = 0;
-    CUDA_TRY(launch_expand(p, nullptr, &tmp_bytes, st, 1));
-    CUDA_TRY(w->d_scan_tmp.reserve(tmp_bytes + 256));
-    CUDA_TRY(launch_expand(p, w->d_scan_tmp.p, &tmp_bytes, st, 1));
+    BFQ_CUDA_TRY(launch_expand(p, nullptr, &tmp_bytes, st, 1));
+    BFQ_CUDA_TRY(w->d_scan_tmp.reserve(tmp_bytes + 256));
+    BFQ_CUDA_TRY(launch_expand(p, w->d_scan_tmp.p, &tmp_bytes, st, 1));
     long long total = 0;
-    CUDA_TRY(cudaMemcpyAsync(&total, d_offsets + n_topics, sizeof(long long), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(&total, d_offsets + n_topics, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
     if (n_ranks) *n_ranks = (int64_t) total;
     int64_t launches = 2;
     if (d_ranks && total <= rank_cap) {
-        CUDA_TRY(launch_expand(p, w->d_scan_tmp.p, &tmp_bytes, st, 2));
+        BFQ_CUDA_TRY(launch_expand(p, w->d_scan_tmp.p, &tmp_bytes, st, 2));
         launches += 2;
     }
     std::lock_guard<std::mutex> g(h->mu);
@@ -2130,21 +2032,21 @@ int32_t bfq_expand_device_budget(const bfq_device_result* res, const int32_t* d_
                                            ": MaxPersistentFanoutBytes must be > 0");
     bfq_index* h = L->h;
     Workspace* w = L->ws;
-    CUDA_TRY(cudaSetDevice(h->device));
+    BFQ_CUDA_TRY(cudaSetDevice(h->device));
     cudaStream_t st = (cudaStream_t) stream;
     const size_t nn = (size_t) std::max<int64_t>(n_topics, 1), nt = (size_t) std::max(n_tenants, 1);
-    CUDA_TRY(w->d_exp_counts.reserve(nn + 1));
-    CUDA_TRY(w->d_bud_bytes.reserve(nt));
-    CUDA_TRY(w->d_bud_bw.reserve(nt));
-    CUDA_TRY(w->d_bud_flags.reserve(nn));
-    CUDA_TRY(w->d_bud_dp.reserve(nn));
-    CUDA_TRY(w->d_bud_list.reserve(nn));
-    CUDA_TRY(w->d_bud_ctr.reserve(BUD_CTR_COUNT));
+    BFQ_CUDA_TRY(w->d_exp_counts.reserve(nn + 1));
+    BFQ_CUDA_TRY(w->d_bud_bytes.reserve(nt));
+    BFQ_CUDA_TRY(w->d_bud_bw.reserve(nt));
+    BFQ_CUDA_TRY(w->d_bud_flags.reserve(nn));
+    BFQ_CUDA_TRY(w->d_bud_dp.reserve(nn));
+    BFQ_CUDA_TRY(w->d_bud_list.reserve(nn));
+    BFQ_CUDA_TRY(w->d_bud_ctr.reserve(BUD_CTR_COUNT));
     if (n_tenants > 0) {
-        CUDA_TRY(cudaMemcpyAsync(w->d_bud_bytes.p, max_pfanout_bytes, (size_t) n_tenants * sizeof(long long), cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(w->d_bud_bw.p, tenant_bandwidth, (size_t) n_tenants, cudaMemcpyHostToDevice, st));
+        BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_bud_bytes.p, max_pfanout_bytes, (size_t) n_tenants * sizeof(long long), cudaMemcpyHostToDevice, st));
+        BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_bud_bw.p, tenant_bandwidth, (size_t) n_tenants, cudaMemcpyHostToDevice, st));
     }
-    CUDA_TRY(cudaMemsetAsync(w->d_bud_ctr.p, 0, BUD_CTR_COUNT * sizeof(unsigned long long), st));
+    BFQ_CUDA_TRY(cudaMemsetAsync(w->d_bud_ctr.p, 0, BUD_CTR_COUNT * sizeof(unsigned long long), st));
     BudgetParams q{};
     q.e = expand_params(L, d_offsets, d_ranks, rank_cap);
     q.n_tenants = n_tenants;
@@ -2156,19 +2058,19 @@ int32_t bfq_expand_device_budget(const bfq_device_result* res, const int32_t* d_
     q.list = w->d_bud_list.p;
     q.ctr = w->d_bud_ctr.p;
     size_t tmp_bytes = 0;
-    CUDA_TRY(launch_budget(q, nullptr, &tmp_bytes, st, 1));
-    CUDA_TRY(w->d_scan_tmp.reserve(tmp_bytes + 256));
-    CUDA_TRY(launch_budget(q, w->d_scan_tmp.p, &tmp_bytes, st, 1));
+    BFQ_CUDA_TRY(launch_budget(q, nullptr, &tmp_bytes, st, 1));
+    BFQ_CUDA_TRY(w->d_scan_tmp.reserve(tmp_bytes + 256));
+    BFQ_CUDA_TRY(launch_budget(q, w->d_scan_tmp.p, &tmp_bytes, st, 1));
     long long total = 0;
     unsigned long long ctr[BUD_CTR_COUNT];
-    CUDA_TRY(cudaMemcpyAsync(&total, d_offsets + n_topics, sizeof(long long), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(ctr, w->d_bud_ctr.p, sizeof(ctr), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(&total, d_offsets + n_topics, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(ctr, w->d_bud_ctr.p, sizeof(ctr), cudaMemcpyDeviceToHost, st));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
     int64_t launches = 2;
     const bool ok = ctr[BUD_BAD_SIZE] == 0;
     if (ok && d_ranks && total <= rank_cap) {
         q.n_listed = (int64_t) ctr[BUD_LISTED];
-        CUDA_TRY(launch_budget(q, w->d_scan_tmp.p, &tmp_bytes, st, 2));
+        BFQ_CUDA_TRY(launch_budget(q, w->d_scan_tmp.p, &tmp_bytes, st, 2));
         launches += 2;
     }
     {
@@ -2235,14 +2137,14 @@ int32_t ensure_fan_table(bfq_index* h, Snapshot* s, std::shared_ptr<Snapshot::Fa
     }
     // ids share rdeliv[] with FO_GROUP_BIT, and n_deliverers and the global pass's n_deliverers + 1 counts are int32
     if (ft->n_deliverers > 0x7FFFFFFEu) return fail(BFQ_E_RANGE, "more than 2^31 - 3 distinct (subBrokerId, delivererKey) pairs on one handle");
-    CUDA_TRY(ft->d_rdeliv.reserve(rdeliv.size()));
-    CUDA_TRY(ft->d_gmem_off.reserve(gmem_off.size()));
-    CUDA_TRY(ft->d_gmem_deliv.reserve(std::max<size_t>(gmem_deliv.size(), 1)));
-    CUDA_TRY(ft->d_gordered.reserve(std::max<size_t>(gordered.size(), 1)));
-    CUDA_TRY(cudaMemcpy(ft->d_rdeliv.p, rdeliv.data(), rdeliv.size() * 4, cudaMemcpyHostToDevice));
-    CUDA_TRY(cudaMemcpy(ft->d_gmem_off.p, gmem_off.data(), gmem_off.size() * 4, cudaMemcpyHostToDevice));
-    if (!gmem_deliv.empty()) CUDA_TRY(cudaMemcpy(ft->d_gmem_deliv.p, gmem_deliv.data(), gmem_deliv.size() * 4, cudaMemcpyHostToDevice));
-    if (!gordered.empty()) CUDA_TRY(cudaMemcpy(ft->d_gordered.p, gordered.data(), gordered.size(), cudaMemcpyHostToDevice));
+    BFQ_CUDA_TRY(ft->d_rdeliv.reserve(rdeliv.size()));
+    BFQ_CUDA_TRY(ft->d_gmem_off.reserve(gmem_off.size()));
+    BFQ_CUDA_TRY(ft->d_gmem_deliv.reserve(std::max<size_t>(gmem_deliv.size(), 1)));
+    BFQ_CUDA_TRY(ft->d_gordered.reserve(std::max<size_t>(gordered.size(), 1)));
+    BFQ_CUDA_TRY(cudaMemcpy(ft->d_rdeliv.p, rdeliv.data(), rdeliv.size() * 4, cudaMemcpyHostToDevice));
+    BFQ_CUDA_TRY(cudaMemcpy(ft->d_gmem_off.p, gmem_off.data(), gmem_off.size() * 4, cudaMemcpyHostToDevice));
+    if (!gmem_deliv.empty()) BFQ_CUDA_TRY(cudaMemcpy(ft->d_gmem_deliv.p, gmem_deliv.data(), gmem_deliv.size() * 4, cudaMemcpyHostToDevice));
+    if (!gordered.empty()) BFQ_CUDA_TRY(cudaMemcpy(ft->d_gordered.p, gordered.data(), gordered.size(), cudaMemcpyHostToDevice));
     s->fan = ft;
     *out = ft;
     return BFQ_OK;
@@ -2257,7 +2159,7 @@ int32_t bfq_fanout_device(const bfq_device_result* res, const int64_t* d_offsets
     if (n_pairs >= (int64_t) 0xFFFFFFF0ll) return fail(BFQ_E_RANGE, "more than 2^32 (topic, route) pairs in one batch; split the batch");
     bfq_index* h = L->h;
     Workspace* w = L->ws;
-    CUDA_TRY(cudaSetDevice(h->device));
+    BFQ_CUDA_TRY(cudaSetDevice(h->device));
     std::shared_ptr<Snapshot::FanTable> ft;
     int32_t rc = ensure_fan_table(h, L->snap.get(), &ft);
     if (rc != BFQ_OK) return rc;
@@ -2269,12 +2171,12 @@ int32_t bfq_fanout_device(const bfq_device_result* res, const int64_t* d_offsets
     }
     const bool tiled = !force_global && fanout_tiled(ft->n_deliverers, n_pairs);
     const size_t words = fanout_scratch_words(ft->n_deliverers, n_pairs, tiled);
-    CUDA_TRY(w->d_fo_counts.reserve(words));
-    CUDA_TRY(w->d_fo_base.reserve(words));
-    CUDA_TRY(w->d_pack_offsets.reserve((size_t) ft->n_deliverers + 1));
-    CUDA_TRY(w->d_pack_topic.reserve((size_t) std::max<int64_t>(n_pairs, 1)));
-    CUDA_TRY(w->d_pack_rank.reserve((size_t) std::max<int64_t>(n_pairs, 1)));
-    CUDA_TRY(w->d_pack_member.reserve((size_t) std::max<int64_t>(n_pairs, 1)));
+    BFQ_CUDA_TRY(w->d_fo_counts.reserve(words));
+    BFQ_CUDA_TRY(w->d_fo_base.reserve(words));
+    BFQ_CUDA_TRY(w->d_pack_offsets.reserve((size_t) ft->n_deliverers + 1));
+    BFQ_CUDA_TRY(w->d_pack_topic.reserve((size_t) std::max<int64_t>(n_pairs, 1)));
+    BFQ_CUDA_TRY(w->d_pack_rank.reserve((size_t) std::max<int64_t>(n_pairs, 1)));
+    BFQ_CUDA_TRY(w->d_pack_member.reserve((size_t) std::max<int64_t>(n_pairs, 1)));
     FanoutParams p{};
     p.n_topics = L->n;
     p.offsets = d_offsets;
@@ -2292,9 +2194,9 @@ int32_t bfq_fanout_device(const bfq_device_result* res, const int64_t* d_offsets
     p.pack_rank = w->d_pack_rank.p;
     p.pack_member = w->d_pack_member.p;
     size_t tmp_bytes = 0;
-    CUDA_TRY(launch_fanout(p, tiled, nullptr, &tmp_bytes, st));
-    CUDA_TRY(w->d_fo_tmp.reserve(tmp_bytes + 256));
-    CUDA_TRY(launch_fanout(p, tiled, w->d_fo_tmp.p, &tmp_bytes, st));
+    BFQ_CUDA_TRY(launch_fanout(p, tiled, nullptr, &tmp_bytes, st));
+    BFQ_CUDA_TRY(w->d_fo_tmp.reserve(tmp_bytes + 256));
+    BFQ_CUDA_TRY(launch_fanout(p, tiled, w->d_fo_tmp.p, &tmp_bytes, st));
     out->d_pack_offsets = (const int64_t*) w->d_pack_offsets.p;
     out->d_pack_topic = w->d_pack_topic.p;
     out->d_pack_rank = w->d_pack_rank.p;

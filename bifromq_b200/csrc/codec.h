@@ -51,7 +51,7 @@ std::string make_tenant_begin_key(sv tenant);                                   
 std::string make_route_key(sv tenant, sv mqtt_topic_filter, sv receiver_url);              // :108-125
 std::string prefix_upper_bound(sv key, bool* open_end);
 
-// thread-local error text behind bfq_last_error() (defined in capi.cu)
+// thread-local error text behind bfq_last_error() (defined in errors.cc)
 int32_t set_error(int32_t code, const std::string& msg);
 
 // ---- retain store key layout (bifromq-retain/bifromq-retain-store-schema/.../schema/KVSchemaUtil.java:44-73, LevelHash.java:31-49):

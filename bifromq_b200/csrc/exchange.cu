@@ -24,21 +24,12 @@
 #include <vector>
 
 #include "../../include/bfq_gpumatch.h"
+#include "cuda_buf.h"
 #include "match_kernels.cuh"
 
-namespace bfq {
-int32_t set_error(int32_t code, const std::string& msg);
-}
 using namespace bfq;
 
 namespace {
-
-int32_t xfail(int32_t code, const std::string& msg) { return bfq::set_error(code, msg); }
-#define X_CUDA(expr)                                                                                \
-    do {                                                                                            \
-        cudaError_t _e = (expr);                                                                    \
-        if (_e != cudaSuccess) return xfail(BFQ_E_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e)); \
-    } while (0)
 
 struct NcclApi {
     ncclResult_t (*GetUniqueId)(ncclUniqueId*) = nullptr;
@@ -89,29 +80,14 @@ NcclApi& nccl() {
 #define X_NCCL(expr)                                                                                \
     do {                                                                                            \
         ncclResult_t _r = (expr);                                                                   \
-        if (_r != ncclSuccess) return xfail(BFQ_E_CUDA, std::string(#expr) + ": " + nccl().GetErrorString(_r)); \
+        if (_r != ncclSuccess) return fail(BFQ_E_CUDA, std::string(#expr) + ": " + nccl().GetErrorString(_r)); \
     } while (0)
 
+// room for n elements, with headroom: the sizes move a little from batch to batch
 template <typename T>
-struct XBuf {
-    T* p = nullptr;
-    size_t cap = 0;
-    cudaError_t reserve(size_t n) {
-        if (n <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        const size_t want = std::max<size_t>(n + n / 4, 1024);   // headroom: the sizes move a little from batch to batch
-        cudaError_t e = cudaMalloc(&p, want * sizeof(T));
-        if (e == cudaSuccess) cap = want;
-        return e;
-    }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
-};
+cudaError_t reserve_headroom(DeviceBuf<T>& b, size_t n) {
+    return n <= b.cap ? cudaSuccess : b.reserve(std::max<size_t>(n + n / 4, 1024));
+}
 
 __global__ void exchange_meta_kernel(long long* meta, long long n_topics, const uint32_t* new_begin, const uint32_t* counts) {
     meta[0] = n_topics;
@@ -123,27 +99,24 @@ __global__ void exchange_meta_kernel(long long* meta, long long n_topics, const 
 struct bfq_exchange {
     int device = 0, rank = 0, world = 1;
     ncclComm_t comm = nullptr;
-    XBuf<uint32_t> d_cnt, d_begin, d_final_begin, d_final_count;   // local compaction scratch
-    XBuf<uint8_t> d_scan_tmp;
-    XBuf<long long> d_meta;                 // {n_topics, n_ranges} x world
-    long long* h_meta = nullptr;            // pinned copy
-    XBuf<uint32_t> g_route_count, g_span_count;
-    XBuf<uint2> g_ranges;
+    DeviceBuf<uint32_t> d_cnt, d_begin, d_final_begin, d_final_count;   // local compaction scratch
+    DeviceBuf<uint8_t> d_scan_tmp;
+    DeviceBuf<long long> d_meta;                 // {n_topics, n_ranges} x world
+    PinnedBuf<long long> h_meta;                 // pinned copy
+    DeviceBuf<uint32_t> g_route_count, g_span_count;
+    DeviceBuf<uint2> g_ranges;
     std::vector<int64_t> topic_base, range_base, topic_count, range_count;
     ~bfq_exchange() {
-        cudaSetDevice(device);
+        cudaSetDevice(device);   // the buffers are freed after this body, on this device
         if (comm && nccl().ok) nccl().CommDestroy(comm);
-        d_cnt.release(); d_begin.release(); d_final_begin.release(); d_final_count.release(); d_scan_tmp.release(); d_meta.release();
-        g_route_count.release(); g_span_count.release(); g_ranges.release();
-        if (h_meta) cudaFreeHost(h_meta);
     }
 };
 
 extern "C" {
 
 int32_t bfq_exchange_unique_id(uint8_t* id_out, int32_t cap) {
-    if (!id_out || cap < (int32_t) sizeof(ncclUniqueId)) return xfail(BFQ_E_INVALID, "id buffer must hold BFQ_EXCHANGE_ID_BYTES bytes");
-    if (!nccl().ok) return xfail(BFQ_E_STATE, nccl().err);
+    if (!id_out || cap < (int32_t) sizeof(ncclUniqueId)) return fail(BFQ_E_INVALID, "id buffer must hold BFQ_EXCHANGE_ID_BYTES bytes");
+    if (!nccl().ok) return fail(BFQ_E_STATE, nccl().err);
     ncclUniqueId id;
     X_NCCL(nccl().GetUniqueId(&id));
     memcpy(id_out, &id, sizeof(id));
@@ -151,9 +124,9 @@ int32_t bfq_exchange_unique_id(uint8_t* id_out, int32_t cap) {
 }
 
 int32_t bfq_exchange_create(int32_t device_ordinal, int32_t rank, int32_t world, const uint8_t* id, bfq_exchange** out) {
-    if (!out || !id || world < 1 || rank < 0 || rank >= world) return xfail(BFQ_E_INVALID, "bad argument");
-    if (!nccl().ok) return xfail(BFQ_E_STATE, nccl().err);
-    X_CUDA(cudaSetDevice(device_ordinal));
+    if (!out || !id || world < 1 || rank < 0 || rank >= world) return fail(BFQ_E_INVALID, "bad argument");
+    if (!nccl().ok) return fail(BFQ_E_STATE, nccl().err);
+    BFQ_CUDA_TRY(cudaSetDevice(device_ordinal));
     auto* x = new bfq_exchange();
     x->device = device_ordinal;
     x->rank = rank;
@@ -164,13 +137,13 @@ int32_t bfq_exchange_create(int32_t device_ordinal, int32_t rank, int32_t world,
     if (r != ncclSuccess) {
         x->comm = nullptr;
         delete x;
-        return xfail(BFQ_E_CUDA, std::string("ncclCommInitRank: ") + nccl().GetErrorString(r));
+        return fail(BFQ_E_CUDA, std::string("ncclCommInitRank: ") + nccl().GetErrorString(r));
     }
-    cudaError_t e = x->d_meta.reserve((size_t) 2 * world);
-    if (e == cudaSuccess) e = cudaMallocHost(&x->h_meta, (size_t) 2 * world * sizeof(long long));
+    cudaError_t e = reserve_headroom(x->d_meta, (size_t) 2 * world);
+    if (e == cudaSuccess) e = x->h_meta.reserve((size_t) 2 * world);
     if (e != cudaSuccess) {
         delete x;
-        return xfail(BFQ_E_CUDA, cudaGetErrorString(e));
+        return fail(BFQ_E_CUDA, cudaGetErrorString(e));
     }
     x->topic_base.assign((size_t) world + 1, 0);
     x->range_base.assign((size_t) world + 1, 0);
@@ -183,18 +156,18 @@ int32_t bfq_exchange_create(int32_t device_ordinal, int32_t rank, int32_t world,
 void bfq_exchange_destroy(bfq_exchange* x) { delete x; }
 
 int32_t bfq_exchange_gather(bfq_exchange* x, const bfq_device_result* res, int32_t what, void* stream, bfq_gathered* out) {
-    if (!x || !res || !out) return xfail(BFQ_E_INVALID, "bad argument");
-    if (what != BFQ_EXCHANGE_COUNTS && what != BFQ_EXCHANGE_RANGES) return xfail(BFQ_E_INVALID, "what: BFQ_EXCHANGE_COUNTS or BFQ_EXCHANGE_RANGES");
-    X_CUDA(cudaSetDevice(x->device));
+    if (!x || !res || !out) return fail(BFQ_E_INVALID, "bad argument");
+    if (what != BFQ_EXCHANGE_COUNTS && what != BFQ_EXCHANGE_RANGES) return fail(BFQ_E_INVALID, "what: BFQ_EXCHANGE_COUNTS or BFQ_EXCHANGE_RANGES");
+    BFQ_CUDA_TRY(cudaSetDevice(x->device));
     cudaStream_t st = (cudaStream_t) stream;
     const int64_t n = res->n_topics;
     const int W = x->world;
     const bool with_ranges = what == BFQ_EXCHANGE_RANGES;
     // ---- 1. local compaction, phase 1 (counts, exclusive scan); the total goes into this rank's meta slot on the device
-    X_CUDA(x->d_cnt.reserve((size_t) std::max<int64_t>(n, 1)));
-    X_CUDA(x->d_begin.reserve((size_t) std::max<int64_t>(n, 1)));
-    X_CUDA(x->d_final_begin.reserve((size_t) std::max<int64_t>(n, 1)));
-    X_CUDA(x->d_final_count.reserve((size_t) std::max<int64_t>(n, 1)));
+    BFQ_CUDA_TRY(reserve_headroom(x->d_cnt, (size_t) std::max<int64_t>(n, 1)));
+    BFQ_CUDA_TRY(reserve_headroom(x->d_begin, (size_t) std::max<int64_t>(n, 1)));
+    BFQ_CUDA_TRY(reserve_headroom(x->d_final_begin, (size_t) std::max<int64_t>(n, 1)));
+    BFQ_CUDA_TRY(reserve_headroom(x->d_final_count, (size_t) std::max<int64_t>(n, 1)));
     CompactParams cp{};
     cp.n_topics = n;
     cp.span_begin = res->d_span_begin;
@@ -210,22 +183,22 @@ int32_t bfq_exchange_gather(bfq_exchange* x, const bfq_device_result* res, int32
     {
         CompactParams q = cp;
         q.n_topics = std::max<int64_t>(n, 1);
-        X_CUDA(launch_compact(q, nullptr, &tmp_bytes, st, 1));
-        X_CUDA(x->d_scan_tmp.reserve(tmp_bytes + 256));
+        BFQ_CUDA_TRY(launch_compact(q, nullptr, &tmp_bytes, st, 1));
+        BFQ_CUDA_TRY(reserve_headroom(x->d_scan_tmp, tmp_bytes + 256));
     }
-    if (n > 0) X_CUDA(launch_compact(cp, x->d_scan_tmp.p, &tmp_bytes, st, 1));
+    if (n > 0) BFQ_CUDA_TRY(launch_compact(cp, x->d_scan_tmp.p, &tmp_bytes, st, 1));
     exchange_meta_kernel<<<1, 1, 0, st>>>(x->d_meta.p + 2 * x->rank, (long long) n, x->d_begin.p, x->d_cnt.p);
-    X_CUDA(cudaGetLastError());
+    BFQ_CUDA_TRY(cudaGetLastError());
     // ---- 2. sizes of every rank (the receive counts NCCL needs on the host): the exchange's one host synchronisation
     X_NCCL(nccl().AllGather(x->d_meta.p + 2 * x->rank, x->d_meta.p, 2, ncclInt64, x->comm, st));
-    X_CUDA(cudaMemcpyAsync(x->h_meta, x->d_meta.p, (size_t) 2 * W * sizeof(long long), cudaMemcpyDeviceToHost, st));
-    X_CUDA(cudaStreamSynchronize(st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(x->h_meta.p, x->d_meta.p, (size_t) 2 * W * sizeof(long long), cudaMemcpyDeviceToHost, st));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
     // every rank's slice has the same (padded) stride, so the payload travels as plain ncclAllGather calls — the ring / NVLS
     // algorithms at full NVLink rate, where per-root broadcasts of exactly-sized slices would serialise the roots
     int64_t max_t = 1, max_r = 1;
     for (int r = 0; r < W; r++) {
-        max_t = std::max<int64_t>(max_t, x->h_meta[2 * r]);
-        max_r = std::max<int64_t>(max_r, x->h_meta[2 * r + 1]);
+        max_t = std::max<int64_t>(max_t, x->h_meta.p[2 * r]);
+        max_r = std::max<int64_t>(max_r, x->h_meta.p[2 * r + 1]);
     }
     max_t = (max_t + 31) / 32 * 32;   // keep every slice 128-byte aligned
     max_r = (max_r + 15) / 16 * 16;
@@ -233,29 +206,29 @@ int32_t bfq_exchange_gather(bfq_exchange* x, const bfq_device_result* res, int32
     for (int r = 0; r < W; r++) {
         x->topic_base[(size_t) r] = (int64_t) r * max_t;
         x->range_base[(size_t) r] = (int64_t) r * max_r;
-        x->topic_count[(size_t) r] = x->h_meta[2 * r];
-        x->range_count[(size_t) r] = x->h_meta[2 * r + 1];
-        nt_all += x->h_meta[2 * r];
-        nr_all += x->h_meta[2 * r + 1];
+        x->topic_count[(size_t) r] = x->h_meta.p[2 * r];
+        x->range_count[(size_t) r] = x->h_meta.p[2 * r + 1];
+        nt_all += x->h_meta.p[2 * r];
+        nr_all += x->h_meta.p[2 * r + 1];
     }
     x->topic_base[(size_t) W] = (int64_t) W * max_t;
     x->range_base[(size_t) W] = (int64_t) W * max_r;
-    if ((int64_t) W * max_r >= (int64_t) 0xFFFFFFF0ll) return xfail(BFQ_E_RANGE, "more than 2^32 ranges in one exchanged batch; split the batch");
-    X_CUDA(x->g_route_count.reserve((size_t) (W * max_t)));
+    if ((int64_t) W * max_r >= (int64_t) 0xFFFFFFF0ll) return fail(BFQ_E_RANGE, "more than 2^32 ranges in one exchanged batch; split the batch");
+    BFQ_CUDA_TRY(reserve_headroom(x->g_route_count, (size_t) (W * max_t)));
     if (with_ranges) {
-        X_CUDA(x->g_span_count.reserve((size_t) (W * max_t)));
-        X_CUDA(x->g_ranges.reserve((size_t) (W * max_r)));
+        BFQ_CUDA_TRY(reserve_headroom(x->g_span_count, (size_t) (W * max_t)));
+        BFQ_CUDA_TRY(reserve_headroom(x->g_ranges, (size_t) (W * max_r)));
     }
     // ---- 3. this rank's slice, written in place
     const int64_t tb = x->topic_base[(size_t) x->rank], rb = x->range_base[(size_t) x->rank];
     if (n > 0) {
-        X_CUDA(cudaMemcpyAsync(x->g_route_count.p + tb, res->d_route_count, (size_t) n * 4, cudaMemcpyDeviceToDevice, st));
+        BFQ_CUDA_TRY(cudaMemcpyAsync(x->g_route_count.p + tb, res->d_route_count, (size_t) n * 4, cudaMemcpyDeviceToDevice, st));
         if (with_ranges) {
-            X_CUDA(cudaMemcpyAsync(x->g_span_count.p + tb, x->d_cnt.p, (size_t) n * 4, cudaMemcpyDeviceToDevice, st));
+            BFQ_CUDA_TRY(cudaMemcpyAsync(x->g_span_count.p + tb, x->d_cnt.p, (size_t) n * 4, cudaMemcpyDeviceToDevice, st));
             cp.ranges_out = x->g_ranges.p + rb;
-            cp.ranges_out_cap = (uint64_t) x->h_meta[2 * x->rank + 1];
+            cp.ranges_out_cap = (uint64_t) x->h_meta.p[2 * x->rank + 1];
             cp.out_base = 0;
-            X_CUDA(launch_compact(cp, x->d_scan_tmp.p, &tmp_bytes, st, 2));
+            BFQ_CUDA_TRY(launch_compact(cp, x->d_scan_tmp.p, &tmp_bytes, st, 2));
         }
     }
     // ---- 4. every rank's slice to every rank: in-place all-gathers over the padded slices, one NCCL group
@@ -278,7 +251,7 @@ int32_t bfq_exchange_gather(bfq_exchange* x, const bfq_device_result* res, int32
     out->n_topics_total = nt_all;
     out->n_ranges_total = nr_all;
     out->world = W;
-    out->bytes_received = (nt_all - n) * (with_ranges ? 8 : 4) + (with_ranges ? (nr_all - x->h_meta[2 * x->rank + 1]) * 8 : 0);
+    out->bytes_received = (nt_all - n) * (with_ranges ? 8 : 4) + (with_ranges ? (nr_all - x->h_meta.p[2 * x->rank + 1]) * 8 : 0);
     return BFQ_OK;
 }
 

@@ -651,6 +651,28 @@ struct TopicQuads {
     }
 };
 
+// What the ordering kernels read: the caller's OrderParams with its scratch carved up by launch_order.
+struct OrderKernelParams {
+    int64_t n_topics;
+    const uint8_t* topics;
+    const int64_t* topic_off;
+    const int32_t* topic_tenant;
+    int32_t n_tenants;
+    uint32_t* keys;
+    uint32_t* leader;
+    uint32_t* order;
+    unsigned long long* hash_tab;
+    uint32_t hash_mask;
+    uint32_t* hist;                 // [n_buckets] zeroed; n_buckets = 2^hist_bits, a multiple of 4096
+    uint32_t* blk_tot;              // [n_buckets / 4096]
+    uint32_t* blk_pfx;              // [n_buckets / 4096]
+    uint32_t* ticket;               // zeroed
+    int hist_bits;
+    int dedup;
+    uint64_t dedup_hash_mask;
+    unsigned long long* counters;
+};
+
 constexpr int ORDER_WINDOW_QUADS = 3;
 constexpr int ORDER_WINDOW_WORDS = 4 * ORDER_WINDOW_QUADS;   // the order key looks at the first 48 bytes: three levels of ordinary topics end well before
 
@@ -682,7 +704,7 @@ __device__ __forceinline__ bool same_topic(const uint8_t* topics, int64_t oa, co
 
 // key = tenant index (T bits) | hash(level 0) | hash(levels 0..1) | hash(levels 0..2): equal leading levels => equal digits =>
 // one bucket. Hash collisions only merge groups. Topics with fewer levels use digit 0.
-__global__ void __launch_bounds__(256, 4) order_prep_kernel(const OrderParams q, int tenant_bits, int key_bits) {
+__global__ void __launch_bounds__(256, 4) order_prep_kernel(const OrderKernelParams q, int tenant_bits, int key_bits) {
     const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= q.n_topics) return;
     const int64_t o = q.topic_off[i];
@@ -812,7 +834,7 @@ __device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t v, uint32_t* w
     __syncthreads();
     return r;
 }
-__global__ void __launch_bounds__(SCAN_THREADS) order_scan_kernel(const OrderParams q) {
+__global__ void __launch_bounds__(SCAN_THREADS) order_scan_kernel(const OrderKernelParams q) {
     __shared__ uint32_t warp_sums[33];
     __shared__ bool is_last;
     uint4* hv = reinterpret_cast<uint4*>(q.hist + (size_t) blockIdx.x * SCAN_PER_BLOCK) + threadIdx.x;
@@ -833,7 +855,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) order_scan_kernel(const OrderPar
     if (threadIdx.x < gridDim.x) q.blk_pfx[threadIdx.x] = pfx;
     if (threadIdx.x == 0) q.counters[CTR_NLEAD] = total;
 }
-__global__ void __launch_bounds__(256) order_scatter_kernel(const OrderParams q) {
+__global__ void __launch_bounds__(256) order_scatter_kernel(const OrderKernelParams q) {
     const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= q.n_topics || q.leader[i] != (uint32_t) i) return;
     const uint32_t b = q.keys[i];
@@ -1269,21 +1291,34 @@ static int order_hist_bits(int64_t n_topics, int32_t n_tenants) {
     while (nb < 22 && (1ll << nb) < 4 * n_topics) nb++;
     return std::max(12, std::min(nb, order_key_bits(order_tenant_bits(n_tenants))));
 }
-size_t order_hist_buckets(int64_t n_topics, int32_t n_tenants) { return (size_t) 1 << order_hist_bits(n_topics, n_tenants); }
+// the scratch of one ordering: histogram | block totals | block prefixes | ticket (kept 256-byte aligned)
+size_t order_scratch_words(int64_t n_topics, int32_t n_tenants) {
+    const size_t buckets = (size_t) 1 << order_hist_bits(n_topics, n_tenants);
+    return (buckets + 2 * (buckets / SCAN_PER_BLOCK) + 64 + 63) / 64 * 64;
+}
 uint32_t order_hash_entries(int64_t n_topics) {
     uint32_t e = 1024;
     while (e < (1u << 31) && (int64_t) e < 2 * n_topics) e <<= 1;
     return e;
 }
 
-cudaError_t launch_order(const OrderParams& q, cudaStream_t stream) {
-    const int64_t n = q.n_topics;
+cudaError_t launch_order(const OrderParams& p, cudaStream_t stream) {
+    const int64_t n = p.n_topics;
     if (n <= 0) return cudaSuccess;
+    const int hist_bits = order_hist_bits(n, p.n_tenants);
+    const size_t buckets = (size_t) 1 << hist_bits, scan_blocks = buckets / SCAN_PER_BLOCK;
+    uint32_t* blk_tot = p.hist + buckets;
+    const OrderKernelParams q{p.n_topics, p.topics, p.topic_off, p.topic_tenant, p.n_tenants, p.keys, p.leader, p.order,
+                              p.hash_tab, p.hash_mask, p.hist, blk_tot, blk_tot + scan_blocks, blk_tot + 2 * scan_blocks, hist_bits,
+                              p.dedup, p.dedup_hash_mask, p.counters};
+    cudaError_t e = cudaMemsetAsync(q.hist, 0, order_scratch_words(n, p.n_tenants) * sizeof(uint32_t), stream);
+    if (e == cudaSuccess && q.dedup) e = cudaMemsetAsync(q.hash_tab, 0xFF, ((size_t) q.hash_mask + 1) * sizeof(unsigned long long), stream);
+    if (e != cudaSuccess) return e;
     const int tenant_bits = order_tenant_bits(q.n_tenants);
     const int kb = order_key_bits(tenant_bits);
     const unsigned blocks = (unsigned) ((n + 255) / 256);
     order_prep_kernel<<<blocks, 256, 0, stream>>>(q, tenant_bits, kb);
-    order_scan_kernel<<<(unsigned) (((size_t) 1 << q.hist_bits) / SCAN_PER_BLOCK), SCAN_THREADS, 0, stream>>>(q);
+    order_scan_kernel<<<(unsigned) scan_blocks, SCAN_THREADS, 0, stream>>>(q);
     order_scatter_kernel<<<blocks, 256, 0, stream>>>(q);
     return cudaGetLastError();
 }

@@ -150,7 +150,7 @@ cudaError_t launch_budget(const BudgetParams& q, void* d_scan_tmp, size_t* tmp_b
 //   prep     one thread per topic: 64-bit hash of (tenant, topic bytes) -> insert into an open-addressing table; the first
 //            inserter of a (tenant, topic) pair is its LEADER, later identical ones (verified byte by byte) are followers that
 //            only remember their leader. Leaders get an order key = tenant index | hashes of the level-0 / 0..1 / 0..2 prefixes
-//            and count themselves into a bucket histogram (bucket = the key's leading hist_bits).
+//            and count themselves into a bucket histogram (bucket = the key's leading bits).
 //   scan     exclusive prefix sum of the histogram (block-local scans; the last block to finish scans the block totals)
 //   scatter  leaders -> order[bucket base + atomic cursor]: a counting sort, unstable inside a bucket (only grouping matters)
 // Tier 0 then matches order[0 .. n_leaders) — topics that walk the same top of the trie are matched by neighbouring lanes at
@@ -166,19 +166,16 @@ struct OrderParams {
     uint32_t* keys;                 // [n] bucket of each leader
     uint32_t* leader;               // [n] out: i for a leader, else the index of the identical topic that leads
     uint32_t* order;                // [n] out: the leaders, grouped by bucket
-    unsigned long long* hash_tab;   // [hash_mask + 1] pre-set to 0xFF bytes
+    unsigned long long* hash_tab;   // [hash_mask + 1], filled with 0xFF bytes by launch_order when dedup is set
     uint32_t hash_mask;
-    uint32_t* hist;                 // [n_buckets] zeroed; n_buckets = 2^hist_bits, a multiple of 4096
-    uint32_t* blk_tot;              // [n_buckets / 4096]
-    uint32_t* blk_pfx;              // [n_buckets / 4096]
-    uint32_t* ticket;               // zeroed
-    int hist_bits;
+    uint32_t* hist;                 // [order_scratch_words(n_topics, n_tenants)] scratch, zeroed and laid out by launch_order
     int dedup;                      // 0: every topic is its own leader
     uint64_t dedup_hash_mask;       // bits of the de-dup hash kept after fmix64 (all of them but in tests: forced collisions)
     unsigned long long* counters;   // CTR_NLEAD is written by the scan
 };
-size_t order_hist_buckets(int64_t n_topics, int32_t n_tenants);   // histogram entries launch_order will use
-uint32_t order_hash_entries(int64_t n_topics);                    // dedup table entries (power of two)
+size_t order_scratch_words(int64_t n_topics, int32_t n_tenants);   // 32-bit words of scratch launch_order needs
+uint32_t order_hash_entries(int64_t n_topics);                     // dedup table entries (power of two)
+// enqueues the scratch and hash-table fills and the three kernels on stream
 cudaError_t launch_order(const OrderParams& q, cudaStream_t stream);
 
 // followers copy their leader's span (and join the flagged list if it needs caps). second_pass: only the followers whose

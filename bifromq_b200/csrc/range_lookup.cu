@@ -25,10 +25,10 @@
 #include <vector>
 
 #include "../../include/bfq_gpumatch.h"
+#include "cuda_buf.h"
 
-namespace bfq {
-int32_t set_error(int32_t code, const std::string& msg);
-}
+using bfq::DeviceBuf;
+using bfq::fail;
 
 namespace {
 
@@ -239,16 +239,6 @@ __global__ void __launch_bounds__(128) range_lookup_kernel(int64_t n_pairs, cons
     out[j] = (exact || r <= 0) ? 1 : 0;
 }
 
-int32_t rl_fail(int32_t code, const std::string& msg) { return bfq::set_error(code, msg); }
-#define RL_CUDA(expr)                                                                               \
-    do {                                                                                            \
-        cudaError_t _e = (expr);                                                                    \
-        if (_e != cudaSuccess) {                                                                    \
-            for (void* q : allocs) cudaFree(q);                                                     \
-            return rl_fail(BFQ_E_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e));         \
-        }                                                                                           \
-    } while (0)
-
 }  // namespace
 
 extern "C" int32_t bfq_range_lookup(int32_t device_ordinal, const uint8_t* tenants, const int64_t* tenant_off, int32_t n_tenants,
@@ -257,51 +247,48 @@ extern "C" int32_t bfq_range_lookup(int32_t device_ordinal, const uint8_t* tenan
                                     const uint8_t* last_blob, const int64_t* last_off, int64_t* keep_off_out, uint8_t* keep_out) {
     if (n_tenants < 0 || n_topics < 0 || !keep_off_out || (n_topics > 0 && (!topics || !topic_off || !topic_tenant || !keep_out)) ||
         (n_tenants > 0 && (!tenants || !tenant_off || !cand_off)))
-        return rl_fail(BFQ_E_INVALID, "bad argument");
+        return fail(BFQ_E_INVALID, "bad argument");
     const int64_t n_cand = n_tenants ? cand_off[n_tenants] : 0;
-    if (n_cand > 0 && (!cand_flags || !first_off || !last_off)) return rl_fail(BFQ_E_INVALID, "NULL candidate arrays");
+    if (n_cand > 0 && (!cand_flags || !first_off || !last_off)) return fail(BFQ_E_INVALID, "NULL candidate arrays");
     // rows: topic i has one cell per candidate of its tenant
     keep_off_out[0] = 0;
     for (int64_t i = 0; i < n_topics; i++) {
         const int t = topic_tenant[i];
-        if (t < 0 || t >= n_tenants) return rl_fail(BFQ_E_RANGE, "topic_tenant out of range");
+        if (t < 0 || t >= n_tenants) return fail(BFQ_E_RANGE, "topic_tenant out of range");
         keep_off_out[i + 1] = keep_off_out[i] + (cand_off[t + 1] - cand_off[t]);
     }
     const int64_t n_pairs = keep_off_out[n_topics];
     if (n_pairs == 0) return BFQ_OK;
-    std::vector<void*> allocs;
-    RL_CUDA(cudaSetDevice(device_ordinal));
-    auto up = [&](const void* src, size_t bytes, void** dst) -> cudaError_t {
-        cudaError_t e = cudaMalloc(dst, std::max<size_t>(bytes, 16));
+    BFQ_CUDA_TRY(cudaSetDevice(device_ordinal));
+    // every input is uploaded into a buffer of its own, of at least 16 bytes
+    auto up = [](const void* src, size_t bytes, DeviceBuf<uint8_t>* dst) -> cudaError_t {
+        cudaError_t e = dst->reserve(std::max<size_t>(bytes, 16));
         if (e != cudaSuccess) return e;
-        allocs.push_back(*dst);
-        return bytes ? cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice) : cudaSuccess;
+        return bytes ? cudaMemcpy(dst->p, src, bytes, cudaMemcpyHostToDevice) : cudaSuccess;
     };
-    void *d_pair_off, *d_topics, *d_topic_off, *d_tt, *d_tenants, *d_tenant_off, *d_cand_off, *d_first, *d_first_off, *d_last, *d_last_off, *d_out;
-    RL_CUDA(up(keep_off_out, (size_t) (n_topics + 1) * 8, &d_pair_off));
-    RL_CUDA(up(topics + topic_off[0], (size_t) (topic_off[n_topics] - topic_off[0]), &d_topics));
+    DeviceBuf<uint8_t> d_pair_off, d_topics, d_topic_off, d_tt, d_tenants, d_tenant_off, d_cand_off, d_first, d_first_off, d_last,
+        d_last_off, d_out;
+    BFQ_CUDA_TRY(up(keep_off_out, (size_t) (n_topics + 1) * 8, &d_pair_off));
+    BFQ_CUDA_TRY(up(topics + topic_off[0], (size_t) (topic_off[n_topics] - topic_off[0]), &d_topics));
     std::vector<int64_t> toff((size_t) n_topics + 1);
     for (int64_t i = 0; i <= n_topics; i++) toff[(size_t) i] = topic_off[i] - topic_off[0];
-    RL_CUDA(up(toff.data(), toff.size() * 8, &d_topic_off));
-    RL_CUDA(up(topic_tenant, (size_t) n_topics * 4, &d_tt));
-    RL_CUDA(up(tenants, (size_t) tenant_off[n_tenants], &d_tenants));
-    RL_CUDA(up(tenant_off, (size_t) (n_tenants + 1) * 8, &d_tenant_off));
-    RL_CUDA(up(cand_off, (size_t) (n_tenants + 1) * 8, &d_cand_off));
-    RL_CUDA(up(first_blob, (size_t) first_off[n_cand], &d_first));
-    RL_CUDA(up(first_off, (size_t) (n_cand + 1) * 8, &d_first_off));
-    RL_CUDA(up(last_blob, (size_t) last_off[n_cand], &d_last));
-    RL_CUDA(up(last_off, (size_t) (n_cand + 1) * 8, &d_last_off));
-    RL_CUDA(cudaMalloc(&d_out, (size_t) n_pairs));
-    allocs.push_back(d_out);
-    range_lookup_kernel<<<(unsigned) ((n_pairs + 127) / 128), 128>>>(n_pairs, (const int64_t*) d_pair_off, n_topics, (const uint8_t*) d_topics,
-                                                                    (const int64_t*) d_topic_off, (const int32_t*) d_tt, (const uint8_t*) d_tenants,
-                                                                    (const int64_t*) d_tenant_off, (const int64_t*) d_cand_off,
-                                                                    (const uint8_t*) d_first, (const int64_t*) d_first_off, (const uint8_t*) d_last,
-                                                                    (const int64_t*) d_last_off, (uint8_t*) d_out);
-    RL_CUDA(cudaGetLastError());
-    RL_CUDA(cudaMemcpy(keep_out, d_out, (size_t) n_pairs, cudaMemcpyDeviceToHost));
-    for (void* q : allocs) cudaFree(q);
-    allocs.clear();
+    BFQ_CUDA_TRY(up(toff.data(), toff.size() * 8, &d_topic_off));
+    BFQ_CUDA_TRY(up(topic_tenant, (size_t) n_topics * 4, &d_tt));
+    BFQ_CUDA_TRY(up(tenants, (size_t) tenant_off[n_tenants], &d_tenants));
+    BFQ_CUDA_TRY(up(tenant_off, (size_t) (n_tenants + 1) * 8, &d_tenant_off));
+    BFQ_CUDA_TRY(up(cand_off, (size_t) (n_tenants + 1) * 8, &d_cand_off));
+    BFQ_CUDA_TRY(up(first_blob, (size_t) first_off[n_cand], &d_first));
+    BFQ_CUDA_TRY(up(first_off, (size_t) (n_cand + 1) * 8, &d_first_off));
+    BFQ_CUDA_TRY(up(last_blob, (size_t) last_off[n_cand], &d_last));
+    BFQ_CUDA_TRY(up(last_off, (size_t) (n_cand + 1) * 8, &d_last_off));
+    BFQ_CUDA_TRY(d_out.reserve((size_t) n_pairs));
+    range_lookup_kernel<<<(unsigned) ((n_pairs + 127) / 128), 128>>>(n_pairs, (const int64_t*) d_pair_off.p, n_topics, d_topics.p,
+                                                                    (const int64_t*) d_topic_off.p, (const int32_t*) d_tt.p, d_tenants.p,
+                                                                    (const int64_t*) d_tenant_off.p, (const int64_t*) d_cand_off.p,
+                                                                    d_first.p, (const int64_t*) d_first_off.p, d_last.p,
+                                                                    (const int64_t*) d_last_off.p, d_out.p);
+    BFQ_CUDA_TRY(cudaGetLastError());
+    BFQ_CUDA_TRY(cudaMemcpy(keep_out, d_out.p, (size_t) n_pairs, cudaMemcpyDeviceToHost));
     // the reference's candidate loop (TenantRangeLookupCache.java:78-104): a range without a Fact is kept, one whose Fact lacks
     // first or last is empty (skipped), and the first range whose seek runs past the end ends the scan
     for (int64_t i = 0; i < n_topics; i++) {

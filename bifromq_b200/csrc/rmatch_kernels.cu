@@ -37,6 +37,7 @@
 
 #include "../../include/bfq_gpumatch.h"
 #include "codec.h"
+#include "cuda_buf.h"
 #include "trie_layout.h"
 #include "hash_probe.cuh"
 #include "match_kernels.cuh"
@@ -44,13 +45,6 @@
 using namespace bfq;
 
 namespace {
-
-int32_t rfail(int32_t code, const std::string& msg) { return bfq::set_error(code, msg); }
-#define RCUDA_TRY(expr)                                                                         \
-    do {                                                                                        \
-        cudaError_t _e = (expr);                                                                \
-        if (_e != cudaSuccess) return rfail(BFQ_E_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e)); \
-    } while (0)
 
 // one topic-trie node, indexed by node id; the node array has a sentinel entry at [n_nodes]
 struct RNode {
@@ -496,45 +490,6 @@ __global__ void __launch_bounds__(256) rinsert_edges_kernel(const Slot* __restri
     }
 }
 
-template <typename T>
-struct DBuf {
-    T* p = nullptr;
-    size_t cap = 0;
-    cudaError_t reserve(size_t n) {
-        if (n <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        cudaError_t e = cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T));
-        if (e == cudaSuccess) cap = n;
-        return e;
-    }
-    // like reserve, but keeps the first `keep` elements (device-to-device copy on st) and grows by at least half the capacity
-    cudaError_t grow(size_t n, size_t keep, cudaStream_t st) {
-        if (n <= cap) return cudaSuccess;
-        const size_t want = std::max(n, cap + cap / 2);
-        T* q = nullptr;
-        cudaError_t e = cudaMalloc(&q, want * sizeof(T));
-        if (e != cudaSuccess) return e;
-        if (keep) e = cudaMemcpyAsync(q, p, keep * sizeof(T), cudaMemcpyDeviceToDevice, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) {
-            cudaFree(q);
-            return e;
-        }
-        if (p) cudaFree(p);
-        p = q;
-        cap = want;
-        return cudaSuccess;
-    }
-    size_t bytes() const { return cap * sizeof(T); }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
-};
-
 }  // namespace
 
 // id -> (tenant, topic); tombstones keep their slot. bfq_rindex_reset starts a new table, so ids restart at 0 there while the
@@ -559,7 +514,7 @@ struct bfq_rindex {
     std::mutex mu;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};   // [0,1] around all kernels of a match, [2,3] around rmatch_kernel
-    unsigned long long* h_small = nullptr;   // pinned scalars
+    PinnedBuf<unsigned long long> h_small;   // pinned scalars
     // staging: (tenant, topic) -> id ; id -> (tenant, topic)
     std::map<std::pair<std::string, std::string>, int64_t> staged;
     std::shared_ptr<IdTable> by_id = std::make_shared<IdTable>();   // staging: add / load_keys append here
@@ -579,22 +534,22 @@ struct bfq_rindex {
     int64_t used_slots = 0;                // occupied table slots, garbage included
     int64_t overflowed_blocks = 0;
     int64_t full_commits = 0, delta_commits = 0, last_rebuilt = 0;
-    DBuf<RNode> d_nodes;
-    DBuf<Slot> d_slots;
-    DBuf<uint8_t> d_tags;
-    DBuf<int64_t> d_dfs_to_id, d_bfs_to_id;
-    DBuf<Slot> d_new_slots;                // slot images of a delta commit
-    DBuf<unsigned long long> d_ins_ctr;
+    DeviceBuf<RNode> d_nodes;
+    DeviceBuf<Slot> d_slots;
+    DeviceBuf<uint8_t> d_tags;
+    DeviceBuf<int64_t> d_dfs_to_id, d_bfs_to_id;
+    DeviceBuf<Slot> d_new_slots;                // slot images of a delta commit
+    DeviceBuf<unsigned long long> d_ins_ctr;
     // workspace
-    DBuf<uint8_t> d_filters, d_scan_tmp;
-    DBuf<int64_t> d_filter_off, d_limit, d_ids;
-    DBuf<int32_t> d_filter_tenant, d_tenant_root;
-    DBuf<uint32_t> d_span_begin, d_span_count, d_overflow;
-    DBuf<unsigned long long> d_total, d_kept, d_offsets, d_counters;
-    DBuf<uint2> d_ranges, d_scratch;
+    DeviceBuf<uint8_t> d_filters, d_scan_tmp;
+    DeviceBuf<int64_t> d_filter_off, d_limit, d_ids;
+    DeviceBuf<int32_t> d_filter_tenant, d_tenant_root;
+    DeviceBuf<uint32_t> d_span_begin, d_span_count, d_overflow;
+    DeviceBuf<unsigned long long> d_total, d_kept, d_offsets, d_counters;
+    DeviceBuf<uint2> d_ranges, d_scratch;
     // locality order of a batch of filters (match_kernels.cu: launch_order, without de-duplication)
-    DBuf<uint32_t> d_ord_keys, d_ord_leader, d_order, d_hist;
-    DBuf<unsigned long long> d_ord_ctr;
+    DeviceBuf<uint32_t> d_ord_keys, d_ord_leader, d_order, d_hist;
+    DeviceBuf<unsigned long long> d_ord_ctr;
     int64_t launches = 0;
 
     int64_t device_bytes() const {
@@ -607,15 +562,8 @@ struct bfq_rindex {
     }
 
     ~bfq_rindex() {
-        cudaSetDevice(device);
-        d_nodes.release(); d_slots.release(); d_tags.release(); d_dfs_to_id.release(); d_bfs_to_id.release(); d_filters.release();
-        d_scan_tmp.release(); d_filter_off.release(); d_limit.release(); d_ids.release(); d_filter_tenant.release();
-        d_tenant_root.release(); d_span_begin.release(); d_span_count.release(); d_overflow.release(); d_total.release();
-        d_kept.release(); d_offsets.release(); d_counters.release(); d_ranges.release(); d_scratch.release();
-        d_ord_keys.release(); d_ord_leader.release(); d_order.release(); d_hist.release(); d_ord_ctr.release();
-        d_new_slots.release(); d_ins_ctr.release();
+        cudaSetDevice(device);   // the buffers are freed after this body, on this device
         for (auto& e : ev) if (e) cudaEventDestroy(e);
-        if (h_small) cudaFreeHost(h_small);
         if (stream) cudaStreamDestroy(stream);
     }
 };
@@ -679,7 +627,7 @@ int32_t build_tenant(Staged::const_iterator first, Staged::const_iterator last, 
         nodes[cur].own = it->second;
     }
     const size_t N = nodes.size();
-    if (N >= ID_LIMIT) return rfail(BFQ_E_RANGE, "topic index too large");
+    if (N >= ID_LIMIT) return fail(BFQ_E_RANGE, "topic index too large");
     // ---- BFS numbering from the root, level by level in parent order
     std::vector<uint32_t> order;
     order.reserve(N);
@@ -767,7 +715,7 @@ int32_t build_tenant(Staged::const_iterator first, Staged::const_iterator last, 
                 auto vk = std::make_tuple(parent, LEN_CONT | j, std::string(chunk));
                 auto vit = virt.find(vk);
                 if (vit == virt.end()) {
-                    if (next_virtual >= VIRT_LIMIT) return rfail(BFQ_E_RANGE, "topic index too large");
+                    if (next_virtual >= VIRT_LIMIT) return fail(BFQ_E_RANGE, "topic index too large");
                     const uint32_t v = (uint32_t) next_virtual++;
                     slots.push_back(slot_of(parent, LEN_CONT | j, chunk, v));
                     virt.emplace(std::move(vk), v);
@@ -824,7 +772,7 @@ int32_t rebuild_full(bfq_rindex* h) {
                                         (uint32_t) bfs_to_id.size(), (uint32_t) next_virtual, &im);
         if (rc != BFQ_OK) return rc;
         if (rn.size() + im.rn.size() + 1 >= ID_LIMIT || dfs_to_id.size() + im.dfs_to_id.size() >= ID_LIMIT)
-            return rfail(BFQ_E_RANGE, "topic index too large");
+            return fail(BFQ_E_RANGE, "topic index too large");
         TenantRegion reg;
         reg.root = (uint32_t) rn.size();
         reg.n_nodes = (uint32_t) im.rn.size();
@@ -840,26 +788,26 @@ int32_t rebuild_full(bfq_rindex* h) {
     }
     const size_t N = rn.size();
     rn.push_back(RNode{(uint32_t) N, 0, 0, 0, (uint32_t) bfs_to_id.size(), 0, 0, 0});   // the sentinel
-    if (((uint64_t) imgs.size() * 2 / BLOCK_USABLE + 64) * BLOCK_SLOTS >= ID_LIMIT) return rfail(BFQ_E_RANGE, "topic index too large");
+    if (((uint64_t) imgs.size() * 2 / BLOCK_USABLE + 64) * BLOCK_SLOTS >= ID_LIMIT) return fail(BFQ_E_RANGE, "topic index too large");
     EdgeTable table;
     table.init(imgs.size());
     for (const Slot& s : imgs) table.slots[table.place(s.w[W_PARENT], s.w[W_LEN], &s.w[W_TOK])] = s;
     SlotVec& slots = table.slots;
     // ---- upload
-    RCUDA_TRY(cudaSetDevice(h->device));
-    RCUDA_TRY(cudaStreamSynchronize(h->stream));
+    BFQ_CUDA_TRY(cudaSetDevice(h->device));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(h->stream));
     h->need_full = true;   // until the upload is complete
-    RCUDA_TRY(h->d_nodes.reserve(rn.size()));
-    RCUDA_TRY(h->d_slots.reserve(slots.size()));
-    RCUDA_TRY(h->d_tags.reserve(table.tags.size()));
-    RCUDA_TRY(h->d_dfs_to_id.reserve(std::max<size_t>(dfs_to_id.size(), 1)));
-    RCUDA_TRY(h->d_bfs_to_id.reserve(std::max<size_t>(bfs_to_id.size(), 1)));
-    RCUDA_TRY(cudaMemcpy(h->d_nodes.p, rn.data(), rn.size() * sizeof(RNode), cudaMemcpyHostToDevice));
-    RCUDA_TRY(cudaMemcpy(h->d_slots.p, slots.data(), slots.size() * sizeof(Slot), cudaMemcpyHostToDevice));
-    RCUDA_TRY(cudaMemcpy(h->d_tags.p, table.tags.data(), table.tags.size(), cudaMemcpyHostToDevice));
+    BFQ_CUDA_TRY(h->d_nodes.reserve(rn.size()));
+    BFQ_CUDA_TRY(h->d_slots.reserve(slots.size()));
+    BFQ_CUDA_TRY(h->d_tags.reserve(table.tags.size()));
+    BFQ_CUDA_TRY(h->d_dfs_to_id.reserve(std::max<size_t>(dfs_to_id.size(), 1)));
+    BFQ_CUDA_TRY(h->d_bfs_to_id.reserve(std::max<size_t>(bfs_to_id.size(), 1)));
+    BFQ_CUDA_TRY(cudaMemcpy(h->d_nodes.p, rn.data(), rn.size() * sizeof(RNode), cudaMemcpyHostToDevice));
+    BFQ_CUDA_TRY(cudaMemcpy(h->d_slots.p, slots.data(), slots.size() * sizeof(Slot), cudaMemcpyHostToDevice));
+    BFQ_CUDA_TRY(cudaMemcpy(h->d_tags.p, table.tags.data(), table.tags.size(), cudaMemcpyHostToDevice));
     if (!dfs_to_id.empty()) {
-        RCUDA_TRY(cudaMemcpy(h->d_dfs_to_id.p, dfs_to_id.data(), dfs_to_id.size() * 8, cudaMemcpyHostToDevice));
-        RCUDA_TRY(cudaMemcpy(h->d_bfs_to_id.p, bfs_to_id.data(), bfs_to_id.size() * 8, cudaMemcpyHostToDevice));
+        BFQ_CUDA_TRY(cudaMemcpy(h->d_dfs_to_id.p, dfs_to_id.data(), dfs_to_id.size() * 8, cudaMemcpyHostToDevice));
+        BFQ_CUDA_TRY(cudaMemcpy(h->d_bfs_to_id.p, bfs_to_id.data(), bfs_to_id.size() * 8, cudaMemcpyHostToDevice));
     }
     h->tenant_root.clear();
     for (const auto& e : regions) h->tenant_root[e.first] = (int32_t) e.second.root;
@@ -938,32 +886,32 @@ int32_t commit_delta(bfq_rindex* h) {
     if (used * OCCUPANCY_DEN > (int64_t) h->n_blocks * BLOCK_USABLE * OCCUPANCY_NUM) return NEED_FULL;
     // ---- device patch, on the handle's stream, finished before the handle lock is released
     cudaStream_t st = h->stream;
-    RCUDA_TRY(cudaSetDevice(h->device));
+    BFQ_CUDA_TRY(cudaSetDevice(h->device));
     h->need_full = true;   // until the patch is complete: a failed patch leaves the device arrays to the next full build
-    RCUDA_TRY(h->d_nodes.grow(n_nodes + 1, node0, st));   // the old sentinel is overwritten by the first appended root
-    RCUDA_TRY(h->d_dfs_to_id.grow(std::max<uint64_t>(n_dfs, 1), dfs0, st));
-    RCUDA_TRY(h->d_bfs_to_id.grow(std::max<uint64_t>(n_bfs, 1), bfs0, st));
+    BFQ_CUDA_TRY(h->d_nodes.grow(n_nodes + 1, node0, st));   // the old sentinel is overwritten by the first appended root
+    BFQ_CUDA_TRY(h->d_dfs_to_id.grow(std::max<uint64_t>(n_dfs, 1), dfs0, st));
+    BFQ_CUDA_TRY(h->d_bfs_to_id.grow(std::max<uint64_t>(n_bfs, 1), bfs0, st));
     rn.push_back(RNode{(uint32_t) n_nodes, 0, 0, 0, (uint32_t) n_bfs, 0, 0, 0});   // the new sentinel
-    RCUDA_TRY(cudaMemcpyAsync(h->d_nodes.p + node0, rn.data(), rn.size() * sizeof(RNode), cudaMemcpyHostToDevice, st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(h->d_nodes.p + node0, rn.data(), rn.size() * sizeof(RNode), cudaMemcpyHostToDevice, st));
     if (!dfs_to_id.empty()) {
-        RCUDA_TRY(cudaMemcpyAsync(h->d_dfs_to_id.p + dfs0, dfs_to_id.data(), dfs_to_id.size() * 8, cudaMemcpyHostToDevice, st));
-        RCUDA_TRY(cudaMemcpyAsync(h->d_bfs_to_id.p + bfs0, bfs_to_id.data(), bfs_to_id.size() * 8, cudaMemcpyHostToDevice, st));
+        BFQ_CUDA_TRY(cudaMemcpyAsync(h->d_dfs_to_id.p + dfs0, dfs_to_id.data(), dfs_to_id.size() * 8, cudaMemcpyHostToDevice, st));
+        BFQ_CUDA_TRY(cudaMemcpyAsync(h->d_bfs_to_id.p + bfs0, bfs_to_id.data(), bfs_to_id.size() * 8, cudaMemcpyHostToDevice, st));
     }
     unsigned long long overflowed = 0;
     if (!imgs.empty()) {
-        RCUDA_TRY(h->d_new_slots.reserve(imgs.size()));
-        RCUDA_TRY(h->d_ins_ctr.reserve(1));
-        RCUDA_TRY(cudaMemcpyAsync(h->d_new_slots.p, imgs.data(), imgs.size() * sizeof(Slot), cudaMemcpyHostToDevice, st));
-        RCUDA_TRY(cudaMemsetAsync(h->d_ins_ctr.p, 0, sizeof(unsigned long long), st));
+        BFQ_CUDA_TRY(h->d_new_slots.reserve(imgs.size()));
+        BFQ_CUDA_TRY(h->d_ins_ctr.reserve(1));
+        BFQ_CUDA_TRY(cudaMemcpyAsync(h->d_new_slots.p, imgs.data(), imgs.size() * sizeof(Slot), cudaMemcpyHostToDevice, st));
+        BFQ_CUDA_TRY(cudaMemsetAsync(h->d_ins_ctr.p, 0, sizeof(unsigned long long), st));
         const int64_t n = (int64_t) imgs.size();
         rinsert_edges_kernel<<<(unsigned) ((n + 255) / 256), 256, 0, st>>>(h->d_new_slots.p, n, h->d_slots.p,
                                                                            reinterpret_cast<uint32_t*>(h->d_tags.p), h->n_blocks,
                                                                            h->d_ins_ctr.p);
         h->launches++;
-        RCUDA_TRY(cudaGetLastError());
-        RCUDA_TRY(cudaMemcpyAsync(&overflowed, h->d_ins_ctr.p, sizeof(overflowed), cudaMemcpyDeviceToHost, st));
+        BFQ_CUDA_TRY(cudaGetLastError());
+        BFQ_CUDA_TRY(cudaMemcpyAsync(&overflowed, h->d_ins_ctr.p, sizeof(overflowed), cudaMemcpyDeviceToHost, st));
     }
-    RCUDA_TRY(cudaStreamSynchronize(st));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
     // ---- publish
     for (const std::string& t : gone) {
         h->regions.erase(t);
@@ -994,18 +942,18 @@ int32_t commit_delta(bfq_rindex* h) {
 extern "C" {
 
 int32_t bfq_rindex_create(int32_t device_ordinal, bfq_rindex** out) {
-    if (!out) return rfail(BFQ_E_INVALID, "out is NULL");
+    if (!out) return fail(BFQ_E_INVALID, "out is NULL");
     int count = 0;
     cudaError_t e = cudaGetDeviceCount(&count);
     if (e != cudaSuccess || count == 0)
-        return rfail(BFQ_E_CUDA, std::string("no usable CUDA device (there is no CPU fallback): ") + cudaGetErrorString(e));
-    if (device_ordinal < 0 || device_ordinal >= count) return rfail(BFQ_E_INVALID, "device ordinal out of range");
-    RCUDA_TRY(cudaSetDevice(device_ordinal));
+        return fail(BFQ_E_CUDA, std::string("no usable CUDA device (there is no CPU fallback): ") + cudaGetErrorString(e));
+    if (device_ordinal < 0 || device_ordinal >= count) return fail(BFQ_E_INVALID, "device ordinal out of range");
+    BFQ_CUDA_TRY(cudaSetDevice(device_ordinal));
     auto* h = new bfq_rindex();
     h->device = device_ordinal;
     if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) {
         delete h;
-        return rfail(BFQ_E_CUDA, "cudaStreamCreate failed");
+        return fail(BFQ_E_CUDA, "cudaStreamCreate failed");
     }
     *out = h;
     return BFQ_OK;
@@ -1013,7 +961,7 @@ int32_t bfq_rindex_create(int32_t device_ordinal, bfq_rindex** out) {
 void bfq_rindex_destroy(bfq_rindex* h) { delete h; }
 
 int32_t bfq_rindex_reset(bfq_rindex* h) {
-    if (!h) return rfail(BFQ_E_INVALID, "handle is NULL");
+    if (!h) return fail(BFQ_E_INVALID, "handle is NULL");
     std::lock_guard<std::mutex> g(h->mu);
     h->staged.clear();
     h->by_id = std::make_shared<IdTable>();   // the committed table stays with the snapshot and its results
@@ -1025,12 +973,12 @@ int32_t bfq_rindex_reset(bfq_rindex* h) {
 
 int32_t bfq_rindex_add(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_off, int32_t n_tenants,
                        const uint8_t* topics, const int64_t* topic_off, const int32_t* topic_tenant, int64_t n, int64_t* ids_out) {
-    if (!h || n < 0 || n_tenants < 0) return rfail(BFQ_E_INVALID, "bad argument");
+    if (!h || n < 0 || n_tenants < 0) return fail(BFQ_E_INVALID, "bad argument");
     std::lock_guard<std::mutex> g(h->mu);
     std::vector<std::string> ts((size_t) n_tenants);
     for (int32_t t = 0; t < n_tenants; t++) ts[(size_t) t].assign((const char*) tenants + tenant_off[t], (size_t) (tenant_off[t + 1] - tenant_off[t]));
     for (int64_t i = 0; i < n; i++) {
-        if (topic_tenant[i] < 0 || topic_tenant[i] >= n_tenants) return rfail(BFQ_E_RANGE, "topic_tenant out of range");
+        if (topic_tenant[i] < 0 || topic_tenant[i] >= n_tenants) return fail(BFQ_E_RANGE, "topic_tenant out of range");
         std::pair<std::string, std::string> key(ts[(size_t) topic_tenant[i]],
                                                 std::string((const char*) topics + topic_off[i], (size_t) (topic_off[i + 1] - topic_off[i])));
         auto it = h->staged.find(key);
@@ -1054,7 +1002,7 @@ int32_t bfq_rindex_add(bfq_rindex* h, const uint8_t* tenants, const int64_t* ten
 // so the index is fed from the keys alone. ids_out[i] < 0 marks a key that is not a retain key (skipped, as the reference logs
 // and skips an unparsable entry).
 int32_t bfq_rindex_load_keys(bfq_rindex* h, const uint8_t* keys, const int64_t* key_off, int64_t n, int64_t* ids_out) {
-    if (!h || n < 0 || (n > 0 && (!keys || !key_off))) return rfail(BFQ_E_INVALID, "bad argument");
+    if (!h || n < 0 || (n > 0 && (!keys || !key_off))) return fail(BFQ_E_INVALID, "bad argument");
     std::lock_guard<std::mutex> g(h->mu);
     if (h->staged.empty()) h->need_full = true;   // a bulk load onto an empty handle: one full build beats a delta per tenant
     for (int64_t i = 0; i < n; i++) {
@@ -1104,7 +1052,7 @@ int64_t bfq_rresult_retain_keys(bfq_rindex* h, const bfq_rresult* r, uint8_t* bl
 }
 
 int32_t bfq_rindex_remove(bfq_rindex* h, const uint8_t* tenant, int64_t tn, const uint8_t* topic, int64_t n) {
-    if (!h) return rfail(BFQ_E_INVALID, "handle is NULL");
+    if (!h) return fail(BFQ_E_INVALID, "handle is NULL");
     std::lock_guard<std::mutex> g(h->mu);
     auto it = h->staged.find({std::string((const char*) tenant, (size_t) tn), std::string((const char*) topic, (size_t) n)});
     if (it != h->staged.end()) {
@@ -1116,7 +1064,7 @@ int32_t bfq_rindex_remove(bfq_rindex* h, const uint8_t* tenant, int64_t tn, cons
 }
 
 int32_t bfq_rindex_commit(bfq_rindex* h) {
-    if (!h) return rfail(BFQ_E_INVALID, "handle is NULL");
+    if (!h) return fail(BFQ_E_INVALID, "handle is NULL");
     std::lock_guard<std::mutex> g(h->mu);
     int32_t rc = commit_delta(h);
     if (rc == NEED_FULL) rc = rebuild_full(h);
@@ -1125,7 +1073,7 @@ int32_t bfq_rindex_commit(bfq_rindex* h) {
 }
 
 int32_t bfq_rindex_stats(bfq_rindex* h, int64_t* stats, int32_t n) {
-    if (!h || (!stats && n > 0)) return rfail(BFQ_E_INVALID, "bad argument");
+    if (!h || (!stats && n > 0)) return fail(BFQ_E_INVALID, "bad argument");
     std::lock_guard<std::mutex> g(h->mu);
     const int64_t v[11] = {h->n_topics, (int64_t) h->regions.size(), h->n_nodes, h->garbage_nodes, h->used_slots,
                            (int64_t) h->n_blocks * BLOCK_USABLE, h->full_commits, h->delta_commits, h->last_rebuilt,
@@ -1136,9 +1084,9 @@ int32_t bfq_rindex_stats(bfq_rindex* h, int64_t* stats, int32_t n) {
 
 int32_t bfq_rindex_lookup(bfq_rindex* h, int64_t id, uint8_t* tenant_out, int64_t tenant_cap, int64_t* tenant_len,
                           uint8_t* topic_out, int64_t topic_cap, int64_t* topic_len) {
-    if (!h) return rfail(BFQ_E_INVALID, "handle is NULL");
+    if (!h) return fail(BFQ_E_INVALID, "handle is NULL");
     std::lock_guard<std::mutex> g(h->mu);
-    if (id < 0 || id >= (int64_t) h->by_id->size()) return rfail(BFQ_E_RANGE, "id out of range");
+    if (id < 0 || id >= (int64_t) h->by_id->size()) return fail(BFQ_E_RANGE, "id out of range");
     const auto& e = (*h->by_id)[(size_t) id];
     if (tenant_len) *tenant_len = (int64_t) e.first.size();
     if (topic_len) *topic_len = (int64_t) e.second.size();
@@ -1150,12 +1098,12 @@ int32_t bfq_rindex_lookup(bfq_rindex* h, int64_t id, uint8_t* tenant_out, int64_
 int32_t bfq_rmatch(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_off, int32_t n_tenants,
                    const uint8_t* filters, const int64_t* filter_off, const int32_t* filter_tenant, int64_t n,
                    const int64_t* limit, bfq_rresult** out) {
-    if (!h || !out || n < 0 || n_tenants < 0) return rfail(BFQ_E_INVALID, "bad argument");
+    if (!h || !out || n < 0 || n_tenants < 0) return fail(BFQ_E_INVALID, "bad argument");
     std::lock_guard<std::mutex> g(h->mu);
-    if (!h->have_snapshot) return rfail(BFQ_E_STATE, "bfq_rmatch before the first bfq_rindex_commit");
+    if (!h->have_snapshot) return fail(BFQ_E_STATE, "bfq_rmatch before the first bfq_rindex_commit");
     for (int64_t i = 0; i < n; i++)
-        if (filter_tenant[i] < 0 || filter_tenant[i] >= n_tenants) return rfail(BFQ_E_RANGE, "filter_tenant out of range");
-    RCUDA_TRY(cudaSetDevice(h->device));
+        if (filter_tenant[i] < 0 || filter_tenant[i] >= n_tenants) return fail(BFQ_E_RANGE, "filter_tenant out of range");
+    BFQ_CUDA_TRY(cudaSetDevice(h->device));
     cudaStream_t st = h->stream;
     auto t0 = std::chrono::steady_clock::now();
     const size_t nn = (size_t) std::max<int64_t>(n, 1), nt = (size_t) std::max(n_tenants, 1);
@@ -1165,19 +1113,19 @@ int32_t bfq_rmatch(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_
         if (it != h->tenant_root.end()) troot[(size_t) t] = it->second;
     }
     const int64_t fbytes = n ? filter_off[n] : 0;
-    RCUDA_TRY(h->d_filters.reserve((size_t) std::max<int64_t>(fbytes, 1)));
-    RCUDA_TRY(h->d_filter_off.reserve(nn + 1));
-    RCUDA_TRY(h->d_filter_tenant.reserve(nn));
-    RCUDA_TRY(h->d_tenant_root.reserve(nt));
-    RCUDA_TRY(h->d_limit.reserve(nn));
-    RCUDA_TRY(h->d_span_begin.reserve(nn));
-    RCUDA_TRY(h->d_span_count.reserve(nn));
-    RCUDA_TRY(h->d_overflow.reserve(nn));
-    RCUDA_TRY(h->d_total.reserve(nn));
-    RCUDA_TRY(h->d_kept.reserve(nn));
-    RCUDA_TRY(h->d_offsets.reserve(nn + 1));
-    RCUDA_TRY(h->d_counters.reserve(RC_COUNT));
-    if (h->d_ranges.cap == 0) RCUDA_TRY(h->d_ranges.reserve(std::max<size_t>(1 << 18, 8 * nn)));
+    BFQ_CUDA_TRY(h->d_filters.reserve((size_t) std::max<int64_t>(fbytes, 1)));
+    BFQ_CUDA_TRY(h->d_filter_off.reserve(nn + 1));
+    BFQ_CUDA_TRY(h->d_filter_tenant.reserve(nn));
+    BFQ_CUDA_TRY(h->d_tenant_root.reserve(nt));
+    BFQ_CUDA_TRY(h->d_limit.reserve(nn));
+    BFQ_CUDA_TRY(h->d_span_begin.reserve(nn));
+    BFQ_CUDA_TRY(h->d_span_count.reserve(nn));
+    BFQ_CUDA_TRY(h->d_overflow.reserve(nn));
+    BFQ_CUDA_TRY(h->d_total.reserve(nn));
+    BFQ_CUDA_TRY(h->d_kept.reserve(nn));
+    BFQ_CUDA_TRY(h->d_offsets.reserve(nn + 1));
+    BFQ_CUDA_TRY(h->d_counters.reserve(RC_COUNT));
+    if (h->d_ranges.cap == 0) BFQ_CUDA_TRY(h->d_ranges.reserve(std::max<size_t>(1 << 18, 8 * nn)));
     auto* res = new bfq_rresult();
     res->by_id = h->committed;
     res->offsets.assign((size_t) n + 1, 0);
@@ -1186,15 +1134,15 @@ int32_t bfq_rmatch(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_
         *out = res;
         return BFQ_OK;
     }
-    RCUDA_TRY(cudaMemcpyAsync(h->d_filters.p, filters, (size_t) fbytes, cudaMemcpyHostToDevice, st));
-    RCUDA_TRY(cudaMemcpyAsync(h->d_filter_off.p, filter_off, (size_t) (n + 1) * 8, cudaMemcpyHostToDevice, st));
-    RCUDA_TRY(cudaMemcpyAsync(h->d_filter_tenant.p, filter_tenant, (size_t) n * 4, cudaMemcpyHostToDevice, st));
-    RCUDA_TRY(cudaMemcpyAsync(h->d_tenant_root.p, troot.data(), nt * 4, cudaMemcpyHostToDevice, st));
-    if (limit) RCUDA_TRY(cudaMemcpyAsync(h->d_limit.p, limit, (size_t) n * 8, cudaMemcpyHostToDevice, st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(h->d_filters.p, filters, (size_t) fbytes, cudaMemcpyHostToDevice, st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(h->d_filter_off.p, filter_off, (size_t) (n + 1) * 8, cudaMemcpyHostToDevice, st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(h->d_filter_tenant.p, filter_tenant, (size_t) n * 4, cudaMemcpyHostToDevice, st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(h->d_tenant_root.p, troot.data(), nt * 4, cudaMemcpyHostToDevice, st));
+    if (limit) BFQ_CUDA_TRY(cudaMemcpyAsync(h->d_limit.p, limit, (size_t) n * 8, cudaMemcpyHostToDevice, st));
     auto t1 = std::chrono::steady_clock::now();
     for (auto& e : h->ev)
-        if (!e) RCUDA_TRY(cudaEventCreate(&e));
-    RCUDA_TRY(cudaEventRecord(h->ev[0], st));   // the inputs are (enqueued to be) resident: device time of the kernels from here
+        if (!e) BFQ_CUDA_TRY(cudaEventCreate(&e));
+    BFQ_CUDA_TRY(cudaEventRecord(h->ev[0], st));   // the inputs are (enqueued to be) resident: device time of the kernels from here
 
     RMatchParams p{};
     p.nodes = h->d_nodes.p;
@@ -1220,13 +1168,11 @@ int32_t bfq_rmatch(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_
     // running at the same time hit the same node records in L2 (the forward path's locality order, reused)
     const uint32_t* order = nullptr;
     if (n >= 4096) {
-        const size_t buckets = order_hist_buckets(n, n_tenants);
-        const size_t hist_words = (buckets + 2 * (buckets / 4096) + 64 + 63) / 64 * 64;
-        RCUDA_TRY(h->d_ord_keys.reserve(nn));
-        RCUDA_TRY(h->d_ord_leader.reserve(nn));
-        RCUDA_TRY(h->d_order.reserve(nn));
-        RCUDA_TRY(h->d_hist.reserve(hist_words));
-        RCUDA_TRY(h->d_ord_ctr.reserve(CTR_COUNT));
+        BFQ_CUDA_TRY(h->d_ord_keys.reserve(nn));
+        BFQ_CUDA_TRY(h->d_ord_leader.reserve(nn));
+        BFQ_CUDA_TRY(h->d_order.reserve(nn));
+        BFQ_CUDA_TRY(h->d_hist.reserve(order_scratch_words(n, n_tenants)));
+        BFQ_CUDA_TRY(h->d_ord_ctr.reserve(CTR_COUNT));
         OrderParams q{};
         q.n_topics = n;
         q.topics = h->d_filters.p;
@@ -1239,15 +1185,9 @@ int32_t bfq_rmatch(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_
         q.hash_tab = nullptr;
         q.hash_mask = 0;
         q.hist = h->d_hist.p;
-        q.blk_tot = q.hist + buckets;
-        q.blk_pfx = q.blk_tot + buckets / 4096;
-        q.ticket = q.blk_pfx + buckets / 4096;
-        q.hist_bits = 0;
-        while (((size_t) 1 << q.hist_bits) < buckets) q.hist_bits++;
         q.dedup = 0;
         q.counters = h->d_ord_ctr.p;
-        RCUDA_TRY(cudaMemsetAsync(q.hist, 0, hist_words * sizeof(uint32_t), st));
-        RCUDA_TRY(launch_order(q, st));
+        BFQ_CUDA_TRY(launch_order(q, st));
         h->launches += 3;
         order = q.order;
     }
@@ -1256,22 +1196,22 @@ int32_t bfq_rmatch(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_
         p.ranges_cap = h->d_ranges.cap;
         p.work_list = order;
         p.n_work = 0;
-        RCUDA_TRY(cudaMemsetAsync(h->d_counters.p, 0, sizeof(hc), st));
+        BFQ_CUDA_TRY(cudaMemsetAsync(h->d_counters.p, 0, sizeof(hc), st));
         int64_t ctas = std::min<int64_t>((n + R_WARPS - 1) / R_WARPS, (int64_t) sms * ctas_per_sm);
-        RCUDA_TRY(cudaEventRecord(h->ev[2], st));
+        BFQ_CUDA_TRY(cudaEventRecord(h->ev[2], st));
         rmatch_kernel<false><<<(unsigned) std::max<int64_t>(ctas, 1), R_WARPS * 32, 0, st>>>(p);
-        RCUDA_TRY(cudaEventRecord(h->ev[3], st));
+        BFQ_CUDA_TRY(cudaEventRecord(h->ev[3], st));
         h->launches++;
-        RCUDA_TRY(cudaGetLastError());
-        RCUDA_TRY(cudaMemcpyAsync(hc, h->d_counters.p, sizeof(hc), cudaMemcpyDeviceToHost, st));
-        RCUDA_TRY(cudaStreamSynchronize(st));
+        BFQ_CUDA_TRY(cudaGetLastError());
+        BFQ_CUDA_TRY(cudaMemcpyAsync(hc, h->d_counters.p, sizeof(hc), cudaMemcpyDeviceToHost, st));
+        BFQ_CUDA_TRY(cudaStreamSynchronize(st));
         if (hc[RC_OVERFLOW] > 0) {
             const uint64_t capF = (uint64_t) h->max_nodes_per_depth + 2;
             const uint64_t capR = 3 * ((uint64_t) h->n_nodes + 2) + 2;
             const uint64_t per_warp = 2 * capF + capR;
             uint64_t warps = std::min<uint64_t>(hc[RC_OVERFLOW], std::max<uint64_t>(8, (1ull << 31) / (per_warp * sizeof(uint2))));
             warps = std::min<uint64_t>((warps + 7) / 8 * 8, (uint64_t) sms * 8);
-            RCUDA_TRY(h->d_scratch.reserve((size_t) (warps * per_warp)));
+            BFQ_CUDA_TRY(h->d_scratch.reserve((size_t) (warps * per_warp)));
             p.scratch = h->d_scratch.p;
             p.scratch_frontier_cap = capF;
             p.scratch_ranges_cap = capR;
@@ -1279,50 +1219,50 @@ int32_t bfq_rmatch(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_
             p.n_work = (int64_t) hc[RC_OVERFLOW];
             rmatch_kernel<true><<<(unsigned) (warps / 8), R_WARPS * 32, 0, st>>>(p);
             h->launches++;
-            RCUDA_TRY(cudaGetLastError());
-            RCUDA_TRY(cudaMemcpyAsync(hc, h->d_counters.p, sizeof(hc), cudaMemcpyDeviceToHost, st));
-            RCUDA_TRY(cudaStreamSynchronize(st));
+            BFQ_CUDA_TRY(cudaGetLastError());
+            BFQ_CUDA_TRY(cudaMemcpyAsync(hc, h->d_counters.p, sizeof(hc), cudaMemcpyDeviceToHost, st));
+            BFQ_CUDA_TRY(cudaStreamSynchronize(st));
             if (hc[RC_ERROR] != 0) {
                 delete res;
-                return rfail(BFQ_E_STATE, "tier-2 scratch exhausted");
+                return fail(BFQ_E_STATE, "tier-2 scratch exhausted");
             }
         }
         if (hc[RC_RANGES] <= h->d_ranges.cap) break;
         const size_t want = (size_t) (hc[RC_RANGES] + hc[RC_RANGES] / 4 + 1024);
         if (want >= 0xFFFFFFF0ull || attempt == 7) {
             delete res;
-            return rfail(BFQ_E_RANGE, "too many matched ranges in one batch; split the batch");
+            return fail(BFQ_E_RANGE, "too many matched ranges in one batch; split the batch");
         }
-        RCUDA_TRY(h->d_ranges.reserve(want));
+        BFQ_CUDA_TRY(h->d_ranges.reserve(want));
     }
     // kept = min(total, limit); exclusive scan; expand to ids
     rkept_kernel<<<(unsigned) ((n + 255) / 256), 256, 0, st>>>(n, h->d_total.p, limit ? h->d_limit.p : nullptr, h->d_kept.p);
     size_t tmp_bytes = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, h->d_kept.p, h->d_offsets.p, (int) n, st);
-    RCUDA_TRY(h->d_scan_tmp.reserve(tmp_bytes));
+    BFQ_CUDA_TRY(h->d_scan_tmp.reserve(tmp_bytes));
     cub::DeviceScan::ExclusiveSum(h->d_scan_tmp.p, tmp_bytes, h->d_kept.p, h->d_offsets.p, (int) n, st);
     h->launches += 2;
     // only the grand total is needed on the host before the expansion (to size the id buffer): two scalars, not the arrays
-    if (!h->h_small) RCUDA_TRY(cudaMallocHost(&h->h_small, 4 * sizeof(unsigned long long)));
-    RCUDA_TRY(cudaMemcpyAsync(h->h_small, h->d_offsets.p + (n - 1), 8, cudaMemcpyDeviceToHost, st));
-    RCUDA_TRY(cudaMemcpyAsync(h->h_small + 1, h->d_kept.p + (n - 1), 8, cudaMemcpyDeviceToHost, st));
-    RCUDA_TRY(cudaStreamSynchronize(st));
-    const unsigned long long total_ids = h->h_small[0] + h->h_small[1];
-    RCUDA_TRY(h->d_ids.reserve((size_t) std::max<unsigned long long>(total_ids, 1)));
+    BFQ_CUDA_TRY(h->h_small.reserve(4));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(h->h_small.p, h->d_offsets.p + (n - 1), 8, cudaMemcpyDeviceToHost, st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(h->h_small.p + 1, h->d_kept.p + (n - 1), 8, cudaMemcpyDeviceToHost, st));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
+    const unsigned long long total_ids = h->h_small.p[0] + h->h_small.p[1];
+    BFQ_CUDA_TRY(h->d_ids.reserve((size_t) std::max<unsigned long long>(total_ids, 1)));
     rexpand_kernel<<<(unsigned) ((n * 32 + 255) / 256), 256, 0, st>>>(n, h->d_span_begin.p, h->d_span_count.p, h->d_ranges.p,
                                                                       h->d_offsets.p, h->d_kept.p, h->d_dfs_to_id.p,
                                                                       h->d_bfs_to_id.p, h->d_ids.p);
     h->launches++;
-    RCUDA_TRY(cudaGetLastError());
-    RCUDA_TRY(cudaEventRecord(h->ev[1], st));
+    BFQ_CUDA_TRY(cudaGetLastError());
+    BFQ_CUDA_TRY(cudaEventRecord(h->ev[1], st));
     auto t2 = std::chrono::steady_clock::now();
     // the result owns its arrays: offsets / totals / ids are read back straight into them (same 8-byte element types)
     static_assert(sizeof(unsigned long long) == sizeof(int64_t), "offsets are copied without conversion");
     res->ids.resize((size_t) total_ids);
-    RCUDA_TRY(cudaMemcpyAsync(res->offsets.data(), h->d_offsets.p, (size_t) n * 8, cudaMemcpyDeviceToHost, st));
-    RCUDA_TRY(cudaMemcpyAsync(res->totals.data(), h->d_total.p, (size_t) n * 8, cudaMemcpyDeviceToHost, st));
-    if (total_ids) RCUDA_TRY(cudaMemcpyAsync(res->ids.data(), h->d_ids.p, (size_t) total_ids * 8, cudaMemcpyDeviceToHost, st));
-    RCUDA_TRY(cudaStreamSynchronize(st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(res->offsets.data(), h->d_offsets.p, (size_t) n * 8, cudaMemcpyDeviceToHost, st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(res->totals.data(), h->d_total.p, (size_t) n * 8, cudaMemcpyDeviceToHost, st));
+    if (total_ids) BFQ_CUDA_TRY(cudaMemcpyAsync(res->ids.data(), h->d_ids.p, (size_t) total_ids * 8, cudaMemcpyDeviceToHost, st));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
     res->offsets[(size_t) n] = (int64_t) total_ids;
     auto t3 = std::chrono::steady_clock::now();
     auto ms = [](auto a, auto b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
@@ -1351,7 +1291,7 @@ const int64_t* bfq_rresult_ids(const bfq_rresult* r, int64_t* n) {
 }
 const int64_t* bfq_rresult_total_matches(const bfq_rresult* r) { return r->totals.data(); }
 int32_t bfq_rresult_timings(const bfq_rresult* r, double* ms, int32_t n) {
-    if (!r || !ms) return rfail(BFQ_E_INVALID, "bad argument");
+    if (!r || !ms) return fail(BFQ_E_INVALID, "bad argument");
     for (int32_t i = 0; i < n && i < 8; i++) ms[i] = r->ms[i];
     return BFQ_OK;
 }
