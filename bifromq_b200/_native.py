@@ -44,6 +44,13 @@ class BfqFanoutResult(C.Structure):
                 ("n_pairs", C.c_int64), ("n_deliverers", C.c_int32), ("ordered_share_id", C.c_int32), ("generation", C.c_uint64)]
 
 
+class BfqDeliveryResult(C.Structure):
+    _fields_ = [("d_package_off", C.c_void_p), ("d_package_tenant", C.c_void_p), ("d_pack_off", C.c_void_p),
+                ("d_pack_topic", C.c_void_p), ("d_match_off", C.c_void_p), ("d_match_rank", C.c_void_p),
+                ("d_match_member", C.c_void_p), ("n_pairs", C.c_int64), ("n_packages", C.c_int64), ("n_packs", C.c_int64),
+                ("n_deliverers", C.c_int32), ("ordered_share_id", C.c_int32), ("generation", C.c_uint64)]
+
+
 class BfqBudgetResult(C.Structure):
     _fields_ = [("d_delivered_persistent", C.c_void_p), ("d_topic_flags", C.c_void_p), ("n_delivered", C.c_int64),
                 ("n_dropped_bytes", C.c_int64), ("n_dropped_persistent_bandwidth", C.c_int64),
@@ -91,6 +98,7 @@ _SIGNATURES = {
     "bfq_range_lookup": (_i32, [_i32, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bfq_fanout_device": (_i32, [C.POINTER(BfqDeviceResult), _vp, _vp, _i64, _vp, C.POINTER(BfqFanoutResult)]),
     "bfq_fanout_deliverer": (_i32, [_vp, _i32, C.POINTER(_i32), _vp, _i64, C.POINTER(_i64)]),
+    "bfq_delivery_device": (_i32, [C.POINTER(BfqDeviceResult), _vp, _vp, _i64, _vp, _vp, C.POINTER(BfqDeliveryResult)]),
     "bfq_exchange_unique_id": (_i32, [_vp, _i32]),
     "bfq_exchange_create": (_i32, [_i32, _i32, _i32, _vp, C.POINTER(_vp)]),
     "bfq_exchange_destroy": (None, [_vp]),

@@ -118,6 +118,11 @@ struct Workspace {
     DeviceBuf<uint32_t> d_fo_counts, d_fo_base, d_pack_topic, d_pack_rank, d_pack_member;
     DeviceBuf<long long> d_pack_offsets;
     DeviceBuf<uint8_t> d_fo_tmp;
+    // delivery nesting (fanout.cu: launch_delivery): scratch per topic (6 words each + 2) and per pair (10 words each + 2), the outputs
+    DeviceBuf<uint32_t> d_dl_topic_tmp, d_dl_pair_tmp, d_dl_pcount, d_package_tenant, d_dl_pack_topic, d_match_rank, d_match_member;
+    DeviceBuf<unsigned long long> d_dl_totals;
+    DeviceBuf<long long> d_package_off, d_dl_pack_off, d_match_off;
+    DeviceBuf<uint8_t> d_dl_tmp;
     // pinned result buffers
     PinnedBuf<uint32_t> h_span_begin, h_span_count, h_route_count;
     PinnedBuf<uint2> h_ranges;
@@ -2208,6 +2213,101 @@ int32_t bfq_fanout_device(const bfq_device_result* res, const int64_t* d_offsets
     std::lock_guard<std::mutex> g(h->mu);
     h->launches += 5;
     if (!tiled) h->global_fanouts++;
+    return BFQ_OK;
+}
+
+int32_t bfq_delivery_device(const bfq_device_result* res, const int64_t* d_offsets, const int64_t* d_ranks, int64_t n_pairs,
+                            const int32_t* d_topic_tenant, void* stream, bfq_delivery_result* out) {
+    if (!res || !res->lease || !out || !d_offsets || n_pairs < 0 || (n_pairs > 0 && !d_ranks)) return fail(BFQ_E_INVALID, "bad argument");
+    auto* L = static_cast<DeviceLease*>(res->lease);
+    if (!L->done || L->rc != BFQ_OK) return fail(BFQ_E_STATE, "bfq_delivery_device needs a completed match (bfq_device_result_wait)");
+    if (L->n > 0 && !d_topic_tenant) return fail(BFQ_E_INVALID, "NULL d_topic_tenant");
+    if (n_pairs >= (int64_t) 0xFFFFFFF0ll) return fail(BFQ_E_RANGE, "more than 2^32 (topic, route) pairs in one batch; split the batch");
+    bfq_index* h = L->h;
+    Workspace* w = L->ws;
+    BFQ_CUDA_TRY(cudaSetDevice(h->device));
+    std::shared_ptr<Snapshot::FanTable> ft;
+    int32_t rc = ensure_fan_table(h, L->snap.get(), &ft);
+    if (rc != BFQ_OK) return rc;
+    cudaStream_t st = (cudaStream_t) stream;
+    const int64_t T = L->n;
+    const size_t np = (size_t) std::max<int64_t>(n_pairs, 1);
+    BFQ_CUDA_TRY(w->d_dl_topic_tmp.reserve(6 * (size_t) T + 2));
+    BFQ_CUDA_TRY(w->d_dl_pair_tmp.reserve(10 * np + 2));
+    BFQ_CUDA_TRY(w->d_dl_pcount.reserve((size_t) ft->n_deliverers + 1));
+    BFQ_CUDA_TRY(w->d_dl_totals.reserve(4));
+    BFQ_CUDA_TRY(w->d_package_off.reserve((size_t) ft->n_deliverers + 1));
+    BFQ_CUDA_TRY(w->d_package_tenant.reserve(np));
+    BFQ_CUDA_TRY(w->d_dl_pack_off.reserve(np + 1));
+    BFQ_CUDA_TRY(w->d_dl_pack_topic.reserve(np));
+    BFQ_CUDA_TRY(w->d_match_off.reserve(np + 1));
+    BFQ_CUDA_TRY(w->d_match_rank.reserve(np));
+    BFQ_CUDA_TRY(w->d_match_member.reserve(np));
+    DeliveryParams q{};
+    q.f.n_topics = T;
+    q.f.offsets = d_offsets;
+    q.f.n_pairs = n_pairs;
+    q.f.ranks = d_ranks;
+    q.f.rdeliv = ft->d_rdeliv.p;
+    q.f.gmem_off = ft->d_gmem_off.p;
+    q.f.gmem_deliv = ft->d_gmem_deliv.p;
+    q.f.gordered = ft->d_gordered.p;
+    q.f.n_deliverers = ft->n_deliverers;
+    q.topic_tenant = d_topic_tenant;
+    q.n_tenants = L->ctx.n_tenants;
+    uint32_t* tt = w->d_dl_topic_tmp.p;
+    q.tkey[0] = tt;
+    q.tkey[1] = tt + T;
+    q.tval[0] = tt + 2 * T;
+    q.tval[1] = tt + 3 * T;
+    q.tcount = tt + 4 * T;
+    q.tstart = tt + 5 * T + 1;
+    uint32_t* pt = w->d_dl_pair_tmp.p;
+    q.key[0] = pt;
+    q.key[1] = pt + np;
+    q.val[0] = pt + 2 * np;
+    q.val[1] = pt + 3 * np;
+    q.e_topic = pt + 4 * np;
+    q.e_rank = pt + 5 * np;
+    q.e_member = pt + 6 * np;
+    q.s_topic = pt + 7 * np;
+    q.package_head = pt + 8 * np;
+    q.pack_head = pt + 9 * np + 1;
+    q.pcount = w->d_dl_pcount.p;
+    q.totals = w->d_dl_totals.p;
+    q.package_off = w->d_package_off.p;
+    q.package_tenant = w->d_package_tenant.p;
+    q.pack_off = w->d_dl_pack_off.p;
+    q.pack_topic = w->d_dl_pack_topic.p;
+    q.match_off = w->d_match_off.p;
+    q.match_rank = w->d_match_rank.p;
+    q.match_member = w->d_match_member.p;
+    size_t tmp_bytes = 0;
+    BFQ_CUDA_TRY(launch_delivery(q, nullptr, &tmp_bytes, st));
+    BFQ_CUDA_TRY(w->d_dl_tmp.reserve(tmp_bytes + 256));
+    BFQ_CUDA_TRY(launch_delivery(q, w->d_dl_tmp.p, &tmp_bytes, st));
+    unsigned long long tot[4];
+    BFQ_CUDA_TRY(cudaMemcpyAsync(tot, w->d_dl_totals.p, sizeof(tot), cudaMemcpyDeviceToHost, st));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
+    {
+        std::lock_guard<std::mutex> g(h->mu);
+        h->launches += 11;
+    }
+    if ((int64_t) tot[3] != n_pairs)
+        return fail(BFQ_E_INVALID, "n_pairs = " + std::to_string(n_pairs) + " but d_offsets[n_topics] = " + std::to_string((int64_t) tot[3]));
+    out->d_package_off = (const int64_t*) w->d_package_off.p;
+    out->d_package_tenant = w->d_package_tenant.p;
+    out->d_pack_off = (const int64_t*) w->d_dl_pack_off.p;
+    out->d_pack_topic = w->d_dl_pack_topic.p;
+    out->d_match_off = (const int64_t*) w->d_match_off.p;
+    out->d_match_rank = w->d_match_rank.p;
+    out->d_match_member = w->d_match_member.p;
+    out->n_pairs = (int64_t) tot[0];
+    out->n_packages = (int64_t) tot[1];
+    out->n_packs = (int64_t) tot[2];
+    out->n_deliverers = (int32_t) ft->n_deliverers;
+    out->ordered_share_id = (int32_t) ft->n_deliverers - 1;
+    out->generation = L->snap->generation;
     return BFQ_OK;
 }
 

@@ -36,6 +36,7 @@
 #include <unordered_map>
 #include <vector>
 
+#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include "../../include/bfq_gpumatch.h"
@@ -195,6 +196,175 @@ cudaError_t launch_fanout(const FanoutParams& p, bool tiled, void* d_tmp, size_t
     if (e != cudaSuccess) return e;
     fanout_scatter_kernel<false><<<n_tiles, FO_THREADS, smem, stream>>>(p);
     fanout_offsets_kernel<<<(p.n_deliverers + 1 + 255) / 256, 256, 0, stream>>>(p, n_tiles);
+    return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------------ delivery nesting
+// BatchDeliveryCall (bifromq-deliverer/.../BatchDeliveryCall.java:58,75-104) nests a deliverer's calls as
+// tenantId -> TopicMessagePack -> Set<MatchInfo> and sends one DeliveryRequest. The pairs are emitted in (tenant, topic position)
+// order, so a STABLE partition on the deliverer id alone leaves every deliverer's pairs in (tenant, topic position) order:
+//   1. tenant-major topic order   stable radix sort of the topic positions by tenant index (work ~ topics, not pairs)
+//   2. emit                       per pair in that order: key = deliverer id (fo_deliverer, as the fan-out), value = emit position
+//   3. partition                  cub::DeviceRadixSort::SortPairs on the bits of the deliverer id (stable)
+//   4. segments                   head flags where (deliverer, tenant) or (deliverer, topic) changes, their exclusive scans
+//                                 (package / pack numbers), one scatter of the offsets
+// Emit positions past the pairs nested (the CSR may hold pairs of a topic without a valid tenant, or disagree with n_pairs)
+// carry the key n_deliverers, so they sort last and are never read back.
+namespace {
+
+constexpr int DL_THREADS = 256;
+
+uint32_t bits_for(uint32_t v) { return v ? 32u - (uint32_t) __builtin_clz(v) : 1u; }
+
+__global__ void __launch_bounds__(DL_THREADS) delivery_topic_keys_kernel(const DeliveryParams q) {
+    const int64_t t = (int64_t) blockIdx.x * DL_THREADS + threadIdx.x;
+    if (t >= q.f.n_topics) return;
+    const int32_t tn = q.topic_tenant[t];
+    q.tkey[0][t] = (tn >= 0 && tn < q.n_tenants) ? (uint32_t) tn : (uint32_t) q.n_tenants;
+    q.tval[0][t] = (uint32_t) t;
+}
+
+// pairs of the i-th topic in tenant-major order; none for a topic without a valid tenant, none at all if the CSR's total is not n_pairs
+__global__ void __launch_bounds__(DL_THREADS) delivery_topic_counts_kernel(const DeliveryParams q, const uint32_t* tkey, const uint32_t* order) {
+    const int64_t i = (int64_t) blockIdx.x * DL_THREADS + threadIdx.x;
+    if (i > q.f.n_topics) return;
+    uint32_t c = 0;
+    if (i < q.f.n_topics && tkey[i] < (uint32_t) q.n_tenants && q.f.offsets[q.f.n_topics] == q.f.n_pairs) {
+        const uint32_t t = order[i];
+        c = (uint32_t) (q.f.offsets[t + 1] - q.f.offsets[t]);
+    }
+    q.tcount[i] = c;
+}
+
+// last i with start[i] <= j (start monotone, start[0] = 0 <= j < start[n])
+__device__ __forceinline__ uint32_t dl_segment_of(const uint32_t* start, int64_t n, uint32_t j) {
+    int64_t lo = 0, hi = n;
+    while (hi - lo > 1) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (start[mid] <= j) lo = mid;
+        else hi = mid;
+    }
+    return (uint32_t) lo;
+}
+
+// a thread owns FO_TILE / FO_THREADS consecutive emit positions, as the fan-out's passes do
+__global__ void __launch_bounds__(FO_THREADS) delivery_emit_kernel(const DeliveryParams q, const uint32_t* order) {
+    constexpr int PER = FO_TILE / FO_THREADS;
+    const int64_t j0 = (int64_t) blockIdx.x * FO_TILE + (int64_t) threadIdx.x * PER;
+    if (j0 >= q.f.n_pairs) return;
+    const int64_t n_emit = q.tstart[q.f.n_topics];
+    uint32_t i = j0 < n_emit ? dl_segment_of(q.tstart, q.f.n_topics, (uint32_t) j0) : 0;
+    for (int k = 0; k < PER && j0 + k < q.f.n_pairs; k++) {
+        const uint32_t j = (uint32_t) (j0 + k);
+        q.val[0][j] = j;
+        if (j >= n_emit) {
+            q.key[0][j] = q.f.n_deliverers;
+            continue;
+        }
+        while (q.tstart[i + 1] <= j) i++;
+        const uint32_t t = order[i];
+        const int64_t r = q.f.ranks[q.f.offsets[t] + (j - q.tstart[i])];
+        uint32_t member;
+        q.key[0][j] = fo_deliverer(q.f, t, r, &member);
+        q.e_topic[j] = i;
+        q.e_rank[j] = (uint32_t) r;
+        q.e_member[j] = member;
+    }
+}
+
+// nested pair k (deliverer-major): its pair, its tenant-major topic index and its head flags
+__global__ void __launch_bounds__(DL_THREADS) delivery_gather_kernel(const DeliveryParams q, const uint32_t* skey, const uint32_t* sval,
+                                                                     const uint32_t* tkey) {
+    const int64_t k = (int64_t) blockIdx.x * DL_THREADS + threadIdx.x;
+    if (k > q.f.n_pairs) return;
+    if (k >= (int64_t) q.tstart[q.f.n_topics]) {
+        q.package_head[k] = 0;
+        q.pack_head[k] = 0;
+        return;
+    }
+    const uint32_t j = sval[k], i = q.e_topic[j], d = skey[k];
+    q.s_topic[k] = i;
+    q.match_rank[k] = q.e_rank[j];
+    q.match_member[k] = q.e_member[j];
+    bool package = true, pack = true;
+    if (k > 0) {
+        const uint32_t i0 = q.e_topic[sval[k - 1]], d0 = skey[k - 1];
+        package = d != d0 || tkey[i] != tkey[i0];
+        pack = d != d0 || i != i0;
+    }
+    q.package_head[k] = package;
+    q.pack_head[k] = pack;
+}
+
+// package_head[] / pack_head[] scanned (exclusive, n_pairs + 1 entries): a head's package / pack number, and the totals at
+// [n_emit]. Thread 0 writes the terminators and the totals.
+__global__ void __launch_bounds__(DL_THREADS) delivery_scatter_kernel(const DeliveryParams q, const uint32_t* skey, const uint32_t* tkey,
+                                                                      const uint32_t* order) {
+    const int64_t k = (int64_t) blockIdx.x * DL_THREADS + threadIdx.x;
+    const int64_t n_emit = q.tstart[q.f.n_topics];
+    if (k == 0) {
+        const uint32_t n_packages = q.package_head[n_emit], n_packs = q.pack_head[n_emit];
+        q.pack_off[n_packages] = n_packs;
+        q.match_off[n_packs] = n_emit;
+        q.totals[0] = (unsigned long long) n_emit;
+        q.totals[1] = n_packages;
+        q.totals[2] = n_packs;
+        q.totals[3] = (unsigned long long) q.f.offsets[q.f.n_topics];
+    }
+    if (k >= n_emit) return;
+    const uint32_t pk = q.pack_head[k], pg = q.package_head[k];
+    const uint32_t i = q.s_topic[k];
+    if (q.pack_head[k + 1] != pk) {
+        q.pack_topic[pk] = order[i];
+        q.match_off[pk] = k;
+    }
+    if (q.package_head[k + 1] != pg) {
+        q.package_tenant[pg] = tkey[i];
+        q.pack_off[pg] = pk;
+        atomicAdd(&q.pcount[skey[k]], 1u);
+    }
+}
+
+unsigned dl_blocks(int64_t n) { return (unsigned) std::max<int64_t>(1, (n + DL_THREADS - 1) / DL_THREADS); }
+
+}  // namespace
+
+cudaError_t launch_delivery(const DeliveryParams& q, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream) {
+    // item counts as uint32 (pairs and topics are below 2^32): CUB then keeps 32-bit offsets
+    const uint32_t T = (uint32_t) q.f.n_topics, n = (uint32_t) q.f.n_pairs;
+    const uint32_t D = q.f.n_deliverers;
+    const int tbits = (int) bits_for((uint32_t) q.n_tenants), dbits = (int) bits_for(D);
+    cub::DoubleBuffer<uint32_t> tk(q.tkey[0], q.tkey[1]), tv(q.tval[0], q.tval[1]);
+    cub::DoubleBuffer<uint32_t> dk(q.key[0], q.key[1]), dv(q.val[0], q.val[1]);
+    if (!d_tmp) {
+        size_t a = 0, b = 0, c = 0, d = 0, e = 0;
+        cudaError_t err = cub::DeviceRadixSort::SortPairs(nullptr, a, tk, tv, T, 0, tbits, stream);
+        if (err == cudaSuccess) err = cub::DeviceScan::ExclusiveSum(nullptr, b, q.tcount, q.tstart, T + 1, stream);
+        if (err == cudaSuccess) err = cub::DeviceRadixSort::SortPairs(nullptr, c, dk, dv, n, 0, dbits, stream);
+        if (err == cudaSuccess) err = cub::DeviceScan::ExclusiveSum(nullptr, d, q.pack_head, n + 1, stream);
+        if (err == cudaSuccess) err = cub::DeviceScan::ExclusiveSum(nullptr, e, q.pcount, q.package_off, D + 1, stream);
+        *tmp_bytes = std::max({a, b, c, d, e});
+        return err;
+    }
+    size_t bytes = *tmp_bytes;
+    cudaError_t err = cudaMemsetAsync(q.pcount, 0, ((size_t) D + 1) * sizeof(uint32_t), stream);
+    if (err != cudaSuccess) return err;
+    delivery_topic_keys_kernel<<<dl_blocks(T), DL_THREADS, 0, stream>>>(q);
+    if ((err = cub::DeviceRadixSort::SortPairs(d_tmp, bytes, tk, tv, T, 0, tbits, stream)) != cudaSuccess) return err;
+    delivery_topic_counts_kernel<<<dl_blocks(T + 1), DL_THREADS, 0, stream>>>(q, tk.Current(), tv.Current());
+    bytes = *tmp_bytes;
+    if ((err = cub::DeviceScan::ExclusiveSum(d_tmp, bytes, q.tcount, q.tstart, T + 1, stream)) != cudaSuccess) return err;
+    delivery_emit_kernel<<<fo_tiles(n), FO_THREADS, 0, stream>>>(q, tv.Current());
+    bytes = *tmp_bytes;
+    if ((err = cub::DeviceRadixSort::SortPairs(d_tmp, bytes, dk, dv, n, 0, dbits, stream)) != cudaSuccess) return err;
+    delivery_gather_kernel<<<dl_blocks(n + 1), DL_THREADS, 0, stream>>>(q, dk.Current(), dv.Current(), tk.Current());
+    bytes = *tmp_bytes;
+    if ((err = cub::DeviceScan::ExclusiveSum(d_tmp, bytes, q.package_head, n + 1, stream)) != cudaSuccess) return err;
+    bytes = *tmp_bytes;
+    if ((err = cub::DeviceScan::ExclusiveSum(d_tmp, bytes, q.pack_head, n + 1, stream)) != cudaSuccess) return err;
+    delivery_scatter_kernel<<<dl_blocks(n), DL_THREADS, 0, stream>>>(q, dk.Current(), tk.Current(), tv.Current());
+    bytes = *tmp_bytes;
+    if ((err = cub::DeviceScan::ExclusiveSum(d_tmp, bytes, q.pcount, q.package_off, D + 1, stream)) != cudaSuccess) return err;
     return cudaGetLastError();
 }
 

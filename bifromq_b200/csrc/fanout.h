@@ -44,6 +44,39 @@ size_t fanout_scratch_words(uint32_t n_deliverers, int64_t n_pairs, bool tiled);
 // d_tmp == nullptr: query the scan scratch size
 cudaError_t launch_fanout(const FanoutParams& p, bool tiled, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream);
 
+// The same pairs nested the way the deliverer's batcher sends them: deliverer -> package (tenant) -> pack (topic position)
+// -> MatchInfos. Deliverer ids and member picks are the fan-out's (the same device function resolves both).
+struct DeliveryParams {
+    FanoutParams f;                  // the CSR and the per-snapshot tables; f's scratch and outputs are not used
+    const int32_t* topic_tenant;     // [n_topics] the match's tenant index per topic position
+    int32_t n_tenants;
+    // scratch
+    uint32_t* tkey[2];               // [n_topics] each: the tenant sort's keys (double buffer)
+    uint32_t* tval[2];               // [n_topics] each: ... and topic positions
+    uint32_t* tcount;                // [n_topics + 1] pairs per topic in tenant-major order
+    uint32_t* tstart;                // [n_topics + 1] their exclusive scan: [n_topics] = pairs nested
+    uint32_t* key[2];                // [n_pairs] each: the deliverer partition's keys (double buffer)
+    uint32_t* val[2];                // [n_pairs] each: ... and emit positions
+    uint32_t* e_topic;               // [n_pairs] per emit position: tenant-major topic index, rank, member
+    uint32_t* e_rank;
+    uint32_t* e_member;
+    uint32_t* s_topic;               // [n_pairs] per nested pair: tenant-major topic index
+    uint32_t* package_head;          // [n_pairs + 1] 1 where (deliverer, tenant) changes, scanned in place (exclusive)
+    uint32_t* pack_head;             // [n_pairs + 1] 1 where (deliverer, topic) changes, scanned in place (exclusive)
+    uint32_t* pcount;                // [n_deliverers + 1] packages per deliverer
+    unsigned long long* totals;      // [4] pairs nested, packages, packs, offsets[n_topics]
+    // outputs
+    long long* package_off;          // [n_deliverers + 1]
+    uint32_t* package_tenant;        // [n_pairs] (n_packages used)
+    long long* pack_off;             // [n_pairs + 1] (n_packages + 1 used)
+    uint32_t* pack_topic;            // [n_pairs] (n_packs used)
+    long long* match_off;            // [n_pairs + 1] (n_packs + 1 used)
+    uint32_t* match_rank;            // [n_pairs]
+    uint32_t* match_member;          // [n_pairs]
+};
+// d_tmp == nullptr: query the scratch size of the sorts and scans. Enqueues everything on `stream`; totals[] is written last.
+cudaError_t launch_delivery(const DeliveryParams& q, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream);
+
 // (subBrokerId, delivererKey) -> dense id, append-only and shared by every snapshot of an index (ids stay valid across commits
 // and resets, and are never freed)
 struct DelivererTable {

@@ -119,6 +119,54 @@ class BatchResult:
         self.close()
 
 
+class DeliveryResult:
+    """One bfq_delivery_device result: the raw struct's fields (d_package_off, n_packs, ordered_share_id, ...) plus nesting()."""
+
+    def __init__(self, raw):
+        self.raw = raw
+
+    def __getattr__(self, name):
+        if name == "raw":
+            raise AttributeError(name)
+        return getattr(self.raw, name)
+
+    def arrays(self, device=None):
+        """the seven arrays copied to the host (numpy), after a device synchronise"""
+        import torch
+
+        from .dist import device_view
+        torch.cuda.synchronize(device)
+        r = self.raw
+
+        def get(p, n, t):
+            return device_view(p, max(n, 1), t, device).cpu().numpy()[:n].astype(np.int64)
+        return {"package_off": get(r.d_package_off, r.n_deliverers + 1, "<i8"),
+                "package_tenant": get(r.d_package_tenant, r.n_packages, "<u4"),
+                "pack_off": get(r.d_pack_off, r.n_packages + 1, "<i8"),
+                "pack_topic": get(r.d_pack_topic, r.n_packs, "<u4"),
+                "match_off": get(r.d_match_off, r.n_packs + 1, "<i8"),
+                "match_rank": get(r.d_match_rank, r.n_pairs, "<u4"),
+                "match_member": get(r.d_match_member, r.n_pairs, "<u4")}
+
+    def nesting(self, device=None):
+        """{deliverer id: {tenant index: [(topic position, {(rank, member), ...}), ...]}}: deliverers without pairs are left
+        out, packages in ascending tenant order, packs in their order. For tests and small batches: the walk is on the host."""
+        a = self.arrays(device)
+        out = {}
+        for d in range(self.raw.n_deliverers):
+            p0, p1 = int(a["package_off"][d]), int(a["package_off"][d + 1])
+            if p0 == p1:
+                continue
+            pkgs = out[d] = {}
+            for p in range(p0, p1):
+                packs = pkgs[int(a["package_tenant"][p])] = []
+                for k in range(int(a["pack_off"][p]), int(a["pack_off"][p + 1])):
+                    m0, m1 = int(a["match_off"][k]), int(a["match_off"][k + 1])
+                    packs.append((int(a["pack_topic"][k]),
+                                  set(zip(a["match_rank"][m0:m1].tolist(), a["match_member"][m0:m1].tolist()))))
+        return out
+
+
 class DeviceResult:
     """One bfq_match_device[_async] result: device pointers + counts; the buffers stay valid until release()."""
 
@@ -160,6 +208,14 @@ class DeviceResult:
         out = N.BfqFanoutResult()
         N.check(N.lib.bfq_fanout_device(C.byref(self.raw), d_offsets_ptr, d_ranks_ptr, n_pairs, stream, C.byref(out)))
         return out
+
+    def delivery(self, d_offsets_ptr, d_ranks_ptr, n_pairs, d_topic_tenant_ptr, stream=0):
+        """bfq_delivery_device: the same pairs nested per deliverer, tenant and topic position, as BatchDeliveryCall sends
+        them -> DeliveryResult (device pointers into this result's workspace)"""
+        out = N.BfqDeliveryResult()
+        N.check(N.lib.bfq_delivery_device(C.byref(self.raw), d_offsets_ptr, d_ranks_ptr, n_pairs, d_topic_tenant_ptr, stream,
+                                          C.byref(out)))
+        return DeliveryResult(out)
 
     def release(self):
         if getattr(self, "raw", None) is not None and self.raw.lease:

@@ -343,6 +343,48 @@ int32_t bfq_fanout_device(const bfq_device_result* res, const int64_t* d_offsets
 int32_t bfq_fanout_deliverer(bfq_index* h, int32_t id, int32_t* sub_broker_id, uint8_t* key_out, int64_t key_cap, int64_t* key_len);
 
 /* ------------------------------------------------------------------------------------------------
+ * Delivery requests on the device: the fan-out laid out the way a deliverer sends it. Every DeliveryCall goes to the
+ * deliverer's batcher, BatchDeliveryCall (bifromq-deliverer/.../BatchDeliveryCall.java:58,75-104), which nests the calls as
+ * tenantId -> TopicMessagePack -> Set<MatchInfo> and sends one DeliveryRequest
+ * (map<tenantId, DeliveryPackage{repeated DeliveryPack{messagePack, repeated MatchInfo}}>, subbroker/type.proto:28-38).
+ * bfq_delivery_device returns the pairs of a device CSR already in that nesting:
+ *   deliverer d's packages  [d_package_off[d], d_package_off[d + 1]); a package is one (deliverer, tenant): its tenant is
+ *                           d_package_tenant[p] (index into the match's tenant list), ascending within a deliverer, each tenant at
+ *                           most once per deliverer even when the batch interleaves tenants
+ *   package p's packs       [d_pack_off[p], d_pack_off[p + 1]); a pack is one (deliverer, topic position): d_pack_topic[k],
+ *                           ascending within a package (the order BatchDeliveryCall.add sees when a request's packs are submitted
+ *                           in order). Repeated (tenant, topic) positions stay separate packs (separate TopicMessagePacks), even
+ *                           though the match de-duplicated them.
+ *   pack k's MatchInfos     pairs [d_match_off[k], d_match_off[k + 1]): d_match_rank (route rank of the result's snapshot) and
+ *                           d_match_member (member index of a $share, 0xFFFFFFFF otherwise). Order inside a pack is unspecified
+ *                           (the reference keeps a HashSet); no pair appears twice.
+ * Input: the device CSR bfq_fanout_device takes (bfq_expand_device or bfq_expand_device_budget) and d_topic_tenant, the device
+ * array the match itself took. A topic whose tenant index is outside the match's list has no pairs (n_pairs counts the pairs
+ * nested). Deliverer ids, ordered_share_id and the $share member pick are exactly those of bfq_fanout_device for the same
+ * result and CSR (one device function resolves both); $oshare pairs and groups without members are nested under
+ * ordered_share_id like any other deliverer.
+ * The arrays live in the result's leased workspace until bfq_device_result_release, in buffers separate from the fan-out's (both
+ * calls may be used on one result); calling this again on the same result overwrites them. The call synchronises `stream` once
+ * (to read n_packages and n_packs). Limits as bfq_fanout_device: fewer than 2^32 pairs and ranks below 2^32, else BFQ_E_RANGE.
+ * Errors: BFQ_E_INVALID for a NULL array the call needs, an n_pairs that disagrees with d_offsets[n_topics] (checked on the
+ * device: nothing is nested) or a receiver url without a delivererKey; BFQ_E_STATE for a match that has not completed.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+    const int64_t* d_package_off;     /* [n_deliverers + 1] */
+    const uint32_t* d_package_tenant; /* [n_packages] */
+    const int64_t* d_pack_off;        /* [n_packages + 1] */
+    const uint32_t* d_pack_topic;     /* [n_packs] */
+    const int64_t* d_match_off;       /* [n_packs + 1] */
+    const uint32_t* d_match_rank;     /* [n_pairs] */
+    const uint32_t* d_match_member;   /* [n_pairs] */
+    int64_t n_pairs, n_packages, n_packs;
+    int32_t n_deliverers, ordered_share_id;
+    uint64_t generation;
+} bfq_delivery_result;
+int32_t bfq_delivery_device(const bfq_device_result* res, const int64_t* d_offsets, const int64_t* d_ranks, int64_t n_pairs,
+                            const int32_t* d_topic_tenant, void* stream, bfq_delivery_result* out);
+
+/* ------------------------------------------------------------------------------------------------
  * Multi-GPU: the one exchange step of the tenant-sharded path (SURVEY.md 8e). Tenants are independent key ranges, so
  * every GPU (one process each) matches the topics of the tenants it hosts with NO data-path collective; what travels is
  * the reply, reassembled on every rank the way the dist-server reassembles the per-worker BatchDistReply messages
