@@ -18,6 +18,7 @@
 #include "cuda_buf.h"
 #include "index_builder.h"
 #include "fanout.h"
+#include "lease.h"
 #include "match_kernels.cuh"
 
 using namespace bfq;
@@ -83,6 +84,7 @@ struct Workspace {
     cudaEvent_t ev_h2d[MAX_CHUNKS] = {};
     cudaEvent_t evk[2] = {nullptr, nullptr};
     cudaEvent_t ev_done = nullptr;   // device path: recorded behind the last thing a match enqueued (what wait() waits for)
+    std::vector<cudaEvent_t> ev_use; // device path: one per stream the result was used on after the match (lease.h), created on demand
     // resolved tenant table of the previous call on this workspace (reused when the same list comes again)
     uint64_t tab_generation = ~0ull;
     std::vector<uint8_t> tab_blob;
@@ -149,6 +151,7 @@ struct Workspace {
         for (auto& e : evk) if (e) cudaEventDestroy(e);
         for (auto& e : ev_h2d) if (e) cudaEventDestroy(e);
         if (ev_done) cudaEventDestroy(ev_done);
+        for (auto& e : ev_use) cudaEventDestroy(e);
         if (copy_stream) cudaStreamDestroy(copy_stream);
         for (auto& w : work_stream) if (w) cudaStreamDestroy(w);
         if (stream) cudaStreamDestroy(stream);
@@ -632,6 +635,10 @@ struct DeviceLease {
     int32_t rc = BFQ_OK;
     CoreOut co;
     double tier0_ms = 0;
+    // streams the result was used on after the match; stream i's last use is recorded on ws->ev_use[i] (lease.h). One event
+    // per stream: re-recording covers that stream's earlier uses, but not another stream's.
+    std::mutex use_mu;
+    std::vector<cudaStream_t> used_on;
 };
 
 void fill_device_result(const DeviceLease* L, bfq_device_result* out) {
@@ -1940,7 +1947,9 @@ void bfq_device_result_release(bfq_device_result* out) {
     if (!out || !out->lease) return;
     auto* L = static_cast<DeviceLease*>(out->lease);
     cudaSetDevice(L->pool->device);
-    if (!L->done) cudaEventSynchronize(L->ws->ev_done);   // never hand a busy workspace back
+    // never hand a busy workspace back: the match, and every call that used the result since, on each of its streams
+    cudaEventSynchronize(L->ws->ev_done);
+    for (size_t i = 0; i < L->used_on.size(); i++) cudaEventSynchronize(L->ws->ev_use[i]);
     give_back(L->pool, L->ws);
     delete L;
     out->lease = nullptr;
@@ -1958,6 +1967,27 @@ int32_t bfq_match_device(bfq_index* h, const uint8_t* tenants, const int64_t* te
 }
 
 }  // extern "C"
+
+int32_t bfq::lease_use(const bfq_device_result* res, cudaStream_t stream, const char* who, cudaEvent_t* ev) {
+    if (!res || !res->lease) return fail(BFQ_E_INVALID, std::string(who) + ": no match in flight behind this result");
+    auto* L = static_cast<DeviceLease*>(res->lease);
+    if (!L->done || L->rc != BFQ_OK) return fail(BFQ_E_STATE, std::string(who) + " needs a completed match (bfq_device_result_wait)");
+    BFQ_CUDA_TRY(cudaSetDevice(L->h->device));
+    std::lock_guard<std::mutex> g(L->use_mu);
+    size_t i = 0;
+    while (i < L->used_on.size() && L->used_on[i] != stream) i++;
+    if (i == L->used_on.size()) {
+        Workspace* w = L->ws;
+        if (w->ev_use.size() == i) {
+            cudaEvent_t e = nullptr;
+            BFQ_CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+            w->ev_use.push_back(e);
+        }
+        L->used_on.push_back(stream);
+    }
+    *ev = L->ws->ev_use[i];
+    return BFQ_OK;
+}
 
 namespace {
 // the expand's inputs for a completed device match (its workspace, snapshot and caps) and the caller's CSR outputs
@@ -1995,12 +2025,14 @@ int32_t bfq_expand_device(const bfq_device_result* res, int64_t* d_offsets, int6
                           int64_t* n_ranks) {
     if (!res || !res->lease || !d_offsets) return fail(BFQ_E_INVALID, "bad argument");
     auto* L = static_cast<DeviceLease*>(res->lease);
-    if (!L->done || L->rc != BFQ_OK) return fail(BFQ_E_STATE, "bfq_expand_device needs a completed match (bfq_device_result_wait)");
+    cudaStream_t st = (cudaStream_t) stream;
+    cudaEvent_t ev = nullptr;
+    const int32_t rc = lease_use(res, st, "bfq_expand_device", &ev);
+    if (rc != BFQ_OK) return rc;
+    RecordOnExit rec(ev, st);   // phase 2 is still running when the call returns
     bfq_index* h = L->h;
     Workspace* w = L->ws;
     const int64_t n_topics = L->n;
-    BFQ_CUDA_TRY(cudaSetDevice(h->device));
-    cudaStream_t st = (cudaStream_t) stream;
     BFQ_CUDA_TRY(w->d_exp_counts.reserve((size_t) n_topics + 1));
     const ExpandParams p = expand_params(L, d_offsets, d_ranks, rank_cap);
     size_t tmp_bytes = 0;
@@ -2026,7 +2058,11 @@ int32_t bfq_expand_device_budget(const bfq_device_result* res, const int32_t* d_
                                  void* stream, bfq_budget_result* out) {
     if (!res || !res->lease || !d_offsets || !out) return fail(BFQ_E_INVALID, "bad argument");
     auto* L = static_cast<DeviceLease*>(res->lease);
-    if (!L->done || L->rc != BFQ_OK) return fail(BFQ_E_STATE, "bfq_expand_device_budget needs a completed match (bfq_device_result_wait)");
+    cudaStream_t st = (cudaStream_t) stream;
+    cudaEvent_t ev = nullptr;
+    const int32_t rc = lease_use(res, st, "bfq_expand_device_budget", &ev);
+    if (rc != BFQ_OK) return rc;
+    RecordOnExit rec(ev, st);   // phase 2 is still running when the call returns
     const int64_t n_topics = L->n;
     const int32_t n_tenants = L->ctx.n_tenants;
     if (n_topics > 0 && !d_msg_bytes) return fail(BFQ_E_INVALID, "NULL d_msg_bytes");
@@ -2037,8 +2073,6 @@ int32_t bfq_expand_device_budget(const bfq_device_result* res, const int32_t* d_
                                            ": MaxPersistentFanoutBytes must be > 0");
     bfq_index* h = L->h;
     Workspace* w = L->ws;
-    BFQ_CUDA_TRY(cudaSetDevice(h->device));
-    cudaStream_t st = (cudaStream_t) stream;
     const size_t nn = (size_t) std::max<int64_t>(n_topics, 1), nt = (size_t) std::max(n_tenants, 1);
     BFQ_CUDA_TRY(w->d_exp_counts.reserve(nn + 1));
     BFQ_CUDA_TRY(w->d_bud_bytes.reserve(nt));
@@ -2160,15 +2194,17 @@ int32_t bfq_fanout_device(const bfq_device_result* res, const int64_t* d_offsets
                           bfq_fanout_result* out) {
     if (!res || !res->lease || !out || !d_offsets || n_pairs < 0 || (n_pairs > 0 && !d_ranks)) return fail(BFQ_E_INVALID, "bad argument");
     auto* L = static_cast<DeviceLease*>(res->lease);
-    if (!L->done || L->rc != BFQ_OK) return fail(BFQ_E_STATE, "bfq_fanout_device needs a completed match (bfq_device_result_wait)");
+    cudaStream_t st = (cudaStream_t) stream;
+    cudaEvent_t ev = nullptr;
+    int32_t rc = lease_use(res, st, "bfq_fanout_device", &ev);
+    if (rc != BFQ_OK) return rc;
+    RecordOnExit rec(ev, st);   // the call never synchronises: every pass is still queued when it returns
     if (n_pairs >= (int64_t) 0xFFFFFFF0ll) return fail(BFQ_E_RANGE, "more than 2^32 (topic, route) pairs in one batch; split the batch");
     bfq_index* h = L->h;
     Workspace* w = L->ws;
-    BFQ_CUDA_TRY(cudaSetDevice(h->device));
     std::shared_ptr<Snapshot::FanTable> ft;
-    int32_t rc = ensure_fan_table(h, L->snap.get(), &ft);
+    rc = ensure_fan_table(h, L->snap.get(), &ft);
     if (rc != BFQ_OK) return rc;
-    cudaStream_t st = (cudaStream_t) stream;
     bool force_global;
     {
         std::lock_guard<std::mutex> g(h->mu);
@@ -2220,16 +2256,18 @@ int32_t bfq_delivery_device(const bfq_device_result* res, const int64_t* d_offse
                             const int32_t* d_topic_tenant, void* stream, bfq_delivery_result* out) {
     if (!res || !res->lease || !out || !d_offsets || n_pairs < 0 || (n_pairs > 0 && !d_ranks)) return fail(BFQ_E_INVALID, "bad argument");
     auto* L = static_cast<DeviceLease*>(res->lease);
-    if (!L->done || L->rc != BFQ_OK) return fail(BFQ_E_STATE, "bfq_delivery_device needs a completed match (bfq_device_result_wait)");
+    cudaStream_t st = (cudaStream_t) stream;
+    cudaEvent_t ev = nullptr;
+    int32_t rc = lease_use(res, st, "bfq_delivery_device", &ev);
+    if (rc != BFQ_OK) return rc;
+    RecordOnExit rec(ev, st);   // the call synchronises after its last launch, but an error return may come before that
     if (L->n > 0 && !d_topic_tenant) return fail(BFQ_E_INVALID, "NULL d_topic_tenant");
     if (n_pairs >= (int64_t) 0xFFFFFFF0ll) return fail(BFQ_E_RANGE, "more than 2^32 (topic, route) pairs in one batch; split the batch");
     bfq_index* h = L->h;
     Workspace* w = L->ws;
-    BFQ_CUDA_TRY(cudaSetDevice(h->device));
     std::shared_ptr<Snapshot::FanTable> ft;
-    int32_t rc = ensure_fan_table(h, L->snap.get(), &ft);
+    rc = ensure_fan_table(h, L->snap.get(), &ft);
     if (rc != BFQ_OK) return rc;
-    cudaStream_t st = (cudaStream_t) stream;
     const int64_t T = L->n;
     const size_t np = (size_t) std::max<int64_t>(n_pairs, 1);
     BFQ_CUDA_TRY(w->d_dl_topic_tmp.reserve(6 * (size_t) T + 2));

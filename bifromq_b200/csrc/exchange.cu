@@ -25,6 +25,7 @@
 
 #include "../../include/bfq_gpumatch.h"
 #include "cuda_buf.h"
+#include "lease.h"
 #include "match_kernels.cuh"
 
 using namespace bfq;
@@ -158,8 +159,12 @@ void bfq_exchange_destroy(bfq_exchange* x) { delete x; }
 int32_t bfq_exchange_gather(bfq_exchange* x, const bfq_device_result* res, int32_t what, void* stream, bfq_gathered* out) {
     if (!x || !res || !out) return fail(BFQ_E_INVALID, "bad argument");
     if (what != BFQ_EXCHANGE_COUNTS && what != BFQ_EXCHANGE_RANGES) return fail(BFQ_E_INVALID, "what: BFQ_EXCHANGE_COUNTS or BFQ_EXCHANGE_RANGES");
-    BFQ_CUDA_TRY(cudaSetDevice(x->device));
     cudaStream_t st = (cudaStream_t) stream;
+    cudaEvent_t ev = nullptr;
+    const int32_t rc = lease_use(res, st, "bfq_exchange_gather", &ev);
+    if (rc != BFQ_OK) return rc;
+    RecordOnExit rec(ev, st);   // the compaction's phase 2 reads the result's ranges after the call's one synchronisation
+    BFQ_CUDA_TRY(cudaSetDevice(x->device));
     const int64_t n = res->n_topics;
     const int W = x->world;
     const bool with_ranges = what == BFQ_EXCHANGE_RANGES;

@@ -204,7 +204,13 @@ void bfq_result_free(bfq_result* r);
  *                           batch is then re-run and the d_* pointers may change — read them after the wait).
  *   bfq_match_device        = async + wait.
  * The result buffers belong to a workspace leased to this result: they stay valid until bfq_device_result_release,
- * whatever else runs on the handle. Several matches may be in flight on one handle (and one stream) at a time. */
+ * whatever else runs on the handle. Several matches may be in flight on one handle (and one stream) at a time.
+ *   bfq_device_result_release  blocks until the match and everything the library enqueued for the result since
+ *                           (bfq_expand_device, bfq_expand_device_budget, bfq_fanout_device, bfq_delivery_device,
+ *                           bfq_exchange_gather), on every stream it was used on, has finished; then the workspace goes back
+ *                           to the handle's pool, where the next match may take it. The caller's own work that reads the
+ *                           result's arrays (or the CSR and fan-out arrays that live in its workspace) must be ordered
+ *                           before the release by the caller. */
 typedef struct {
     const uint32_t* d_span_begin;   /* [n_topics] */
     const uint32_t* d_span_count;   /* [n_topics] */
@@ -399,6 +405,9 @@ int32_t bfq_delivery_device(const bfq_device_result* res, const int64_t* d_offse
  *   per batch, every rank: bfq_match_device(...) ; bfq_exchange_gather(x, &res, what, stream, &g)   (collective)
  * The gathered arrays live in device memory owned by the exchange, valid until the next gather on it; topic_base /
  * range_base (host, [world + 1]) give each rank's slice. A world of 1 is allowed (the gather is then a local compaction).
+ * The gather reads the result's arrays on `stream` after its host synchronisation, so it returns while that work may still
+ * run: bfq_device_result_release waits for it, and nothing else needs to. Errors: BFQ_E_STATE for a match that has not
+ * completed (bfq_device_result_wait), BFQ_E_INVALID for a result without a match behind it.
  * ---------------------------------------------------------------------------------------------- */
 #define BFQ_EXCHANGE_ID_BYTES 128
 #define BFQ_EXCHANGE_COUNTS 1
