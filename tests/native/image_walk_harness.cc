@@ -11,6 +11,12 @@
 //                                <dir>/topics.bin topic_off.bin topic_tenant.bin (int32)
 //                                <dir>/deltas.bin (optional)  records: u8 op (1 = upsert, 2 = erase), u32 klen, key, u32 vlen, val
 //                         writes <dir>/out_off.bin (int64[n + 1]) out_ranks.bin (int64, ascending per topic)
+//   image_walk <dir> dump  also writes <dir>/dump.txt: the image's tag-table size, then for every topic read as a node path
+//                          (its levels as exact edges, '+' as the '+' child) the node reached at each depth with its record id
+//                          and child lookup, then every tag block's 16 bytes:
+//                            n_blocks <n>
+//                            node <topic> <depth> <id or NONE> <none|single|perfect|big> <lg> <seed or fingerprint>
+//                            tags <block> <32 hex digits, byte 0 first>
 #include <algorithm>
 #include <cstdio>
 #include <cstring>
@@ -177,6 +183,35 @@ int main(int argc, char** argv) {
             im.match(ROOT_BASE + it->second, sv((const char*) topics.data() + topic_off[(size_t) i], (size_t) (topic_off[(size_t) i + 1] - topic_off[(size_t) i])), &one);
         out_ranks.insert(out_ranks.end(), one.begin(), one.end());
         out_off.push_back((int64_t) out_ranks.size());
+    }
+    if (argc > 2 && std::string(argv[2]) == "dump") {
+        FILE* d = fopen((dir + "/dump.txt").c_str(), "w");
+        fprintf(d, "n_blocks %u\n", im.f.n_blocks);
+        for (int64_t i = 0; i < n; i++) {
+            const int32_t t = topic_tenant[(size_t) i];
+            const std::string tid((const char*) tenants.data() + tenant_off[(size_t) t], (size_t) (tenant_off[(size_t) t + 1] - tenant_off[(size_t) t]));
+            auto it = im.f.tenant_ordinal.find(tid);
+            uint32_t id = it == im.f.tenant_ordinal.end() ? NONE : ROOT_BASE + it->second;
+            std::vector<sv> levels;
+            for_each_level(sv((const char*) topics.data() + topic_off[(size_t) i], (size_t) (topic_off[(size_t) i + 1] - topic_off[(size_t) i])), '/',
+                           [&](sv l) { levels.push_back(l); });
+            for (size_t k = 0; k <= levels.size() && id != NONE; k++) {
+                if (k > 0) id = levels[k - 1] == "+" ? im.rec(id).w[W_PLUS] : im.level_child(id, levels[k - 1]);
+                if (id == NONE) {
+                    fprintf(d, "node %lld %zu NONE none 0 0\n", (long long) i, k);
+                    break;
+                }
+                const uint32_t meta = im.rec(id).w[W_META];
+                const char* kind = !(meta & FLAG_HAS_EXACT) ? "none" : (meta & FLAG_BIG) ? "big" : meta_log2size(meta) ? "perfect" : "single";
+                fprintf(d, "node %lld %zu %u %s %u %u\n", (long long) i, k, id, kind, meta_log2size(meta), meta >> 16);
+            }
+        }
+        for (uint32_t b = 0; b < im.f.n_blocks; b++) {
+            fprintf(d, "tags %u ", b);
+            for (uint32_t j = 0; j < 16; j++) fprintf(d, "%02x", im.f.tags[(size_t) b * 16 + j]);
+            fprintf(d, "\n");
+        }
+        fclose(d);
     }
     std::ofstream(dir + "/out_off.bin", std::ios::binary).write((const char*) out_off.data(), (std::streamsize) (out_off.size() * 8));
     std::ofstream(dir + "/out_ranks.bin", std::ios::binary).write((const char*) out_ranks.data(), (std::streamsize) (out_ranks.size() * 8));

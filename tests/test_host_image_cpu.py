@@ -39,8 +39,9 @@ def _blob(items):
 PIECES = {"BFQ_INSERT_PARALLEL_MIN": "2", "BFQ_INSERT_THREADS": "6"}   # force the several-thread insertion of large tenants
 
 
-def walk(walker, tmp, pairs, tenants, topics, tt, deltas=(), env=None):
-    """pairs: the KV handed to load (sorted); deltas: [("put", key, value) | ("del", key)] staged on top, like bfq_index_apply"""
+def walk(walker, tmp, pairs, tenants, topics, tt, deltas=(), env=None, dump=False):
+    """pairs: the KV handed to load (sorted); deltas: [("put", key, value) | ("del", key)] staged on top, like bfq_index_apply;
+    dump: the harness also writes <tmp>/dump.txt (node ids and kinds along every topic, every tag block)"""
     os.makedirs(tmp, exist_ok=True)
     kb, ko = _blob([k for k, _ in pairs])
     vb, vo = _blob([v for _, v in pairs])
@@ -56,7 +57,8 @@ def walk(walker, tmp, pairs, tenants, topics, tt, deltas=(), env=None):
             k = d[1]
             v = d[2] if d[0] == "put" else b""
             f.write(struct.pack("<BI", 1 if d[0] == "put" else 2, len(k)) + k + struct.pack("<I", len(v)) + v)
-    r = subprocess.run([walker, tmp], capture_output=True, text=True, timeout=300, env=dict(os.environ, **(env or {})))
+    r = subprocess.run([walker, tmp] + (["dump"] if dump else []), capture_output=True, text=True, timeout=300,
+                       env=dict(os.environ, **(env or {})))
     assert r.returncode == 0, r.stdout + r.stderr
     return np.fromfile(os.path.join(tmp, "out_off.bin"), np.int64), np.fromfile(os.path.join(tmp, "out_ranks.bin"), np.int64), r.stdout
 

@@ -62,54 +62,8 @@ def wide_tenants(pairs):
     return sorted(t for t, c in fan.items() if c >= WIDE_MIN)
 
 
-# ---- a model of the tag table (trie_layout.h) for an index whose only wide node is one tenant's root: its children claim slots
-# in key order, each in the first block of its probe sequence with a free slot, setting the overflow byte of every full block
-# it walks past. A delta commit frees all of the tenant's slots first, so it re-places them into an empty table whose overflow
-# bytes stay as they were. The GPU tests predict the path of every commit at the tag table's bounds from it.
-_M = (1 << 64) - 1
-_TOKC = [0x9E3779B97F4A7C15, 0xA24BAED4963EE407, 0x9FB21C651E98DF25, 0xD6E8FEB86659FD93, 0xCA5A826395121157, 0x8CB92BA72F3D8DD7,
-         0xE7037ED1A0B428DB]
-ROOT_BASE = 0x80000000
-
-
-def _fmix64(k):
-    k ^= k >> 33
-    k = (k * 0xff51afd7ed558ccd) & _M
-    k ^= k >> 33
-    k = (k * 0xc4ceb9fe1a85ec53) & _M
-    return k ^ (k >> 33)
-
-
-def home_block(level, parent, n_blocks):
-    b = level.encode()
-    assert len(b) <= 24
-    w = np.frombuffer(b.ljust(24, b"\0"), "<u4").tolist()
-    h = len(b) * _TOKC[0] + sum(int(x) * c for x, c in zip(w, _TOKC[1:]))
-    e = _fmix64((h + parent * 0xC2B2AE3D27D4EB4F) & _M)
-    return ((e >> 32) * n_blocks) >> 32
-
-
-class TagModel:
-    def __init__(self, n_edges):
-        """the table a full build makes for n_edges wide edges (load 0.5, at least 64 blocks of 15 usable slots)"""
-        self.n_blocks = max(64, (2 * n_edges + 14) // 15)
-        self.usable = 15 * self.n_blocks
-        self.overflowed = set()
-
-    def place(self, names, ordinal):
-        """the tenant's root children (same-length names: key order == sorted order); returns the overflowed block count"""
-        occ = [0] * self.n_blocks
-        for nm in sorted(names):
-            b = home_block(nm, ROOT_BASE + ordinal, self.n_blocks)
-            while occ[b] == 15:
-                self.overflowed.add(b)
-                b = (b + 1) % self.n_blocks
-            occ[b] += 1
-        return len(self.overflowed)
-
-    def path(self, n_edges, overflowed):
-        """the path the delta rules give a commit that leaves n_edges claimed and `overflowed` blocks overflowed"""
-        return "full" if 4 * n_edges > 3 * self.usable or 4 * overflowed > self.n_blocks else "delta"
+# the tag-table model the GPU tests use to predict commit paths lives in tests/trie_hash.py
+from trie_hash import ROOT_BASE, TagModel, level_home_block as home_block  # noqa: E402,F401
 
 
 def route(tenant, tf, i, broker=0):
