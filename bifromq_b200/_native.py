@@ -51,6 +51,11 @@ class BfqDeliveryResult(C.Structure):
                 ("n_deliverers", C.c_int32), ("ordered_share_id", C.c_int32), ("generation", C.c_uint64)]
 
 
+class BfqDeliveryOrderedResult(C.Structure):
+    _fields_ = [("d", BfqDeliveryResult), ("d_pack_pub_off", C.c_void_p), ("d_pack_pub", C.c_void_p), ("n_pack_pubs", C.c_int64),
+                ("n_ordered_packs", C.c_int64)]
+
+
 class BfqBudgetResult(C.Structure):
     _fields_ = [("d_delivered_persistent", C.c_void_p), ("d_topic_flags", C.c_void_p), ("n_delivered", C.c_int64),
                 ("n_dropped_bytes", C.c_int64), ("n_dropped_persistent_bandwidth", C.c_int64),
@@ -99,6 +104,8 @@ _SIGNATURES = {
     "bfq_fanout_device": (_i32, [C.POINTER(BfqDeviceResult), _vp, _vp, _i64, _vp, C.POINTER(BfqFanoutResult)]),
     "bfq_fanout_deliverer": (_i32, [_vp, _i32, C.POINTER(_i32), _vp, _i64, C.POINTER(_i64)]),
     "bfq_delivery_device": (_i32, [C.POINTER(BfqDeviceResult), _vp, _vp, _i64, _vp, _vp, C.POINTER(BfqDeliveryResult)]),
+    "bfq_delivery_device_ordered": (_i32, [C.POINTER(BfqDeviceResult), _vp, _vp, _i64, _vp, _vp, _vp, _i64, _vp,
+                                           C.POINTER(BfqDeliveryOrderedResult)]),
     "bfq_exchange_unique_id": (_i32, [_vp, _i32]),
     "bfq_exchange_create": (_i32, [_i32, _i32, _i32, _vp, C.POINTER(_vp)]),
     "bfq_exchange_destroy": (None, [_vp]),

@@ -47,8 +47,16 @@ struct Snapshot {
         DeviceBuf<uint8_t> d_gordered;
         uint32_t n_deliverers = 0;   // incl. the reserved last id (ordered shared subscriptions)
     };
+    // receiverUrls of the ordered groups' members (device), for the $oshare pick: built on the first ordered delivery call
+    struct UrlTable {
+        DeviceBuf<unsigned long long> d_words;   // member m: its url at byte 4 of words d_word[m] .., zero-padded
+        DeviceBuf<long long> d_word;             // [members of the fan table]
+        DeviceBuf<uint32_t> d_len;
+        uint32_t member_bits = 1;                // bits of the largest ordered group's size
+    };
     std::mutex fan_mu;
     std::shared_ptr<FanTable> fan;
+    std::shared_ptr<UrlTable> urls;
     std::vector<TenantHost> th;
     uint64_t garbage_slots = 0;   // slots of regions that delta commits replaced (reclaimed by the next full build)
     int64_t delta_commits = 0;    // delta commits since the last full build
@@ -125,6 +133,11 @@ struct Workspace {
     DeviceBuf<unsigned long long> d_dl_totals;
     DeviceBuf<long long> d_package_off, d_dl_pack_off, d_match_off;
     DeviceBuf<uint8_t> d_dl_tmp;
+    // $oshare resolution (bfq_delivery_device_ordered): per CSR pair flags and item counts, the check words, the sort keys of
+    // pairs and items, the per-item / per-emit-position words, and the publisher outputs
+    DeviceBuf<uint32_t> d_os_flag, d_os_u32, d_pack_pub;
+    DeviceBuf<unsigned long long> d_os_items, d_os_check, d_os_key;
+    DeviceBuf<long long> d_pack_pub_off;
     // pinned result buffers
     PinnedBuf<uint32_t> h_span_begin, h_span_count, h_route_count;
     PinnedBuf<uint2> h_ranges;
@@ -2188,6 +2201,45 @@ int32_t ensure_fan_table(bfq_index* h, Snapshot* s, std::shared_ptr<Snapshot::Fa
     *out = ft;
     return BFQ_OK;
 }
+
+// the snapshot's ordered-group member urls, from the tenants' fan-out tables (call after ensure_fan_table), in the fan table's
+// member order: each url at byte 4 of its own run of 8-byte words, so the pick reads LE32(hash) ‖ url as whole words
+int32_t ensure_url_table(Snapshot* s, std::shared_ptr<Snapshot::UrlTable>* out) {
+    std::lock_guard<std::mutex> g(s->fan_mu);
+    if (s->urls) {
+        *out = s->urls;
+        return BFQ_OK;
+    }
+    std::vector<unsigned long long> words;
+    std::vector<long long> word;
+    std::vector<uint32_t> len;
+    uint32_t largest = 0;
+    for (const auto& th : s->th) {
+        const TenantFan& tf = *th.fan;
+        for (size_t m = 0; m + 1 < tf.ourl_off.size(); m++) {
+            const uint32_t a = tf.ourl_off[m], n = tf.ourl_off[m + 1] - a;
+            word.push_back((long long) words.size());
+            len.push_back(n);
+            if (n == 0) continue;
+            const size_t w0 = words.size();
+            words.resize(w0 + (4 + (size_t) n + 7) / 8, 0);
+            memcpy(reinterpret_cast<uint8_t*>(words.data() + w0) + 4, tf.ourl.data() + a, n);
+        }
+        for (size_t k = 0; k < tf.gordered.size(); k++)
+            if (tf.gordered[k]) largest = std::max(largest, tf.gmem_off[k + 1] - tf.gmem_off[k]);
+    }
+    auto ut = std::make_shared<Snapshot::UrlTable>();
+    ut->member_bits = largest ? 32u - (uint32_t) __builtin_clz(largest) : 1u;
+    BFQ_CUDA_TRY(ut->d_words.reserve(std::max<size_t>(words.size(), 1)));
+    BFQ_CUDA_TRY(ut->d_word.reserve(std::max<size_t>(word.size(), 1)));
+    BFQ_CUDA_TRY(ut->d_len.reserve(std::max<size_t>(len.size(), 1)));
+    if (!words.empty()) BFQ_CUDA_TRY(cudaMemcpy(ut->d_words.p, words.data(), words.size() * 8, cudaMemcpyHostToDevice));
+    if (!word.empty()) BFQ_CUDA_TRY(cudaMemcpy(ut->d_word.p, word.data(), word.size() * 8, cudaMemcpyHostToDevice));
+    if (!len.empty()) BFQ_CUDA_TRY(cudaMemcpy(ut->d_len.p, len.data(), len.size() * 4, cudaMemcpyHostToDevice));
+    s->urls = ut;
+    *out = ut;
+    return BFQ_OK;
+}
 }  // namespace
 
 int32_t bfq_fanout_device(const bfq_device_result* res, const int64_t* d_offsets, const int64_t* d_ranks, int64_t n_pairs, void* stream,
@@ -2252,35 +2304,35 @@ int32_t bfq_fanout_device(const bfq_device_result* res, const int64_t* d_offsets
     return BFQ_OK;
 }
 
-int32_t bfq_delivery_device(const bfq_device_result* res, const int64_t* d_offsets, const int64_t* d_ranks, int64_t n_pairs,
-                            const int32_t* d_topic_tenant, void* stream, bfq_delivery_result* out) {
-    if (!res || !res->lease || !out || !d_offsets || n_pairs < 0 || (n_pairs > 0 && !d_ranks)) return fail(BFQ_E_INVALID, "bad argument");
+namespace {
+struct PublisherPacks {   // bfq_delivery_device_ordered's publisher arrays
+    const int64_t* pub_off;
+    const int32_t* pub_hash;
+    int64_t n_pubs;
+};
+
+// bfq_delivery_device (pubs == nullptr) and bfq_delivery_device_ordered (pubs and oout set)
+int32_t run_delivery_call(const bfq_device_result* res, const int64_t* d_offsets, const int64_t* d_ranks, int64_t n_pairs,
+                          const int32_t* d_topic_tenant, void* stream, const char* who, const PublisherPacks* pubs,
+                          bfq_delivery_result* out, bfq_delivery_ordered_result* oout) {
     auto* L = static_cast<DeviceLease*>(res->lease);
     cudaStream_t st = (cudaStream_t) stream;
     cudaEvent_t ev = nullptr;
-    int32_t rc = lease_use(res, st, "bfq_delivery_device", &ev);
+    int32_t rc = lease_use(res, st, who, &ev);
     if (rc != BFQ_OK) return rc;
     RecordOnExit rec(ev, st);   // the call synchronises after its last launch, but an error return may come before that
     if (L->n > 0 && !d_topic_tenant) return fail(BFQ_E_INVALID, "NULL d_topic_tenant");
+    if (pubs && !pubs->pub_off) return fail(BFQ_E_INVALID, "NULL d_pub_off");
+    if (pubs && (pubs->n_pubs < 0 || (pubs->n_pubs > 0 && !pubs->pub_hash))) return fail(BFQ_E_INVALID, "bad d_pub_hash / n_pubs");
     if (n_pairs >= (int64_t) 0xFFFFFFF0ll) return fail(BFQ_E_RANGE, "more than 2^32 (topic, route) pairs in one batch; split the batch");
     bfq_index* h = L->h;
     Workspace* w = L->ws;
     std::shared_ptr<Snapshot::FanTable> ft;
     rc = ensure_fan_table(h, L->snap.get(), &ft);
     if (rc != BFQ_OK) return rc;
+    std::shared_ptr<Snapshot::UrlTable> ut;
+    if (pubs && (rc = ensure_url_table(L->snap.get(), &ut)) != BFQ_OK) return rc;
     const int64_t T = L->n;
-    const size_t np = (size_t) std::max<int64_t>(n_pairs, 1);
-    BFQ_CUDA_TRY(w->d_dl_topic_tmp.reserve(6 * (size_t) T + 2));
-    BFQ_CUDA_TRY(w->d_dl_pair_tmp.reserve(10 * np + 2));
-    BFQ_CUDA_TRY(w->d_dl_pcount.reserve((size_t) ft->n_deliverers + 1));
-    BFQ_CUDA_TRY(w->d_dl_totals.reserve(4));
-    BFQ_CUDA_TRY(w->d_package_off.reserve((size_t) ft->n_deliverers + 1));
-    BFQ_CUDA_TRY(w->d_package_tenant.reserve(np));
-    BFQ_CUDA_TRY(w->d_dl_pack_off.reserve(np + 1));
-    BFQ_CUDA_TRY(w->d_dl_pack_topic.reserve(np));
-    BFQ_CUDA_TRY(w->d_match_off.reserve(np + 1));
-    BFQ_CUDA_TRY(w->d_match_rank.reserve(np));
-    BFQ_CUDA_TRY(w->d_match_member.reserve(np));
     DeliveryParams q{};
     q.f.n_topics = T;
     q.f.offsets = d_offsets;
@@ -2293,6 +2345,51 @@ int32_t bfq_delivery_device(const bfq_device_result* res, const int64_t* d_offse
     q.f.n_deliverers = ft->n_deliverers;
     q.topic_tenant = d_topic_tenant;
     q.n_tenants = L->ctx.n_tenants;
+    int64_t n_items = 0;
+    if (pubs) {
+        // phase 1: which pairs are $oshare pairs to resolve, how many (pair, publisher) items, and the d_pub_off check
+        q.oshare = true;
+        q.o.pub_off = pubs->pub_off;
+        q.o.pub_hash = pubs->pub_hash;
+        q.o.n_pubs = pubs->n_pubs;
+        q.o.url_words = ut->d_words.p;
+        q.o.url_word = ut->d_word.p;
+        q.o.url_len = ut->d_len.p;
+        q.o.member_bits = ut->member_bits;
+        BFQ_CUDA_TRY(w->d_os_flag.reserve((size_t) n_pairs + 1));
+        BFQ_CUDA_TRY(w->d_os_items.reserve((size_t) n_pairs + 1));
+        BFQ_CUDA_TRY(w->d_os_check.reserve(4));
+        q.o.oflag = w->d_os_flag.p;
+        q.o.oitems = w->d_os_items.p;
+        q.o.check = w->d_os_check.p;
+        size_t tmp_bytes = 0;
+        BFQ_CUDA_TRY(launch_oshare_count(q, nullptr, &tmp_bytes, st));
+        BFQ_CUDA_TRY(w->d_dl_tmp.reserve(tmp_bytes + 256));
+        BFQ_CUDA_TRY(launch_oshare_count(q, w->d_dl_tmp.p, &tmp_bytes, st));
+        unsigned long long chk[4];
+        BFQ_CUDA_TRY(cudaMemcpyAsync(chk, w->d_os_check.p, sizeof(chk), cudaMemcpyDeviceToHost, st));
+        BFQ_CUDA_TRY(cudaStreamSynchronize(st));
+        if ((int64_t) chk[3] != n_pairs)
+            return fail(BFQ_E_INVALID, "n_pairs = " + std::to_string(n_pairs) + " but d_offsets[n_topics] = " + std::to_string((int64_t) chk[3]));
+        if (chk[2]) return fail(BFQ_E_INVALID, "d_pub_off must run from 0 to n_pubs = " + std::to_string(pubs->n_pubs) + " without decreasing");
+        if (chk[1] >= 0xFFFFFFF0ull || (uint64_t) n_pairs + chk[1] >= 0xFFFFFFF0ull)
+            return fail(BFQ_E_RANGE, "more than 2^32 pairs and ($oshare pair, publisher) items in one batch; split the batch");
+        q.o.n_opairs = (int64_t) chk[0];
+        n_items = (int64_t) chk[1];
+        q.o.n_items = n_items;
+    }
+    const size_t np = (size_t) std::max<int64_t>(n_pairs + n_items, 1);
+    BFQ_CUDA_TRY(w->d_dl_topic_tmp.reserve(6 * (size_t) T + 2));
+    BFQ_CUDA_TRY(w->d_dl_pair_tmp.reserve(10 * np + 2));
+    BFQ_CUDA_TRY(w->d_dl_pcount.reserve((size_t) ft->n_deliverers + 1));
+    BFQ_CUDA_TRY(w->d_dl_totals.reserve(5));
+    BFQ_CUDA_TRY(w->d_package_off.reserve((size_t) ft->n_deliverers + 1));
+    BFQ_CUDA_TRY(w->d_package_tenant.reserve(np));
+    BFQ_CUDA_TRY(w->d_dl_pack_off.reserve(np + 1));
+    BFQ_CUDA_TRY(w->d_dl_pack_topic.reserve(np));
+    BFQ_CUDA_TRY(w->d_match_off.reserve(np + 1));
+    BFQ_CUDA_TRY(w->d_match_rank.reserve(np));
+    BFQ_CUDA_TRY(w->d_match_member.reserve(np));
     uint32_t* tt = w->d_dl_topic_tmp.p;
     q.tkey[0] = tt;
     q.tkey[1] = tt + T;
@@ -2320,16 +2417,45 @@ int32_t bfq_delivery_device(const bfq_device_result* res, const int64_t* d_offse
     q.match_off = w->d_match_off.p;
     q.match_rank = w->d_match_rank.p;
     q.match_member = w->d_match_member.p;
+    if (pubs) {
+        const size_t O = (size_t) q.o.n_opairs, I = (size_t) n_items;
+        BFQ_CUDA_TRY(w->d_os_key.reserve(std::max<size_t>(2 * O + 2 * I, 1)));
+        BFQ_CUDA_TRY(w->d_os_u32.reserve((O + 1) + 2 * I + 2 * (I + 1) + I + 3 * np + 1));
+        BFQ_CUDA_TRY(w->d_pack_pub.reserve(std::max<size_t>(I, 1)));
+        BFQ_CUDA_TRY(w->d_pack_pub_off.reserve(np + 1));
+        unsigned long long* kp = w->d_os_key.p;
+        q.o.okey[0] = kp;
+        q.o.okey[1] = kp + O;
+        q.o.ikey[0] = kp + 2 * O;
+        q.o.ikey[1] = kp + 2 * O + I;
+        uint32_t* up = w->d_os_u32.p;
+        q.o.istart = up;
+        up += O + 1;
+        q.o.ival[0] = up;
+        q.o.ival[1] = up + I;
+        up += 2 * I;
+        q.o.ihead = up;
+        up += I + 1;
+        q.o.sub_start = up;
+        up += I + 1;
+        q.o.sub_pack = up;
+        up += I;
+        q.o.e_sub = up;
+        q.o.s_sub = up + np;
+        q.o.pub_count = up + 2 * np;
+        q.o.pack_pub_off = w->d_pack_pub_off.p;
+        q.o.pack_pub = w->d_pack_pub.p;
+    }
     size_t tmp_bytes = 0;
     BFQ_CUDA_TRY(launch_delivery(q, nullptr, &tmp_bytes, st));
     BFQ_CUDA_TRY(w->d_dl_tmp.reserve(tmp_bytes + 256));
     BFQ_CUDA_TRY(launch_delivery(q, w->d_dl_tmp.p, &tmp_bytes, st));
-    unsigned long long tot[4];
-    BFQ_CUDA_TRY(cudaMemcpyAsync(tot, w->d_dl_totals.p, sizeof(tot), cudaMemcpyDeviceToHost, st));
+    unsigned long long tot[5] = {0, 0, 0, 0, 0};
+    BFQ_CUDA_TRY(cudaMemcpyAsync(tot, w->d_dl_totals.p, (pubs ? 5 : 4) * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     BFQ_CUDA_TRY(cudaStreamSynchronize(st));
     {
         std::lock_guard<std::mutex> g(h->mu);
-        h->launches += 11;
+        h->launches += pubs ? 25 : 11;
     }
     if ((int64_t) tot[3] != n_pairs)
         return fail(BFQ_E_INVALID, "n_pairs = " + std::to_string(n_pairs) + " but d_offsets[n_topics] = " + std::to_string((int64_t) tot[3]));
@@ -2346,7 +2472,29 @@ int32_t bfq_delivery_device(const bfq_device_result* res, const int64_t* d_offse
     out->n_deliverers = (int32_t) ft->n_deliverers;
     out->ordered_share_id = (int32_t) ft->n_deliverers - 1;
     out->generation = L->snap->generation;
+    if (oout) {
+        oout->d_pack_pub_off = (const int64_t*) w->d_pack_pub_off.p;
+        oout->d_pack_pub = w->d_pack_pub.p;
+        oout->n_pack_pubs = n_items;
+        oout->n_ordered_packs = (int64_t) tot[4];
+    }
     return BFQ_OK;
+}
+}  // namespace
+
+int32_t bfq_delivery_device(const bfq_device_result* res, const int64_t* d_offsets, const int64_t* d_ranks, int64_t n_pairs,
+                            const int32_t* d_topic_tenant, void* stream, bfq_delivery_result* out) {
+    if (!res || !res->lease || !out || !d_offsets || n_pairs < 0 || (n_pairs > 0 && !d_ranks)) return fail(BFQ_E_INVALID, "bad argument");
+    return run_delivery_call(res, d_offsets, d_ranks, n_pairs, d_topic_tenant, stream, "bfq_delivery_device", nullptr, out, nullptr);
+}
+
+int32_t bfq_delivery_device_ordered(const bfq_device_result* res, const int64_t* d_offsets, const int64_t* d_ranks, int64_t n_pairs,
+                                    const int32_t* d_topic_tenant, const int64_t* d_pub_off, const int32_t* d_pub_hash, int64_t n_pubs,
+                                    void* stream, bfq_delivery_ordered_result* out) {
+    if (!res || !res->lease || !out || !d_offsets || n_pairs < 0 || (n_pairs > 0 && !d_ranks)) return fail(BFQ_E_INVALID, "bad argument");
+    const PublisherPacks pubs{d_pub_off, d_pub_hash, n_pubs};
+    return run_delivery_call(res, d_offsets, d_ranks, n_pairs, d_topic_tenant, stream, "bfq_delivery_device_ordered", &pubs, &out->d,
+                             out);
 }
 
 int32_t bfq_fanout_deliverer(bfq_index* h, int32_t id, int32_t* sub_broker_id, uint8_t* key_out, int64_t key_cap, int64_t* key_len) {

@@ -210,11 +210,27 @@ cudaError_t launch_fanout(const FanoutParams& p, bool tiled, void* d_tmp, size_t
 //                                 (package / pack numbers), one scatter of the offsets
 // Emit positions past the pairs nested (the CSR may hold pairs of a topic without a valid tenant, or disagree with n_pairs)
 // carry the key n_deliverers, so they sort last and are never read back.
+//
+// $oshare resolution (q.oshare, bfq_delivery_device_ordered) adds, between 1 and 2, the ordered branch of
+// DeliverExecutorGroup.send (DW/DeliverExecutorGroup.java:242-278): per ($oshare pair, publisher of its topic position) an
+// "item", per item the rendezvous winner (RendezvousHash.get: the first member whose Guava murmur3_128 score over
+// LE32(publisher hash) ‖ receiverUrl is strictly greater than every earlier one), and per (pair, winner) a "sub-pack" of the
+// publishers that picked it, in publisher order. Each topic then emits its ordinary pairs (the resolved $oshare pairs emit the
+// key n_deliverers: dropped) and after them its sub-packs in (rank, member) order; a sub-pack is a pack of its own. The stable
+// partition keeps that order per deliverer. Kernels templated on OSH: without it they compile to the plain nesting.
 namespace {
 
 constexpr int DL_THREADS = 256;
+constexpr uint32_t NO_SUB = 0xFFFFFFFFu;
 
 uint32_t bits_for(uint32_t v) { return v ? 32u - (uint32_t) __builtin_clz(v) : 1u; }
+
+// emit positions of the nesting: the pairs, plus (with $oshare) room for one sub-pack per item
+template <bool OSH>
+__host__ __device__ __forceinline__ int64_t dl_emit_cap(const DeliveryParams& q) {
+    if constexpr (OSH) return q.f.n_pairs + q.o.n_items;
+    else return q.f.n_pairs;
+}
 
 __global__ void __launch_bounds__(DL_THREADS) delivery_topic_keys_kernel(const DeliveryParams q) {
     const int64_t t = (int64_t) blockIdx.x * DL_THREADS + threadIdx.x;
@@ -224,7 +240,16 @@ __global__ void __launch_bounds__(DL_THREADS) delivery_topic_keys_kernel(const D
     q.tval[0][t] = (uint32_t) t;
 }
 
+// the sub-packs of topic position t: [first, first + n) (OSH; the $oshare pairs of t are the scanned oflag's range over t's
+// pairs, their items istart[] of those, and their sub-packs the item heads before them)
+__device__ __forceinline__ void os_topic_subs(const DeliveryParams& q, uint32_t t, uint32_t* first, uint32_t* n) {
+    const uint32_t olo = q.o.oflag[q.f.offsets[t]], ohi = q.o.oflag[q.f.offsets[t + 1]];
+    *first = q.o.ihead[q.o.istart[olo]];
+    *n = q.o.ihead[q.o.istart[ohi]] - *first;
+}
+
 // pairs of the i-th topic in tenant-major order; none for a topic without a valid tenant, none at all if the CSR's total is not n_pairs
+template <bool OSH>
 __global__ void __launch_bounds__(DL_THREADS) delivery_topic_counts_kernel(const DeliveryParams q, const uint32_t* tkey, const uint32_t* order) {
     const int64_t i = (int64_t) blockIdx.x * DL_THREADS + threadIdx.x;
     if (i > q.f.n_topics) return;
@@ -232,6 +257,11 @@ __global__ void __launch_bounds__(DL_THREADS) delivery_topic_counts_kernel(const
     if (i < q.f.n_topics && tkey[i] < (uint32_t) q.n_tenants && q.f.offsets[q.f.n_topics] == q.f.n_pairs) {
         const uint32_t t = order[i];
         c = (uint32_t) (q.f.offsets[t + 1] - q.f.offsets[t]);
+        if constexpr (OSH) {
+            uint32_t s0, ns;
+            os_topic_subs(q, t, &s0, &ns);
+            c += ns;
+        }
     }
     q.tcount[i] = c;
 }
@@ -248,13 +278,16 @@ __device__ __forceinline__ uint32_t dl_segment_of(const uint32_t* start, int64_t
 }
 
 // a thread owns FO_TILE / FO_THREADS consecutive emit positions, as the fan-out's passes do
+template <bool OSH>
 __global__ void __launch_bounds__(FO_THREADS) delivery_emit_kernel(const DeliveryParams q, const uint32_t* order) {
     constexpr int PER = FO_TILE / FO_THREADS;
+    const int64_t cap = dl_emit_cap<OSH>(q);
     const int64_t j0 = (int64_t) blockIdx.x * FO_TILE + (int64_t) threadIdx.x * PER;
-    if (j0 >= q.f.n_pairs) return;
+    if (j0 >= cap) return;
     const int64_t n_emit = q.tstart[q.f.n_topics];
     uint32_t i = j0 < n_emit ? dl_segment_of(q.tstart, q.f.n_topics, (uint32_t) j0) : 0;
-    for (int k = 0; k < PER && j0 + k < q.f.n_pairs; k++) {
+    uint32_t cur = 0xFFFFFFFFu, s0 = 0, ns = 0;   // OSH: the topic whose sub-packs s0 / ns hold
+    for (int k = 0; k < PER && j0 + k < cap; k++) {
         const uint32_t j = (uint32_t) (j0 + k);
         q.val[0][j] = j;
         if (j >= n_emit) {
@@ -263,21 +296,58 @@ __global__ void __launch_bounds__(FO_THREADS) delivery_emit_kernel(const Deliver
         }
         while (q.tstart[i + 1] <= j) i++;
         const uint32_t t = order[i];
-        const int64_t r = q.f.ranks[q.f.offsets[t] + (j - q.tstart[i])];
-        uint32_t member;
-        q.key[0][j] = fo_deliverer(q.f, t, r, &member);
+        const uint32_t local = j - q.tstart[i];
+        const uint32_t cnt = (uint32_t) (q.f.offsets[t + 1] - q.f.offsets[t]);
+        int64_t r;
+        uint32_t member = 0xFFFFFFFFu, d;
+        if constexpr (OSH) {
+            if (local < cnt) {
+                const int64_t pj = q.f.offsets[t] + local;
+                r = q.f.ranks[pj];
+                // a resolved $oshare pair: its sub-packs stand for it
+                d = q.o.oflag[pj + 1] != q.o.oflag[pj] ? q.f.n_deliverers : fo_deliverer(q.f, t, r, &member);
+                q.o.e_sub[j] = NO_SUB;
+            } else {
+                if (cur != t) {
+                    os_topic_subs(q, t, &s0, &ns);
+                    cur = t;
+                }
+                const uint32_t s = s0 + (local - cnt);
+                const unsigned long long kk = q.o.ikey[0][q.o.sub_start[s]];
+                const uint32_t w = (uint32_t) (kk & ((1ull << q.o.member_bits) - 1));
+                r = (int64_t) (q.o.okey[0][kk >> q.o.member_bits] & 0xFFFFFFFFu);
+                const uint32_t g = q.f.rdeliv[r] & ~FO_GROUP_BIT;
+                const uint32_t b = q.f.gmem_off[g], n = q.f.gmem_off[g + 1] - b;
+                // w == n: every member scored Long.MIN_VALUE, no winner: parked like a member-less group
+                member = w < n ? w : 0xFFFFFFFFu;
+                d = w < n ? q.f.gmem_deliv[b + w] : q.f.n_deliverers - 1;
+                q.o.e_sub[j] = s;
+            }
+        } else {
+            r = q.f.ranks[q.f.offsets[t] + local];
+            d = fo_deliverer(q.f, t, r, &member);
+        }
+        q.key[0][j] = d;
         q.e_topic[j] = i;
         q.e_rank[j] = (uint32_t) r;
         q.e_member[j] = member;
     }
 }
 
+// pairs nested: the emit positions, less the resolved $oshare pairs (their key was n_deliverers)
+template <bool OSH>
+__device__ __forceinline__ int64_t dl_nested(const DeliveryParams& q) {
+    if constexpr (OSH) return (int64_t) q.tstart[q.f.n_topics] - q.o.n_opairs;
+    else return (int64_t) q.tstart[q.f.n_topics];
+}
+
 // nested pair k (deliverer-major): its pair, its tenant-major topic index and its head flags
+template <bool OSH>
 __global__ void __launch_bounds__(DL_THREADS) delivery_gather_kernel(const DeliveryParams q, const uint32_t* skey, const uint32_t* sval,
                                                                      const uint32_t* tkey) {
     const int64_t k = (int64_t) blockIdx.x * DL_THREADS + threadIdx.x;
-    if (k > q.f.n_pairs) return;
-    if (k >= (int64_t) q.tstart[q.f.n_topics]) {
+    if (k > dl_emit_cap<OSH>(q)) return;
+    if (k >= dl_nested<OSH>(q)) {
         q.package_head[k] = 0;
         q.pack_head[k] = 0;
         return;
@@ -291,17 +361,20 @@ __global__ void __launch_bounds__(DL_THREADS) delivery_gather_kernel(const Deliv
         const uint32_t i0 = q.e_topic[sval[k - 1]], d0 = skey[k - 1];
         package = d != d0 || tkey[i] != tkey[i0];
         pack = d != d0 || i != i0;
+        if constexpr (OSH) pack = pack || q.o.e_sub[j] != NO_SUB || q.o.e_sub[sval[k - 1]] != NO_SUB;
     }
+    if constexpr (OSH) q.o.s_sub[k] = q.o.e_sub[j];
     q.package_head[k] = package;
     q.pack_head[k] = pack;
 }
 
-// package_head[] / pack_head[] scanned (exclusive, n_pairs + 1 entries): a head's package / pack number, and the totals at
-// [n_emit]. Thread 0 writes the terminators and the totals.
+// package_head[] / pack_head[] scanned (exclusive, emit cap + 1 entries): a head's package / pack number, and the totals at
+// [pairs nested]. Thread 0 writes the terminators and the totals.
+template <bool OSH>
 __global__ void __launch_bounds__(DL_THREADS) delivery_scatter_kernel(const DeliveryParams q, const uint32_t* skey, const uint32_t* tkey,
                                                                       const uint32_t* order) {
     const int64_t k = (int64_t) blockIdx.x * DL_THREADS + threadIdx.x;
-    const int64_t n_emit = q.tstart[q.f.n_topics];
+    const int64_t n_emit = dl_nested<OSH>(q);
     if (k == 0) {
         const uint32_t n_packages = q.package_head[n_emit], n_packs = q.pack_head[n_emit];
         q.pack_off[n_packages] = n_packs;
@@ -310,6 +383,7 @@ __global__ void __launch_bounds__(DL_THREADS) delivery_scatter_kernel(const Deli
         q.totals[1] = n_packages;
         q.totals[2] = n_packs;
         q.totals[3] = (unsigned long long) q.f.offsets[q.f.n_topics];
+        if constexpr (OSH) q.totals[4] = q.o.ihead[q.o.n_items];
     }
     if (k >= n_emit) return;
     const uint32_t pk = q.pack_head[k], pg = q.package_head[k];
@@ -317,6 +391,13 @@ __global__ void __launch_bounds__(DL_THREADS) delivery_scatter_kernel(const Deli
     if (q.pack_head[k + 1] != pk) {
         q.pack_topic[pk] = order[i];
         q.match_off[pk] = k;
+        if constexpr (OSH) {
+            const uint32_t s = q.o.s_sub[k];
+            if (s != NO_SUB) {
+                q.o.pub_count[pk] = q.o.sub_start[s + 1] - q.o.sub_start[s];
+                q.o.sub_pack[s] = pk;
+            }
+        }
     }
     if (q.package_head[k + 1] != pg) {
         q.package_tenant[pg] = tkey[i];
@@ -327,23 +408,214 @@ __global__ void __launch_bounds__(DL_THREADS) delivery_scatter_kernel(const Deli
 
 unsigned dl_blocks(int64_t n) { return (unsigned) std::max<int64_t>(1, (n + DL_THREADS - 1) / DL_THREADS); }
 
-}  // namespace
+// ---- $oshare: Guava's Hashing.murmur3_128() (MurmurHash3_x64_128, seed 0; Murmur3_128HashFunction.java) restated
+__device__ __forceinline__ uint64_t mm3_rotl(uint64_t x, int r) { return (x << r) | (x >> (64 - r)); }
+__device__ __forceinline__ uint64_t mm3_fmix(uint64_t k) {
+    k ^= k >> 33;
+    k *= 0xff51afd7ed558ccdull;
+    k ^= k >> 33;
+    k *= 0xc4ceb9fe1a85ec53ull;
+    k ^= k >> 33;
+    return k;
+}
+constexpr uint64_t MM3_C1 = 0x87c37b91114253d5ull, MM3_C2 = 0x4cf5ad432745937full;
 
-cudaError_t launch_delivery(const DeliveryParams& q, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream) {
-    // item counts as uint32 (pairs and topics are below 2^32): CUB then keeps 32-bit offsets
-    const uint32_t T = (uint32_t) q.f.n_topics, n = (uint32_t) q.f.n_pairs;
+// newHasher().putInt(hash).putString(url, UTF_8).hash().asLong(): h1 over the n = 4 + len bytes LE32(hash) ‖ url. The url sits
+// at byte 4 of the aligned words w[], zero-padded to its last word, so every 16-byte block and the tail are whole word loads.
+__device__ __forceinline__ int64_t rendezvous_score(uint32_t hash, const unsigned long long* w, uint32_t len) {
+    const uint32_t n = len + 4, nb = n >> 4;
+    uint64_t h1 = 0, h2 = 0;
+    for (uint32_t i = 0; i < nb; i++) {
+        uint64_t k1 = __ldg(w + 2 * i), k2 = __ldg(w + 2 * i + 1);
+        if (i == 0) k1 |= hash;
+        k1 *= MM3_C1; k1 = mm3_rotl(k1, 31); k1 *= MM3_C2; h1 ^= k1;
+        h1 = mm3_rotl(h1, 27); h1 += h2; h1 = h1 * 5 + 0x52dce729;
+        k2 *= MM3_C2; k2 = mm3_rotl(k2, 33); k2 *= MM3_C1; h2 ^= k2;
+        h2 = mm3_rotl(h2, 31); h2 += h1; h2 = h2 * 5 + 0x38495ab5;
+    }
+    const uint32_t rem = n & 15;
+    if (rem) {
+        uint64_t k1 = __ldg(w + 2 * nb);
+        if (nb == 0) k1 |= hash;
+        if (rem > 8) {
+            uint64_t k2 = __ldg(w + 2 * nb + 1);
+            k2 *= MM3_C2; k2 = mm3_rotl(k2, 33); k2 *= MM3_C1; h2 ^= k2;
+        }
+        k1 *= MM3_C1; k1 = mm3_rotl(k1, 31); k1 *= MM3_C2; h1 ^= k1;
+    }
+    h1 ^= n;
+    h2 ^= n;
+    h1 += h2;
+    h2 += h1;
+    h1 = mm3_fmix(h1);
+    h2 = mm3_fmix(h2);
+    return (int64_t) (h1 + h2);
+}
+
+// phase 1: d_pub_off must run from 0, never decrease and end at n_pubs (check[2] = 1 otherwise); the scans' last entries
+__global__ void __launch_bounds__(DL_THREADS) oshare_check_kernel(const DeliveryParams q) {
+    const int64_t t = (int64_t) blockIdx.x * DL_THREADS + threadIdx.x;
+    const int64_t T = q.f.n_topics;
+    if (t == 0) {
+        q.o.oflag[q.f.n_pairs] = 0;
+        q.o.oitems[q.f.n_pairs] = 0;
+    }
+    if (t > T) return;
+    const int64_t* po = q.o.pub_off;
+    const bool bad = (t == 0 && po[0] != 0) || (t == T && po[T] != q.o.n_pubs) || (t < T && po[t + 1] < po[t]);
+    if (bad) atomicOr(&q.o.check[2], 1ull);
+}
+
+// phase 1, per CSR pair (the fan-out's walk): an $oshare pair with members in a topic the nesting keeps, and its publishers
+__global__ void __launch_bounds__(FO_THREADS) oshare_flag_kernel(const DeliveryParams q) {
+    constexpr int PER = FO_TILE / FO_THREADS;
+    const int64_t j0 = (int64_t) blockIdx.x * FO_TILE + (int64_t) threadIdx.x * PER;
+    if (j0 >= q.f.n_pairs) return;
+    const bool csr_ok = q.f.offsets[q.f.n_topics] == q.f.n_pairs;   // else nothing is nested (and the walk has no bound)
+    uint32_t t = csr_ok ? fo_topic_of(q.f.offsets, q.f.n_topics, j0) : 0;
+    for (int k = 0; k < PER && j0 + k < q.f.n_pairs; k++) {
+        const int64_t j = j0 + k;
+        uint32_t fl = 0;
+        unsigned long long items = 0;
+        if (csr_ok) {
+            while (q.f.offsets[t + 1] <= j) t++;
+            const int32_t tn = q.topic_tenant[t];
+            const uint32_t d = q.f.rdeliv[q.f.ranks[j]];
+            if (tn >= 0 && tn < q.n_tenants && (d & FO_GROUP_BIT)) {
+                const uint32_t g = d & ~FO_GROUP_BIT;
+                if (q.f.gordered[g] && q.f.gmem_off[g + 1] > q.f.gmem_off[g]) {
+                    fl = 1;
+                    items = (unsigned long long) (q.o.pub_off[t + 1] - q.o.pub_off[t]);
+                }
+            }
+        }
+        q.o.oflag[j] = fl;
+        q.o.oitems[j] = items;
+    }
+}
+
+__global__ void oshare_total_kernel(const DeliveryParams q) {
+    q.o.check[0] = q.o.oflag[q.f.n_pairs];
+    q.o.check[1] = q.o.oitems[q.f.n_pairs];
+    q.o.check[3] = (unsigned long long) q.f.offsets[q.f.n_topics];
+}
+
+// phase 2: the $oshare pairs compacted (scanned oflag), keyed (topic position, rank) so the sort puts each topic's in rank order
+__global__ void __launch_bounds__(FO_THREADS) oshare_compact_kernel(const DeliveryParams q) {
+    constexpr int PER = FO_TILE / FO_THREADS;
+    const int64_t j0 = (int64_t) blockIdx.x * FO_TILE + (int64_t) threadIdx.x * PER;
+    if (j0 >= q.f.n_pairs || q.o.n_opairs == 0) return;
+    uint32_t t = fo_topic_of(q.f.offsets, q.f.n_topics, j0);
+    for (int k = 0; k < PER && j0 + k < q.f.n_pairs; k++) {
+        const int64_t j = j0 + k;
+        const uint32_t o = q.o.oflag[j];
+        if (q.o.oflag[j + 1] == o) continue;
+        while (q.f.offsets[t + 1] <= j) t++;
+        q.o.okey[0][o] = (unsigned long long) t << 32 | (uint32_t) q.f.ranks[j];
+    }
+}
+
+// items per sorted $oshare pair (its topic's publishers), scanned in place into istart[]
+__global__ void __launch_bounds__(DL_THREADS) oshare_items_kernel(const DeliveryParams q) {
+    const int64_t o = (int64_t) blockIdx.x * DL_THREADS + threadIdx.x;
+    if (o > q.o.n_opairs) return;
+    uint32_t c = 0;
+    if (o < q.o.n_opairs) {
+        const uint32_t t = (uint32_t) (q.o.okey[0][o] >> 32);
+        c = (uint32_t) (q.o.pub_off[t + 1] - q.o.pub_off[t]);
+    }
+    q.o.istart[o] = c;
+}
+
+// one warp per item: lanes over the group's members, each keeping its first strictly best score, then a warp argmax that
+// breaks ties by the lower member index -- the reference's "first member with a strictly greater score". Key (pair, winner).
+constexpr int RV_THREADS = 256;
+__global__ void __launch_bounds__(RV_THREADS) oshare_rendezvous_kernel(const DeliveryParams q) {
+    const int64_t item = ((int64_t) blockIdx.x * RV_THREADS + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31u;
+    if (item >= q.o.n_items) return;
+    const uint32_t o = dl_segment_of(q.o.istart, q.o.n_opairs, (uint32_t) item);
+    const unsigned long long ok = q.o.okey[0][o];
+    const uint32_t t = (uint32_t) (ok >> 32), r = (uint32_t) ok;
+    const uint32_t p = (uint32_t) (q.o.pub_off[t] + ((uint32_t) item - q.o.istart[o]));
+    const uint32_t hash = (uint32_t) q.o.pub_hash[p];
+    const uint32_t g = q.f.rdeliv[r] & ~FO_GROUP_BIT;
+    const uint32_t b = q.f.gmem_off[g], n = q.f.gmem_off[g + 1] - b;
+    int64_t best = INT64_MIN;
+    uint32_t bm = 0xFFFFFFFFu;
+    for (uint32_t m = lane; m < n; m += 32) {
+        const int64_t sc = rendezvous_score(hash, q.o.url_words + q.o.url_word[b + m], q.o.url_len[b + m]);
+        if (sc > best) {
+            best = sc;
+            bm = m;
+        }
+    }
+    for (int off = 16; off > 0; off >>= 1) {
+        const int64_t ob = __shfl_xor_sync(0xFFFFFFFFu, best, off);
+        const uint32_t om = __shfl_xor_sync(0xFFFFFFFFu, bm, off);
+        if (ob > best || (ob == best && om < bm)) {
+            best = ob;
+            bm = om;
+        }
+    }
+    if (lane == 0) {
+        q.o.ikey[0][item] = (unsigned long long) o << q.o.member_bits | (bm == 0xFFFFFFFFu ? n : bm);
+        q.o.ival[0][item] = p;
+    }
+}
+
+// sorted items: 1 where (pair, winner) changes (exclusive scan: an item's heads before it), [n_items] = 0
+__global__ void __launch_bounds__(DL_THREADS) oshare_heads_kernel(const DeliveryParams q) {
+    const int64_t x = (int64_t) blockIdx.x * DL_THREADS + threadIdx.x;
+    if (x > q.o.n_items) return;
+    const unsigned long long* ikey = q.o.ikey[0];
+    q.o.ihead[x] = x < q.o.n_items && (x == 0 || ikey[x] != ikey[x - 1]);
+}
+
+// sub-pack s starts at its head item; sub_start[n_subs] = n_items
+__global__ void __launch_bounds__(DL_THREADS) oshare_subs_kernel(const DeliveryParams q) {
+    const int64_t x = (int64_t) blockIdx.x * DL_THREADS + threadIdx.x;
+    if (x == 0) q.o.sub_start[q.o.ihead[q.o.n_items]] = (uint32_t) q.o.n_items;
+    if (x < q.o.n_items && q.o.ihead[x + 1] != q.o.ihead[x]) q.o.sub_start[q.o.ihead[x]] = (uint32_t) x;
+}
+
+// every item's publisher into its sub-pack's pack: pack_pub[pack_pub_off[pack] + its place in the sub-pack]
+__global__ void __launch_bounds__(DL_THREADS) oshare_pubs_kernel(const DeliveryParams q, const uint32_t* ival) {
+    const int64_t x = (int64_t) blockIdx.x * DL_THREADS + threadIdx.x;
+    if (x >= q.o.n_items) return;
+    const uint32_t s = q.o.ihead[x + 1] - 1;
+    q.o.pack_pub[q.o.pack_pub_off[q.o.sub_pack[s]] + ((uint32_t) x - q.o.sub_start[s])] = ival[x];
+}
+
+template <bool OSH>
+cudaError_t run_delivery(const DeliveryParams& q0, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream) {
+    DeliveryParams q = q0;   // OSH: okey[0] / ikey[0] are re-pointed at the sorted buffers
+    // item counts as uint32 (emit positions and topics are below 2^32): CUB then keeps 32-bit offsets
+    const uint32_t T = (uint32_t) q.f.n_topics, n = (uint32_t) dl_emit_cap<OSH>(q);
     const uint32_t D = q.f.n_deliverers;
     const int tbits = (int) bits_for((uint32_t) q.n_tenants), dbits = (int) bits_for(D);
     cub::DoubleBuffer<uint32_t> tk(q.tkey[0], q.tkey[1]), tv(q.tval[0], q.tval[1]);
     cub::DoubleBuffer<uint32_t> dk(q.key[0], q.key[1]), dv(q.val[0], q.val[1]);
+    // $oshare: pairs sorted on (topic position, rank), items on (pair, winner)
+    const uint32_t O = OSH ? (uint32_t) q.o.n_opairs : 0, I = OSH ? (uint32_t) q.o.n_items : 0;
+    const int okbits = 32 + (int) bits_for(T), ikbits = OSH ? (int) (q.o.member_bits + bits_for(O)) : 0;
+    cub::DoubleBuffer<unsigned long long> ok(q.o.okey[0], q.o.okey[1]), ik(q.o.ikey[0], q.o.ikey[1]);
+    cub::DoubleBuffer<uint32_t> iv(q.o.ival[0], q.o.ival[1]);
     if (!d_tmp) {
-        size_t a = 0, b = 0, c = 0, d = 0, e = 0;
+        size_t a = 0, b = 0, c = 0, d = 0, e = 0, f = 0, g = 0, h = 0, k = 0;
         cudaError_t err = cub::DeviceRadixSort::SortPairs(nullptr, a, tk, tv, T, 0, tbits, stream);
         if (err == cudaSuccess) err = cub::DeviceScan::ExclusiveSum(nullptr, b, q.tcount, q.tstart, T + 1, stream);
         if (err == cudaSuccess) err = cub::DeviceRadixSort::SortPairs(nullptr, c, dk, dv, n, 0, dbits, stream);
         if (err == cudaSuccess) err = cub::DeviceScan::ExclusiveSum(nullptr, d, q.pack_head, n + 1, stream);
         if (err == cudaSuccess) err = cub::DeviceScan::ExclusiveSum(nullptr, e, q.pcount, q.package_off, D + 1, stream);
-        *tmp_bytes = std::max({a, b, c, d, e});
+        if constexpr (OSH) {
+            if (err == cudaSuccess) err = cub::DeviceRadixSort::SortKeys(nullptr, f, ok, O, 0, okbits, stream);
+            if (err == cudaSuccess) err = cub::DeviceScan::ExclusiveSum(nullptr, g, q.o.istart, O + 1, stream);
+            if (err == cudaSuccess) err = cub::DeviceRadixSort::SortPairs(nullptr, h, ik, iv, I, 0, ikbits, stream);
+            if (err == cudaSuccess) err = cub::DeviceScan::ExclusiveSum(nullptr, k, q.o.pub_count, q.o.pack_pub_off, n + 1, stream);
+            g = std::max(g, k);
+        }
+        *tmp_bytes = std::max({a, b, c, d, e, f, g, h});
         return err;
     }
     size_t bytes = *tmp_bytes;
@@ -351,20 +623,73 @@ cudaError_t launch_delivery(const DeliveryParams& q, void* d_tmp, size_t* tmp_by
     if (err != cudaSuccess) return err;
     delivery_topic_keys_kernel<<<dl_blocks(T), DL_THREADS, 0, stream>>>(q);
     if ((err = cub::DeviceRadixSort::SortPairs(d_tmp, bytes, tk, tv, T, 0, tbits, stream)) != cudaSuccess) return err;
-    delivery_topic_counts_kernel<<<dl_blocks(T + 1), DL_THREADS, 0, stream>>>(q, tk.Current(), tv.Current());
+    if constexpr (OSH) {
+        if ((err = cudaMemsetAsync(q.o.pub_count, 0, ((size_t) n + 1) * sizeof(uint32_t), stream)) != cudaSuccess) return err;
+        oshare_compact_kernel<<<fo_tiles(q.f.n_pairs), FO_THREADS, 0, stream>>>(q);
+        bytes = *tmp_bytes;
+        if ((err = cub::DeviceRadixSort::SortKeys(d_tmp, bytes, ok, O, 0, okbits, stream)) != cudaSuccess) return err;
+        q.o.okey[0] = ok.Current();
+        oshare_items_kernel<<<dl_blocks(O + 1), DL_THREADS, 0, stream>>>(q);
+        bytes = *tmp_bytes;
+        if ((err = cub::DeviceScan::ExclusiveSum(d_tmp, bytes, q.o.istart, O + 1, stream)) != cudaSuccess) return err;
+        if (I > 0) {
+            const unsigned warps_per_block = RV_THREADS / 32;
+            oshare_rendezvous_kernel<<<(unsigned) ((I + warps_per_block - 1) / warps_per_block), RV_THREADS, 0, stream>>>(q);
+        }
+        bytes = *tmp_bytes;
+        if ((err = cub::DeviceRadixSort::SortPairs(d_tmp, bytes, ik, iv, I, 0, ikbits, stream)) != cudaSuccess) return err;
+        q.o.ikey[0] = ik.Current();
+        oshare_heads_kernel<<<dl_blocks(I + 1), DL_THREADS, 0, stream>>>(q);
+        bytes = *tmp_bytes;
+        if ((err = cub::DeviceScan::ExclusiveSum(d_tmp, bytes, q.o.ihead, I + 1, stream)) != cudaSuccess) return err;
+        oshare_subs_kernel<<<dl_blocks(I), DL_THREADS, 0, stream>>>(q);
+    }
+    delivery_topic_counts_kernel<OSH><<<dl_blocks(T + 1), DL_THREADS, 0, stream>>>(q, tk.Current(), tv.Current());
     bytes = *tmp_bytes;
     if ((err = cub::DeviceScan::ExclusiveSum(d_tmp, bytes, q.tcount, q.tstart, T + 1, stream)) != cudaSuccess) return err;
-    delivery_emit_kernel<<<fo_tiles(n), FO_THREADS, 0, stream>>>(q, tv.Current());
+    delivery_emit_kernel<OSH><<<fo_tiles(n), FO_THREADS, 0, stream>>>(q, tv.Current());
     bytes = *tmp_bytes;
     if ((err = cub::DeviceRadixSort::SortPairs(d_tmp, bytes, dk, dv, n, 0, dbits, stream)) != cudaSuccess) return err;
-    delivery_gather_kernel<<<dl_blocks(n + 1), DL_THREADS, 0, stream>>>(q, dk.Current(), dv.Current(), tk.Current());
+    delivery_gather_kernel<OSH><<<dl_blocks(n + 1), DL_THREADS, 0, stream>>>(q, dk.Current(), dv.Current(), tk.Current());
     bytes = *tmp_bytes;
     if ((err = cub::DeviceScan::ExclusiveSum(d_tmp, bytes, q.package_head, n + 1, stream)) != cudaSuccess) return err;
     bytes = *tmp_bytes;
     if ((err = cub::DeviceScan::ExclusiveSum(d_tmp, bytes, q.pack_head, n + 1, stream)) != cudaSuccess) return err;
-    delivery_scatter_kernel<<<dl_blocks(n), DL_THREADS, 0, stream>>>(q, dk.Current(), tk.Current(), tv.Current());
+    delivery_scatter_kernel<OSH><<<dl_blocks(n), DL_THREADS, 0, stream>>>(q, dk.Current(), tk.Current(), tv.Current());
+    if constexpr (OSH) {
+        bytes = *tmp_bytes;
+        if ((err = cub::DeviceScan::ExclusiveSum(d_tmp, bytes, q.o.pub_count, q.o.pack_pub_off, n + 1, stream)) != cudaSuccess) return err;
+        oshare_pubs_kernel<<<dl_blocks(I), DL_THREADS, 0, stream>>>(q, iv.Current());
+    }
     bytes = *tmp_bytes;
     if ((err = cub::DeviceScan::ExclusiveSum(d_tmp, bytes, q.pcount, q.package_off, D + 1, stream)) != cudaSuccess) return err;
+    return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t launch_delivery(const DeliveryParams& q, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream) {
+    return q.oshare ? run_delivery<true>(q, d_tmp, tmp_bytes, stream) : run_delivery<false>(q, d_tmp, tmp_bytes, stream);
+}
+
+cudaError_t launch_oshare_count(const DeliveryParams& q, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream) {
+    const uint32_t n = (uint32_t) q.f.n_pairs;
+    if (!d_tmp) {
+        size_t a = 0, b = 0;
+        cudaError_t err = cub::DeviceScan::ExclusiveSum(nullptr, a, q.o.oflag, n + 1, stream);
+        if (err == cudaSuccess) err = cub::DeviceScan::ExclusiveSum(nullptr, b, q.o.oitems, n + 1, stream);
+        *tmp_bytes = std::max(a, b);
+        return err;
+    }
+    cudaError_t err = cudaMemsetAsync(q.o.check, 0, 4 * sizeof(unsigned long long), stream);
+    if (err != cudaSuccess) return err;
+    oshare_check_kernel<<<dl_blocks(q.f.n_topics + 1), DL_THREADS, 0, stream>>>(q);
+    oshare_flag_kernel<<<fo_tiles(n), FO_THREADS, 0, stream>>>(q);
+    size_t bytes = *tmp_bytes;
+    if ((err = cub::DeviceScan::ExclusiveSum(d_tmp, bytes, q.o.oflag, n + 1, stream)) != cudaSuccess) return err;
+    bytes = *tmp_bytes;
+    if ((err = cub::DeviceScan::ExclusiveSum(d_tmp, bytes, q.o.oitems, n + 1, stream)) != cudaSuccess) return err;
+    oshare_total_kernel<<<1, 1, 0, stream>>>(q);
     return cudaGetLastError();
 }
 
@@ -454,6 +779,8 @@ bool build_tenant_fan(const KVBlob& kv, DelivererTable* table, TenantFan* out, s
     out->gmem_off.assign(1, 0);
     out->gmem_deliv.clear();
     out->gordered.clear();
+    out->ourl_off.assign(1, 0);
+    out->ourl.clear();
     for (int64_t r = 0; r < n; r++) {
         DecodedKey d;
         if (!decode_route_key(kv.key(r), &d)) {
@@ -471,7 +798,8 @@ bool build_tenant_fan(const KVBlob& kv, DelivererTable* table, TenantFan* out, s
             continue;
         }
         out->rdeliv[(size_t) r] = FO_GROUP_BIT | (uint32_t) out->gordered.size();
-        out->gordered.push_back(d.flag == FLAG_ORDERED ? 1 : 0);
+        const bool ordered = d.flag == FLAG_ORDERED;
+        out->gordered.push_back(ordered ? 1 : 0);
         bool ok = true;
         const bool parsed = for_each_group_member(kv.val(r), [&](sv url) {
             int32_t broker = 0;
@@ -481,6 +809,8 @@ bool build_tenant_fan(const KVBlob& kv, DelivererTable* table, TenantFan* out, s
                 return;
             }
             out->gmem_deliv.push_back(table->intern(broker, dk));
+            if (ordered) out->ourl.append(url);
+            out->ourl_off.push_back((uint32_t) out->ourl.size());
         });
         if (!parsed || !ok) {
             if (err) *err = "undecodable RouteGroup value";

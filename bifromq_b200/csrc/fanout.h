@@ -44,6 +44,41 @@ size_t fanout_scratch_words(uint32_t n_deliverers, int64_t n_pairs, bool tiled);
 // d_tmp == nullptr: query the scan scratch size
 cudaError_t launch_fanout(const FanoutParams& p, bool tiled, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream);
 
+// The ordered shared subscriptions of a delivery nesting resolved per publisher (RendezvousHash over each member's
+// receiverUrl). An "item" is one ($oshare pair, publisher); a "sub-pack" the publishers of one pair that picked the same member.
+// Pair arrays below are sized for the pairs AND the sub-packs: the nesting then holds emit_cap = n_pairs + n_items slots.
+struct OshareParams {
+    // inputs
+    const int64_t* pub_off;          // [n_topics + 1] publishers of topic position t: pub_hash[pub_off[t] .. pub_off[t + 1])
+    const int32_t* pub_hash;         // [n_pubs] ClientInfo.hashCode() of each publisher
+    int64_t n_pubs;
+    // per-snapshot member receiverUrls: member m's bytes sit at byte 4 of the 8-byte words from url_word[m] on, zero before and
+    // after, so LE32(hash) ‖ url is read as whole aligned words (bfq_delivery_device_ordered builds them on first use)
+    const unsigned long long* url_words;
+    const long long* url_word;       // [n_members]
+    const uint32_t* url_len;         // [n_members]
+    uint32_t member_bits;            // bits_for(largest $oshare group): a pick, or the group size for "no winner", fits
+    // phase 1 (sized by the host): flags and item counts per CSR pair, their scans, the pub_off check
+    uint32_t* oflag;                 // [n_pairs + 1] 1 = an $oshare pair with members in a nested topic; scanned in place
+    unsigned long long* oitems;      // [n_pairs + 1] its publishers; scanned in place
+    unsigned long long* check;       // [4]: opairs, items, bad pub_off, offsets[n_topics] (written by launch_oshare_count)
+    // phase 2 (sized by the host after reading check[]): n_opairs and n_items known
+    int64_t n_opairs, n_items;
+    unsigned long long* okey[2];     // [n_opairs] each: (topic position << 32 | rank), sorted
+    uint32_t* istart;                // [n_opairs + 1] first item of every sorted $oshare pair
+    unsigned long long* ikey[2];     // [n_items] each: (sorted pair << member_bits | pick), sorted (stable: publishers in order)
+    uint32_t* ival[2];               // [n_items] each: ... and the publisher position
+    uint32_t* ihead;                 // [n_items + 1] 1 where (pair, pick) changes, scanned in place: the item's sub-pack
+    uint32_t* sub_start;             // [n_items + 1] first item of every sub-pack ([n_subs] = n_items)
+    uint32_t* sub_pack;              // [n_items] the pack each sub-pack became
+    uint32_t* e_sub;                 // [emit_cap] per emit position: its sub-pack or 0xFFFFFFFF
+    uint32_t* s_sub;                 // [emit_cap] per nested pair: ditto
+    uint32_t* pub_count;             // [emit_cap + 1] publishers per pack (0 for a whole pack), scanned into pack_pub_off
+    // outputs
+    long long* pack_pub_off;         // [emit_cap + 1] (n_packs + 1 used)
+    uint32_t* pack_pub;              // [n_items]
+};
+
 // The same pairs nested the way the deliverer's batcher sends them: deliverer -> package (tenant) -> pack (topic position)
 // -> MatchInfos. Deliverer ids and member picks are the fan-out's (the same device function resolves both).
 struct DeliveryParams {
@@ -55,6 +90,7 @@ struct DeliveryParams {
     uint32_t* tval[2];               // [n_topics] each: ... and topic positions
     uint32_t* tcount;                // [n_topics + 1] pairs per topic in tenant-major order
     uint32_t* tstart;                // [n_topics + 1] their exclusive scan: [n_topics] = pairs nested
+    // the [n_pairs] arrays below are [n_pairs + o.n_items] with oshare (the sub-packs' emit positions)
     uint32_t* key[2];                // [n_pairs] each: the deliverer partition's keys (double buffer)
     uint32_t* val[2];                // [n_pairs] each: ... and emit positions
     uint32_t* e_topic;               // [n_pairs] per emit position: tenant-major topic index, rank, member
@@ -64,7 +100,7 @@ struct DeliveryParams {
     uint32_t* package_head;          // [n_pairs + 1] 1 where (deliverer, tenant) changes, scanned in place (exclusive)
     uint32_t* pack_head;             // [n_pairs + 1] 1 where (deliverer, topic) changes, scanned in place (exclusive)
     uint32_t* pcount;                // [n_deliverers + 1] packages per deliverer
-    unsigned long long* totals;      // [4] pairs nested, packages, packs, offsets[n_topics]
+    unsigned long long* totals;      // [4] pairs nested, packages, packs, offsets[n_topics] (+ [4] sub-packs with oshare)
     // outputs
     long long* package_off;          // [n_deliverers + 1]
     uint32_t* package_tenant;        // [n_pairs] (n_packages used)
@@ -73,9 +109,17 @@ struct DeliveryParams {
     long long* match_off;            // [n_pairs + 1] (n_packs + 1 used)
     uint32_t* match_rank;            // [n_pairs]
     uint32_t* match_member;          // [n_pairs]
+    // $oshare resolution (bfq_delivery_device_ordered); oshare == false: $oshare pairs stay under the ordered-share id
+    bool oshare;
+    OshareParams o;
 };
-// d_tmp == nullptr: query the scratch size of the sorts and scans. Enqueues everything on `stream`; totals[] is written last.
+
+// d_tmp == nullptr: query the scratch size of the sorts and scans. Enqueues everything on `stream`; totals[] is written last
+// (with q.oshare: [4] = sub-packs).
 cudaError_t launch_delivery(const DeliveryParams& q, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream);
+// Phase 1 of the $oshare resolution: flags, item counts and the pub_off check into o.check[] (the host reads them to size
+// phase 2, which is launch_delivery with q.oshare set). d_tmp == nullptr: query the scan scratch size.
+cudaError_t launch_oshare_count(const DeliveryParams& q, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream);
 
 // (subBrokerId, delivererKey) -> dense id, append-only and shared by every snapshot of an index (ids stay valid across commits
 // and resets, and are never freed)
@@ -92,6 +136,10 @@ struct TenantFan {
     std::vector<uint32_t> gmem_off;      // tenant-local
     std::vector<uint32_t> gmem_deliv;
     std::vector<uint8_t> gordered;
+    // receiverUrl of every member of an ordered group (empty for the members of other groups): member m is
+    // ourl[ourl_off[m] .. ourl_off[m + 1]); the $oshare pick hashes it
+    std::vector<uint32_t> ourl_off;
+    std::string ourl;
 };
 bool build_tenant_fan(const KVBlob& kv, DelivererTable* table, TenantFan* out, std::string* err);
 

@@ -120,18 +120,21 @@ class BatchResult:
 
 
 class DeliveryResult:
-    """One bfq_delivery_device result: the raw struct's fields (d_package_off, n_packs, ordered_share_id, ...) plus nesting()."""
+    """One bfq_delivery_device result: the raw struct's fields (d_package_off, n_packs, ordered_share_id, ...) plus nesting().
+    A bfq_delivery_device_ordered result also carries each pack's publisher positions (`ordered` is its full struct)."""
 
-    def __init__(self, raw):
+    def __init__(self, raw, ordered=None):
         self.raw = raw
+        self.ordered = ordered
 
     def __getattr__(self, name):
-        if name == "raw":
+        if name in ("raw", "ordered"):
             raise AttributeError(name)
         return getattr(self.raw, name)
 
     def arrays(self, device=None):
-        """the seven arrays copied to the host (numpy), after a device synchronise"""
+        """the seven arrays copied to the host (numpy), after a device synchronise; an ordered result adds pack_pub_off and
+        pack_pub"""
         import torch
 
         from .dist import device_view
@@ -140,17 +143,23 @@ class DeliveryResult:
 
         def get(p, n, t):
             return device_view(p, max(n, 1), t, device).cpu().numpy()[:n].astype(np.int64)
-        return {"package_off": get(r.d_package_off, r.n_deliverers + 1, "<i8"),
-                "package_tenant": get(r.d_package_tenant, r.n_packages, "<u4"),
-                "pack_off": get(r.d_pack_off, r.n_packages + 1, "<i8"),
-                "pack_topic": get(r.d_pack_topic, r.n_packs, "<u4"),
-                "match_off": get(r.d_match_off, r.n_packs + 1, "<i8"),
-                "match_rank": get(r.d_match_rank, r.n_pairs, "<u4"),
-                "match_member": get(r.d_match_member, r.n_pairs, "<u4")}
+        a = {"package_off": get(r.d_package_off, r.n_deliverers + 1, "<i8"),
+             "package_tenant": get(r.d_package_tenant, r.n_packages, "<u4"),
+             "pack_off": get(r.d_pack_off, r.n_packages + 1, "<i8"),
+             "pack_topic": get(r.d_pack_topic, r.n_packs, "<u4"),
+             "match_off": get(r.d_match_off, r.n_packs + 1, "<i8"),
+             "match_rank": get(r.d_match_rank, r.n_pairs, "<u4"),
+             "match_member": get(r.d_match_member, r.n_pairs, "<u4")}
+        if self.ordered is not None:
+            a["pack_pub_off"] = get(self.ordered.d_pack_pub_off, r.n_packs + 1, "<i8")
+            a["pack_pub"] = get(self.ordered.d_pack_pub, self.ordered.n_pack_pubs, "<u4")
+        return a
 
     def nesting(self, device=None):
         """{deliverer id: {tenant index: [(topic position, {(rank, member), ...}), ...]}}: deliverers without pairs are left
-        out, packages in ascending tenant order, packs in their order. For tests and small batches: the walk is on the host."""
+        out, packages in ascending tenant order, packs in their order. An ordered result's packs are
+        (topic position, {(rank, member)}, (publisher position, ...)), the tuple empty for a whole TopicMessagePack.
+        For tests and small batches: the walk is on the host."""
         a = self.arrays(device)
         out = {}
         for d in range(self.raw.n_deliverers):
@@ -162,8 +171,10 @@ class DeliveryResult:
                 packs = pkgs[int(a["package_tenant"][p])] = []
                 for k in range(int(a["pack_off"][p]), int(a["pack_off"][p + 1])):
                     m0, m1 = int(a["match_off"][k]), int(a["match_off"][k + 1])
-                    packs.append((int(a["pack_topic"][k]),
-                                  set(zip(a["match_rank"][m0:m1].tolist(), a["match_member"][m0:m1].tolist()))))
+                    pack = (int(a["pack_topic"][k]), set(zip(a["match_rank"][m0:m1].tolist(), a["match_member"][m0:m1].tolist())))
+                    if self.ordered is not None:
+                        pack += (tuple(a["pack_pub"][int(a["pack_pub_off"][k]):int(a["pack_pub_off"][k + 1])].tolist()),)
+                    packs.append(pack)
         return out
 
 
@@ -216,6 +227,16 @@ class DeviceResult:
         N.check(N.lib.bfq_delivery_device(C.byref(self.raw), d_offsets_ptr, d_ranks_ptr, n_pairs, d_topic_tenant_ptr, stream,
                                           C.byref(out)))
         return DeliveryResult(out)
+
+    def delivery_ordered(self, d_offsets_ptr, d_ranks_ptr, n_pairs, d_topic_tenant_ptr, d_pub_off_ptr, d_pub_hash_ptr, n_pubs,
+                         stream=0):
+        """bfq_delivery_device_ordered: delivery() with every $oshare pair resolved per publisher. d_pub_off_ptr: int64
+        [n_topics + 1] publisher packs per topic position, d_pub_hash_ptr: int32 [n_pubs] each publisher's
+        ClientInfo.hashCode() (device). -> DeliveryResult whose nesting() also gives each pack's publisher positions"""
+        out = N.BfqDeliveryOrderedResult()
+        N.check(N.lib.bfq_delivery_device_ordered(C.byref(self.raw), d_offsets_ptr, d_ranks_ptr, n_pairs, d_topic_tenant_ptr,
+                                                  d_pub_off_ptr, d_pub_hash_ptr, n_pubs, stream, C.byref(out)))
+        return DeliveryResult(out.d, out)
 
     def release(self):
         if getattr(self, "raw", None) is not None and self.raw.lease:

@@ -207,7 +207,7 @@ void bfq_result_free(bfq_result* r);
  * whatever else runs on the handle. Several matches may be in flight on one handle (and one stream) at a time.
  *   bfq_device_result_release  blocks until the match and everything the library enqueued for the result since
  *                           (bfq_expand_device, bfq_expand_device_budget, bfq_fanout_device, bfq_delivery_device,
- *                           bfq_exchange_gather), on every stream it was used on, has finished; then the workspace goes back
+ *                           bfq_delivery_device_ordered, bfq_exchange_gather), on every stream it was used on, has finished; then the workspace goes back
  *                           to the handle's pool, where the next match may take it. The caller's own work that reads the
  *                           result's arrays (or the CSR and fan-out arrays that live in its workspace) must be ordered
  *                           before the release by the caller. */
@@ -389,6 +389,58 @@ typedef struct {
 } bfq_delivery_result;
 int32_t bfq_delivery_device(const bfq_device_result* res, const int64_t* d_offsets, const int64_t* d_ranks, int64_t n_pairs,
                             const int32_t* d_topic_tenant, void* stream, bfq_delivery_result* out);
+
+/* ------------------------------------------------------------------------------------------------
+ * Ordered shared subscriptions ($oshare) resolved in the delivery nesting. The ordered branch of DeliverExecutorGroup.send
+ * (DW/DeliverExecutorGroup.java:242-278) sends, for every publisher pack of the topic's TopicMessagePack, to ONE member of the
+ * group: RendezvousHash.get (base-util/.../RendezvousHash.java) scores member m as
+ *   Hashing.murmur3_128() (seed 0).newHasher().putInt(publisher.hashCode()).putString(receiverUrl_m, UTF_8).hash().asLong()
+ * i.e. h1 of MurmurHash3_x64_128 over LE32(hash) ‖ utf8(receiverUrl), as a signed 64-bit value, and picks the first member
+ * (in the stored RouteGroup's wire order, the fan-out's member order) whose score is strictly greater than every earlier one
+ * (the running best starts at Long.MIN_VALUE). Publishers with the same winner form one new TopicMessagePack (the topic, those
+ * publisher packs in their original order), sent to the winner's deliverer with the winner's MatchInfo in a fresh
+ * TopicMessagePackHolder; BatchDeliveryCall keys packs by holder identity, so every such sub-pack is a DeliveryPack of its own
+ * with exactly one MatchInfo, even when two $oshare routes of a topic pick members on one deliverer.
+ * bfq_delivery_device_ordered is bfq_delivery_device plus that pick. Per topic position t the host passes its publisher packs:
+ * d_pub_off[n_topics + 1] (device, from 0 to n_pubs, never decreasing) and d_pub_hash[n_pubs] (device,
+ * publisherPack.getPublisher().hashCode(): a protobuf object hash, which native code cannot recompute). Repeated topic
+ * positions carry their own publishers.
+ *   d                       the nesting of bfq_delivery_device (same deliverer ids, tenants, pack order and $share picks), with
+ *                           every $oshare pair whose group has members replaced by its sub-packs: a sub-pack's MatchInfo is
+ *                           (rank, winning member index). Only member-less groups stay under d.ordered_share_id (the reference
+ *                           would fail on them), and so would a publisher for which every member scores exactly
+ *                           Long.MIN_VALUE (the reference finds no winner: member 0xFFFFFFFF). A topic position with no
+ *                           publisher packs gives no sub-pack for its $oshare routes; its other routes still get the whole pack.
+ *                           d.n_pairs counts the MatchInfos nested. Within a package a topic position's whole pack comes first,
+ *                           then its sub-packs ordered by (rank, member).
+ *   d_pack_pub_off          [d.n_packs + 1]: pack k's publishers are d_pack_pub[d_pack_pub_off[k] .. d_pack_pub_off[k + 1]). An
+ *                           empty span is the whole TopicMessagePack of d_pack_topic[k]; a non-empty span is an $oshare sub-pack.
+ *   d_pack_pub              publisher positions (indices into d_pub_hash), ascending within a pack; n_pack_pubs of them
+ *   n_ordered_packs         the sub-packs (packs with a non-empty span)
+ * The pick is stateless: it scores the members of the result's own snapshot. The reference caches it per (tenantId,
+ * mqttTopicFilter, ClientInfo) but drops that cache on every add or remove of the ordered filter's routes
+ * (DistWorkerCoProc.mutate -> refreshOrderedShareSubRoutes), so a pick over the snapshot's members is the same answer.
+ * The first call on a snapshot uploads its ordered groups' member receiverUrls; bfq_fanout_device and bfq_delivery_device never
+ * need them. The arrays live in the result's leased workspace until bfq_device_result_release and share buffers with
+ * bfq_delivery_device: a later call of either on the same result overwrites the earlier one's arrays. The call synchronises
+ * `stream` twice (to size the (pair, publisher) items, and to read the totals).
+ * Errors: BFQ_E_INVALID for a NULL array the call needs, an n_pairs that disagrees with d_offsets[n_topics], or a d_pub_off
+ * that does not run from 0 to n_pubs without decreasing (both checked on the device: nothing is nested), or a receiver url
+ * without a delivererKey; BFQ_E_RANGE for 2^32 or more pairs plus ($oshare pair, publisher) items; BFQ_E_STATE for a match that
+ * has not completed.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+    bfq_delivery_result d;          /* as bfq_delivery_device, with $oshare pairs resolved: only member-less groups stay
+                                       under d.ordered_share_id; d.n_pairs counts the MatchInfos nested */
+    const int64_t* d_pack_pub_off;  /* [d.n_packs + 1]: an empty span = the whole TopicMessagePack of d_pack_topic[k];
+                                       a non-empty span = an $oshare sub-pack made of these publisher packs */
+    const uint32_t* d_pack_pub;     /* publisher positions (indices into d_pub_hash), ascending within a pack */
+    int64_t n_pack_pubs, n_ordered_packs;
+} bfq_delivery_ordered_result;
+int32_t bfq_delivery_device_ordered(const bfq_device_result* res, const int64_t* d_offsets, const int64_t* d_ranks,
+                                    int64_t n_pairs, const int32_t* d_topic_tenant, const int64_t* d_pub_off,
+                                    const int32_t* d_pub_hash, int64_t n_pubs, void* stream,
+                                    bfq_delivery_ordered_result* out);
 
 /* ------------------------------------------------------------------------------------------------
  * Multi-GPU: the one exchange step of the tenant-sharded path (SURVEY.md 8e). Tenants are independent key ranges, so
