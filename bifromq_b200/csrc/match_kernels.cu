@@ -279,7 +279,8 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32) match_topics_kernel(const 
 //   * per step a lane reads the 28 bytes at its current level start (up to three aligned 16-byte granules, word select +
 //     funnel shift), finds the '/' with a SWAR zero-byte test — the level table is filled lazily, there is no tokenising
 //     pre-pass —, issues the exact-child slot read (4 x LDG.128) and the '+' child payload read (2 x LDG.128) together and
-//     writes the discovered ranges straight to the topic's INLINE_RANGES inline slots: no staging, no output atomics;
+//     writes the discovered ranges straight to the INLINE_RANGES inline slots of the topic's position in the work order:
+//     no staging, no output atomics;
 //   * a lane that finishes takes the next topic at once (warp-uniform refill from 32-topic chunks claimed with
 //     one atomicAdd per chunk), so a straggler never idles the other 31 lanes (a warp that waits for its whole batch of 32
 //     runs with a third of its lanes active);
@@ -449,7 +450,10 @@ __global__ void __launch_bounds__(L_WARPS * 32) match_topics_lane_kernel(const M
                     tenant = ws.m_tenant[i];
                     const int root_ord = ws.m_root[i];
                     n_rg = 0; acc_r = 0; acc_p = 0; acc_g = 0; pending = 0;
-                    rg_out = p.ranges + (uint64_t) t * INLINE_RANGES;
+                    // the inline slots of the topic's POSITION in the work order (idx), not of its topic index t: a warp's topics come
+                    // from the chunks it claimed, so its range writes stay in a few KB of the array instead of scattering over all
+                    // of it (in locality order t is effectively random over an array larger than L2)
+                    rg_out = p.ranges + (uint64_t) idx * INLINE_RANGES;
                     bad = len > 65535;
                     have = true;
                     ws.lv[0][lane] = 0;

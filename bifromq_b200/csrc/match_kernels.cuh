@@ -197,7 +197,7 @@ void launch_match_lanes(const MatchParams& p, cudaStream_t stream);
 void launch_match(const MatchParams& p, bool tier2, int n_warps_tier2, cudaStream_t stream);
 void launch_caps(const CapsParams& p, cudaStream_t stream);
 
-constexpr uint32_t INLINE_RANGES = 12;   // tier 0 writes topic t's ranges at ranges[t * INLINE_RANGES ...)
+constexpr uint32_t INLINE_RANGES = 12;   // tier 0 writes the ranges of the topic at work-order position i at ranges[i * INLINE_RANGES ...)
 constexpr uint32_t SPILL_RANGES = 64;    // ... and moves a topic with more of them, once, to a block of this many ranges
 
 // Compaction for the host path: gathers the sparse (inline + dynamic) ranges into one dense array in topic order.
