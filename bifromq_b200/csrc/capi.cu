@@ -112,6 +112,7 @@ struct Workspace {
     DeviceBuf<uint32_t> d_cnt, d_new_begin, d_final_begin, d_final_count;
     // locality order + dedup (launch_order): per compute-stream slot (two sub-batches can be in flight)
     DeviceBuf<uint32_t> d_ord_keys, d_leader, d_order;
+    DeviceBuf<SpanRecord> d_pos_rec;            // tier 0's span record per work-order position (MatchParams::pos_rec)
     DeviceBuf<unsigned long long> d_hash_tab;   // 2 x hash_stride
     DeviceBuf<uint32_t> d_hist;                 // 2 x hist_stride (launch_order's scratch)
     size_t hash_stride = 0, hist_stride = 0;
@@ -358,6 +359,7 @@ int32_t prepare_workspace(bfq_index* h, Workspace* w, int64_t n, int n_chunks, i
         BFQ_CUDA_TRY(w->d_ord_keys.reserve(nn));
         BFQ_CUDA_TRY(w->d_leader.reserve(nn));
         BFQ_CUDA_TRY(w->d_order.reserve(nn));
+        BFQ_CUDA_TRY(w->d_pos_rec.reserve(nn));
         const size_t hist_stride = order_scratch_words(per_chunk, n_tenants);
         const size_t hash_stride = order_hash_entries(per_chunk);
         if (hist_stride > w->hist_stride) {
@@ -447,12 +449,13 @@ CapsParams caps_params(const CoreCtx& c, const SubBatch& sb, const MatchParams& 
 }
 
 bool wants_order(const CoreCtx& c, const SubBatch& sb) {
-    return sb.n >= c.h->order_min && c.w->d_order.cap >= (size_t) (sb.begin + sb.n) && c.w->hist_stride > 0 &&
+    return sb.n >= c.h->order_min && c.w->d_order.cap >= (size_t) (sb.begin + sb.n) &&
+           c.w->d_pos_rec.cap >= (size_t) (sb.begin + sb.n) && c.w->hist_stride > 0 &&
            c.w->hist_stride >= order_scratch_words(sb.n, c.n_tenants) && c.w->hash_stride >= order_hash_entries(sb.n);
 }
 
-// Enqueues one sub-batch on c.stream WITHOUT synchronising: [dedup + locality order] -> tier 0 -> tier 1 -> [followers] ->
-// [caps], every count read on the device. The host looks at the counters only in finish_core.
+// Enqueues one sub-batch on c.stream WITHOUT synchronising: [dedup + locality order] -> tier 0 -> tier 1 -> [span records
+// to topic order, followers] -> [caps], every count read on the device. The host looks at the counters only in finish_core.
 int32_t enqueue_core(const CoreCtx& c, const SubBatch& sb, CoreOut* out) {
     Workspace* w = c.w;
     cudaStream_t stream = c.stream;
@@ -469,7 +472,7 @@ int32_t enqueue_core(const CoreCtx& c, const SubBatch& sb, CoreOut* out) {
         cudaGetLastError();
     }
     BFQ_CUDA_TRY(cudaMemsetAsync(p.counters, 0, CTR_COUNT * sizeof(unsigned long long), stream));
-    bool ordered = false, dedup = false;
+    bool ordered = false;
     if (wants_order(c, sb)) {
         // group the topics by tenant and leading levels so that neighbouring lanes walk the same part of the trie, and
         // match every distinct (tenant, topic) pair once
@@ -492,9 +495,9 @@ int32_t enqueue_core(const CoreCtx& c, const SubBatch& sb, CoreOut* out) {
         BFQ_CUDA_TRY(launch_order(q, stream));
         p.order = q.order;
         p.order_count = p.counters + CTR_NLEAD;
+        p.pos_rec = w->d_pos_rec.p + b;
         out->n_launches += 3;
         ordered = true;
-        dedup = q.dedup != 0;
     }
     if (n > 0) {
         // tier 0 (one lane per topic), then tier 1 (one warp per topic) over whatever tier 0 deferred — its count is read
@@ -506,10 +509,13 @@ int32_t enqueue_core(const CoreCtx& c, const SubBatch& sb, CoreOut* out) {
         p.n_work = -1;
         launch_match(p, false, 0, stream);
         out->n_launches += 2;
-        if (ordered && dedup) {
+        if (ordered) {
+            // tier 0 wrote span records by position: gather them to topic order (behind tier 1, whose spans repeats copy)
             FinalizeParams f{};
             f.n_topics = n;
             f.leader = w->d_leader.p + b;
+            f.pos = w->d_ord_keys.p + b;
+            f.pos_rec = p.pos_rec;
             f.span_begin = p.span_begin;
             f.span_count = p.span_count;
             f.route_count = p.route_count;

@@ -326,6 +326,7 @@ __global__ void __launch_bounds__(L_WARPS * 32) match_topics_lane_kernel(const M
     // per-lane topic state; level < 0: the tenant root has not been expanded yet (`node` holds the root ordinal)
     bool have = false, bad = false;
     uint32_t t = 0, node = 0 /* child ref a (root ordinal while level < 0) */, plusf = NONE31, meta = 0, pending = 0, n_rg = 0, acc_r = 0;
+    uint32_t pos = 0;   // the topic's position in the work order (= t without an order)
     // matched persistent / group routes so far; bit 31 = "a node's saturated count byte was seen" (then the true sum is
     // unknown but large: the topic is flagged unless the cap is INT_MAX). <= INLINE_RANGES * 254 otherwise.
     uint32_t acc_p = 0, acc_g = 0;
@@ -359,13 +360,21 @@ __global__ void __launch_bounds__(L_WARPS * 32) match_topics_lane_kernel(const M
         acc_p = (acc_p + cp) | (cp == 0xFFu ? 0x80000000u : 0u);   // <= SPILL_RANGES additions of <= 255: no carry into bit 31
         acc_g = (acc_g + cg) | (cg == 0xFFu ? 0x80000000u : 0u);
     };
+    // the topic's span: one record at its position in an ordered batch (finalize_kernel gathers it), else the topic-indexed arrays
+    auto put_span = [&](uint32_t begin, uint32_t count, uint32_t routes, uint32_t deferred) {
+        if (p.order) {
+            p.pos_rec[pos] = SpanRecord{begin, count, routes, deferred};
+        } else {
+            p.span_begin[t] = begin;
+            p.span_count[t] = count;
+            p.route_count[t] = routes;
+        }
+    };
     auto finish = [&]() {
         if (bad) {
             const unsigned long long idx = atomicAdd(&p.counters[CTR_DEFER], 1ull);
             p.defer_list[idx] = t;
-            p.span_begin[t] = 0;
-            p.span_count[t] = SPAN_OVERFLOW;
-            p.route_count[t] = 0;
+            put_span(0u, SPAN_OVERFLOW, 0u, 1u);   // tier 1 writes the topic-indexed span
         } else {
             // the caps are only read for a topic that matched capped-kind routes in a tenant with a finite cap (bit 30 of
             // `tenant`, set when the chunk was claimed): the loads would otherwise stall the whole warp at every finish
@@ -377,9 +386,8 @@ __global__ void __launch_bounds__(L_WARPS * 32) match_topics_lane_kernel(const M
                 const bool flag_g = maxG != 0x7FFFFFFF && acc_g > (uint32_t) (maxG < 0 ? 0 : maxG);
                 flagged = flag_p || flag_g;
             }
-            p.span_begin[t] = (uint32_t) ((rg_out - n_rg) - p.ranges);   // the inline slots, or the spill block
-            p.span_count[t] = n_rg | (flagged ? SPAN_FLAGGED : 0u);
-            p.route_count[t] = acc_r;
+            put_span((uint32_t) ((rg_out - n_rg) - p.ranges),   // the inline slots, or the spill block
+                     n_rg | (flagged ? SPAN_FLAGGED : 0u), acc_r, 0u);
             if (flagged) {
                 const unsigned long long idx = atomicAdd(&p.counters[CTR_FLAGGED], 1ull);
                 p.flagged_list[idx] = t;
@@ -454,6 +462,7 @@ __global__ void __launch_bounds__(L_WARPS * 32) match_topics_lane_kernel(const M
                     // from the chunks it claimed, so its range writes stay in a few KB of the array instead of scattering over all
                     // of it (in locality order t is effectively random over an array larger than L2)
                     rg_out = p.ranges + (uint64_t) idx * INLINE_RANGES;
+                    pos = (uint32_t) idx;
                     bad = len > 65535;
                     have = true;
                     ws.lv[0][lane] = 0;
@@ -863,14 +872,29 @@ __global__ void __launch_bounds__(256) order_scatter_kernel(const OrderKernelPar
     const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= q.n_topics || q.leader[i] != (uint32_t) i) return;
     const uint32_t b = q.keys[i];
-    q.order[q.blk_pfx[b / SCAN_PER_BLOCK] + atomicAdd(&q.hist[b], 1u)] = (uint32_t) i;
+    const uint32_t at = q.blk_pfx[b / SCAN_PER_BLOCK] + atomicAdd(&q.hist[b], 1u);
+    q.order[at] = (uint32_t) i;
+    q.keys[i] = at;   // the bucket is dead now: keep the position for finalize_kernel (a coalesced store)
 }
 
-// followers take their leader's span; spans index the sparse range array, so the ranges themselves are shared
+// Topic order from tier 0's position records: a leader's record goes to its own index, a follower takes its leader's (spans
+// index the sparse range array, so the ranges themselves are shared). Every access but the record read is coalesced.
 __global__ void __launch_bounds__(256) finalize_kernel(const FinalizeParams p) {
     const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= p.n_topics) return;
     const uint32_t l = p.leader[i];
+    if (!p.second_pass) {
+        const SpanRecord r = p.pos_rec[p.pos[l]];
+        if (!r.deferred) {
+            p.span_begin[i] = r.span_begin;
+            p.span_count[i] = r.span_count;
+            p.route_count[i] = r.route_count;
+            // a flagged leader joined the list in tier 0
+            if (l != (uint32_t) i && (r.span_count & SPAN_FLAGGED)) p.flagged_list[atomicAdd(&p.counters[CTR_FLAGGED], 1ull)] = (uint32_t) i;
+            return;
+        }
+        // deferred to tier 1, which wrote the leader's topic-indexed span: a follower copies it below
+    }
     if (l == (uint32_t) i) return;
     if (p.second_pass && p.span_count[i] != SPAN_OVERFLOW) return;
     const uint32_t sc = p.span_count[l];

@@ -26,6 +26,17 @@ constexpr uint32_t SPAN_FLAGGED = 0x80000000u;   // in span_count: caps must be 
 constexpr uint32_t SPAN_OVERFLOW = 0x40000000u;  // in span_count: deferred to tier 2 (never visible to callers)
 constexpr uint32_t SPAN_COUNT_MASK = 0x3FFFFFFFu;
 
+// Tier 0's result for the topic at work-order position i when the batch is ordered (MatchParams::order set), written with one
+// 16-byte store to pos_rec[i]: the 32 positions of a chunk are neighbours, so a warp's record writes stay within a few hundred
+// bytes instead of scattering 3 x 32 words over the topic-indexed arrays. finalize_kernel gathers the records to topic order.
+struct __align__(16) SpanRecord {
+    uint32_t span_begin;
+    uint32_t span_count;    // count | SPAN_FLAGGED
+    uint32_t route_count;
+    uint32_t deferred;      // != 0: tier 0 handed the topic to tier 1, which writes the topic-indexed arrays itself
+};
+static_assert(sizeof(SpanRecord) == 16, "a span record is one 16-byte store");
+
 struct MatchParams {
     // index snapshot
     const Slot* slots;              // blocked edge table (trie_layout.h)
@@ -42,9 +53,12 @@ struct MatchParams {
     int32_t n_tenants;
     int64_t n_topics;
     // tier 0: optional processing order (topic indices grouped by tenant and leading levels, see launch_order); nullptr =>
-    // 0..n_topics. Only the order in which lanes pick topics changes; every output stays indexed by topic.
+    // 0..n_topics. With an order, tier 0 writes a topic's span record at its position in the order (pos_rec) and leaves the
+    // topic-indexed span_begin / span_count / route_count to finalize_kernel; without one it writes those three directly.
+    // Tiers 1 and 2 always write the topic-indexed arrays.
     const uint32_t* order;
     const unsigned long long* order_count;   // device scalar: entries of `order` (the batch's distinct topics); with order only
+    SpanRecord* pos_rec;                     // [n] with order only: tier 0's record of the topic at each position
     int32_t max_ctas_per_sm;        // tier 0: cap of resident CTAs per SM (0 = as many as fit); one slot less leaves room for a
                                     // concurrently running exchange (NCCL) kernel
     // tiers 1/2: list of topic indices to process (nullptr => all topics 0..n_topics)
@@ -152,18 +166,20 @@ cudaError_t launch_budget(const BudgetParams& q, void* d_scan_tmp, size_t* tmp_b
 //            only remember their leader. Leaders get an order key = tenant index | hashes of the level-0 / 0..1 / 0..2 prefixes
 //            and count themselves into a bucket histogram (bucket = the key's leading bits).
 //   scan     exclusive prefix sum of the histogram (block-local scans; the last block to finish scans the block totals)
-//   scatter  leaders -> order[bucket base + atomic cursor]: a counting sort, unstable inside a bucket (only grouping matters)
+//   scatter  leaders -> order[bucket base + atomic cursor]: a counting sort, unstable inside a bucket (only grouping matters);
+//            each leader's position goes back to keys[leader] for finalize_kernel
 // Tier 0 then matches order[0 .. n_leaders) — topics that walk the same top of the trie are matched by neighbouring lanes at
-// the same time — and finalize_kernel copies each follower's span from its leader (spans are indices into the sparse range
-// array, so no range is copied). The reference never sees duplicates (matchAll takes a Set<String>,
-// DW/cache/ITenantRouteMatcher.java:28-38; DW/cache/TenantRouteCache.java:100-139 serves repeats from its cache).
+// the same time — and finalize_kernel gathers tier 0's span records back to topic order, giving each follower its leader's
+// span (spans are indices into the sparse range array, so no range is copied). The reference never sees duplicates
+// (matchAll takes a Set<String>, DW/cache/ITenantRouteMatcher.java:28-38; DW/cache/TenantRouteCache.java:100-139 serves
+// repeats from its cache).
 struct OrderParams {
     int64_t n_topics;
     const uint8_t* topics;
     const int64_t* topic_off;
     const int32_t* topic_tenant;
     int32_t n_tenants;
-    uint32_t* keys;                 // [n] bucket of each leader
+    uint32_t* keys;                 // [n] bucket of each leader; after the scatter: the leader's position in `order`
     uint32_t* leader;               // [n] out: i for a leader, else the index of the identical topic that leads
     uint32_t* order;                // [n] out: the leaders, grouped by bucket
     unsigned long long* hash_tab;   // [hash_mask + 1], filled with 0xFF bytes by launch_order when dedup is set
@@ -178,11 +194,15 @@ uint32_t order_hash_entries(int64_t n_topics);                     // dedup tabl
 // enqueues the scratch and hash-table fills and the three kernels on stream
 cudaError_t launch_order(const OrderParams& q, cudaStream_t stream);
 
-// followers copy their leader's span (and join the flagged list if it needs caps). second_pass: only the followers whose
-// span still carries the tier-2 marker (their leader was finished by tier 2 after the first pass).
+// Runs behind tiers 0 and 1 of every ordered batch. First pass: every topic takes its leader's span record from tier 0's
+// position records (a repeat of a flagged record also joins the flagged list); a repeat of a leader that tier 0 deferred copies
+// the leader's topic-indexed span, which tier 1 wrote. second_pass: only the repeats whose span still carries the tier-2 marker
+// (their leader was finished by tier 2 after the first pass) copy it again.
 struct FinalizeParams {
     int64_t n_topics;
     const uint32_t* leader;
+    const uint32_t* pos;            // [n] OrderParams::keys after launch_order: position of each leader in the order
+    const SpanRecord* pos_rec;      // MatchParams::pos_rec
     uint32_t* span_begin;
     uint32_t* span_count;
     uint32_t* route_count;
