@@ -56,6 +56,11 @@ class BfqDeliveryOrderedResult(C.Structure):
                 ("n_ordered_packs", C.c_int64)]
 
 
+class BfqDeliveryWireResult(C.Structure):
+    _fields_ = [("d_req_off", C.c_void_p), ("n_bytes", C.c_int64), ("n_match_infos", C.c_int64), ("n_skipped", C.c_int64),
+                ("n_deliverers", C.c_int32), ("ordered_share_id", C.c_int32), ("generation", C.c_uint64)]
+
+
 class BfqBudgetResult(C.Structure):
     _fields_ = [("d_delivered_persistent", C.c_void_p), ("d_topic_flags", C.c_void_p), ("n_delivered", C.c_int64),
                 ("n_dropped_bytes", C.c_int64), ("n_dropped_persistent_bandwidth", C.c_int64),
@@ -106,6 +111,10 @@ _SIGNATURES = {
     "bfq_delivery_device": (_i32, [C.POINTER(BfqDeviceResult), _vp, _vp, _i64, _vp, _vp, C.POINTER(BfqDeliveryResult)]),
     "bfq_delivery_device_ordered": (_i32, [C.POINTER(BfqDeviceResult), _vp, _vp, _i64, _vp, _vp, _vp, _i64, _vp,
                                            C.POINTER(BfqDeliveryOrderedResult)]),
+    "bfq_delivery_encode": (_i32, [C.POINTER(BfqDeviceResult), C.POINTER(BfqDeliveryResult), _vp, _vp, _i32, _vp, _vp, _vp, _vp,
+                                   _vp, _vp, _i64, _vp, C.POINTER(BfqDeliveryWireResult)]),
+    "bfq_delivery_encode_ordered": (_i32, [C.POINTER(BfqDeviceResult), C.POINTER(BfqDeliveryOrderedResult), _vp, _vp, _i32, _vp,
+                                           _vp, _vp, _vp, _vp, _vp, _i64, _vp, C.POINTER(BfqDeliveryWireResult)]),
     "bfq_exchange_unique_id": (_i32, [_vp, _i32]),
     "bfq_exchange_create": (_i32, [_i32, _i32, _i32, _vp, C.POINTER(_vp)]),
     "bfq_exchange_destroy": (None, [_vp]),

@@ -40,6 +40,7 @@ struct Snapshot {
         std::shared_ptr<const KVBlob> kv;
         std::shared_ptr<const std::vector<uint8_t>> rkind;
         std::shared_ptr<const TenantFan> fan;   // routes -> deliverer ids, built on the first fan-out that sees this blob
+        std::shared_ptr<const TenantWire> wire; // routes -> MatchInfo bytes, built on the first encode that sees this blob
     };
     // fan-out tables of the whole snapshot (device), assembled from the tenants' on first use
     struct FanTable {
@@ -54,9 +55,18 @@ struct Snapshot {
         DeviceBuf<uint32_t> d_len;
         uint32_t member_bits = 1;                // bits of the largest ordered group's size
     };
+    // every route's MatchInfo bytes (device), for bfq_delivery_encode: built on the first encode call
+    struct WireTable {
+        DeviceBuf<uint32_t> d_first;             // per rank: its first entry
+        DeviceBuf<unsigned long long> d_off;     // [entries + 1]
+        DeviceBuf<uint8_t> d_bytes;
+        int64_t bytes() const { return (int64_t) (d_first.bytes() + d_off.bytes() + d_bytes.bytes()); }
+    };
     std::mutex fan_mu;
     std::shared_ptr<FanTable> fan;
     std::shared_ptr<UrlTable> urls;
+    std::shared_ptr<WireTable> wire;
+    std::atomic<int64_t> wire_bytes{0};      // wire->bytes() once built (bfq_index_stats reads it without fan_mu)
     std::vector<TenantHost> th;
     uint64_t garbage_slots = 0;   // slots of regions that delta commits replaced (reclaimed by the next full build)
     int64_t delta_commits = 0;    // delta commits since the last full build
@@ -139,6 +149,13 @@ struct Workspace {
     DeviceBuf<uint32_t> d_os_flag, d_os_u32, d_pack_pub;
     DeviceBuf<unsigned long long> d_os_items, d_os_check, d_os_key;
     DeviceBuf<long long> d_pack_pub_off;
+    // the nesting the last delivery call left in the buffers above (n_packs < 0: none, or a call that failed)
+    int64_t dl_n_pairs = -1, dl_n_packages = -1, dl_n_packs = -1;
+    bool dl_ordered = false;
+    // DeliveryRequest encoding (bfq_delivery_encode): the size scans (pairs, packs, packages), the checks, the offsets
+    DeviceBuf<unsigned long long> d_wr_pos, d_wr_check;
+    DeviceBuf<long long> d_req_off, d_wr_tenant_off;
+    DeviceBuf<uint8_t> d_wr_tenants, d_wr_tmp;
     // pinned result buffers
     PinnedBuf<uint32_t> h_span_begin, h_span_count, h_route_count;
     PinnedBuf<uint2> h_ranges;
@@ -259,6 +276,7 @@ int32_t acquire(bfq_index* h, std::shared_ptr<Snapshot>* snap, Workspace** ws, c
             return fail(BFQ_E_CUDA, std::string("workspace: ") + cudaGetErrorString(e));
         }
     }
+    w->dl_n_packs = -1;   // a new lease starts without a delivery nesting: one left by the previous lease is not this result's
     *ws = w;
     return BFQ_OK;
 }
@@ -1373,14 +1391,15 @@ int32_t bfq_index_stats(bfq_index* h, int64_t* stats, int32_t n) {
     std::lock_guard<std::mutex> g(h->mu);
     static const FlatIndex empty;
     const FlatIndex& f = h->snap ? h->snap->flat : empty;
-    const int64_t v[22] = {f.n_routes, (int64_t) f.tenant_ordinal.size(), f.n_nodes, (int64_t) f.n_slots,
+    const int64_t wire_bytes = h->snap ? h->snap->wire_bytes.load() : 0;
+    const int64_t v[23] = {f.n_routes, (int64_t) f.tenant_ordinal.size(), f.n_nodes, (int64_t) f.n_slots,
                            h->snap ? h->snap->device_bytes() : 0, f.max_nodes_per_depth, h->launches, h->overflow_topics,
                            h->flagged_topics, f.n_multi, f.n_cont_chunks, h->deferred_topics, h->duplicate_topics,
                            h->full_commits, h->delta_commits, h->snap ? (int64_t) h->snap->garbage_slots : 0,
                            h->buffer_retries, h->global_fanouts,
                            h->snap ? (int64_t) f.n_blocks * BLOCK_USABLE : 0, (int64_t) f.n_big_edges, f.overflowed_blocks,
-                           h->rebuilt_tenants};
-    for (int32_t i = 0; i < n && i < 22; i++) stats[i] = v[i];
+                           h->rebuilt_tenants, wire_bytes};
+    for (int32_t i = 0; i < n && i < 23; i++) stats[i] = v[i];
     return BFQ_OK;
 }
 
@@ -2333,6 +2352,7 @@ int32_t run_delivery_call(const bfq_device_result* res, const int64_t* d_offsets
     if (n_pairs >= (int64_t) 0xFFFFFFF0ll) return fail(BFQ_E_RANGE, "more than 2^32 (topic, route) pairs in one batch; split the batch");
     bfq_index* h = L->h;
     Workspace* w = L->ws;
+    w->dl_n_packs = -1;   // the buffers below are about to change
     std::shared_ptr<Snapshot::FanTable> ft;
     rc = ensure_fan_table(h, L->snap.get(), &ft);
     if (rc != BFQ_OK) return rc;
@@ -2478,6 +2498,10 @@ int32_t run_delivery_call(const bfq_device_result* res, const int64_t* d_offsets
     out->n_deliverers = (int32_t) ft->n_deliverers;
     out->ordered_share_id = (int32_t) ft->n_deliverers - 1;
     out->generation = L->snap->generation;
+    w->dl_n_pairs = out->n_pairs;
+    w->dl_n_packages = out->n_packages;
+    w->dl_n_packs = out->n_packs;
+    w->dl_ordered = pubs != nullptr;
     if (oout) {
         oout->d_pack_pub_off = (const int64_t*) w->d_pack_pub_off.p;
         oout->d_pack_pub = w->d_pack_pub.p;
@@ -2501,6 +2525,181 @@ int32_t bfq_delivery_device_ordered(const bfq_device_result* res, const int64_t*
     const PublisherPacks pubs{d_pub_off, d_pub_hash, n_pubs};
     return run_delivery_call(res, d_offsets, d_ranks, n_pairs, d_topic_tenant, stream, "bfq_delivery_device_ordered", &pubs, &out->d,
                              out);
+}
+
+namespace {
+// the snapshot's MatchInfo table: every tenant's entries (cached per tenant blob, so a delta commit re-encodes only the tenants it
+// rebuilt), concatenated in rank order and uploaded once per snapshot
+int32_t ensure_wire_table(Snapshot* s, std::shared_ptr<Snapshot::WireTable>* out) {
+    std::lock_guard<std::mutex> g(s->fan_mu);
+    if (s->wire) {
+        *out = s->wire;
+        return BFQ_OK;
+    }
+    const size_t T = s->th.size();
+    std::vector<std::string> errs(T);
+    {
+        std::atomic<size_t> cursor{0};
+        auto worker = [&]() {
+            while (true) {
+                const size_t i = cursor.fetch_add(1);
+                if (i >= T) break;
+                if (s->th[i].wire) continue;
+                auto tw = std::make_shared<TenantWire>();
+                if (build_tenant_wire(*s->th[i].kv, tw.get(), &errs[i])) s->th[i].wire = std::move(tw);
+            }
+        };
+        const unsigned nt = (unsigned) std::max<size_t>(1, std::min<size_t>(std::min<size_t>(std::thread::hardware_concurrency(), 64), T));
+        std::vector<std::thread> th;
+        for (unsigned t = 1; t < nt; t++) th.emplace_back(worker);
+        worker();
+        for (auto& x : th) x.join();
+    }
+    size_t entries = 0, bytes = 0;
+    for (size_t i = 0; i < T; i++) {
+        if (!s->th[i].wire) return fail(BFQ_E_INVALID, "MatchInfo table: " + errs[i]);
+        entries += s->th[i].wire->off.size() - 1;
+        bytes += s->th[i].wire->bytes.size();
+    }
+    if (entries >= 0xFFFFFFFFull) return fail(BFQ_E_RANGE, "2^32 or more MatchInfos in one snapshot");
+    std::vector<uint32_t> first((size_t) std::max<int64_t>(s->flat.n_routes, 1), 0);
+    std::vector<unsigned long long> off(1, 0);
+    off.reserve(entries + 1);
+    std::vector<uint8_t> blob;
+    blob.reserve(bytes);
+    for (size_t i = 0; i < T; i++) {
+        const TenantWire& tw = *s->th[i].wire;
+        const uint32_t ebase = (uint32_t) (off.size() - 1);
+        const unsigned long long bbase = blob.size();
+        const int64_t lo = s->flat.tenants[i].lo;
+        for (size_t r = 0; r < tw.first.size(); r++) first[(size_t) lo + r] = tw.first[r] + ebase;
+        for (size_t e = 1; e < tw.off.size(); e++) off.push_back(tw.off[e] + bbase);
+        blob.insert(blob.end(), tw.bytes.begin(), tw.bytes.end());
+    }
+    auto wt = std::make_shared<Snapshot::WireTable>();
+    BFQ_CUDA_TRY(wt->d_first.reserve(first.size()));
+    BFQ_CUDA_TRY(wt->d_off.reserve(off.size()));
+    BFQ_CUDA_TRY(wt->d_bytes.reserve(std::max<size_t>(blob.size(), 1)));
+    BFQ_CUDA_TRY(cudaMemcpy(wt->d_first.p, first.data(), first.size() * 4, cudaMemcpyHostToDevice));
+    BFQ_CUDA_TRY(cudaMemcpy(wt->d_off.p, off.data(), off.size() * 8, cudaMemcpyHostToDevice));
+    if (!blob.empty()) BFQ_CUDA_TRY(cudaMemcpy(wt->d_bytes.p, blob.data(), blob.size(), cudaMemcpyHostToDevice));
+    s->wire = wt;
+    s->wire_bytes = wt->bytes();
+    *out = wt;
+    return BFQ_OK;
+}
+
+// bfq_delivery_encode (oout == nullptr) and bfq_delivery_encode_ordered: nest is the nesting's plain part either way
+int32_t run_encode(const bfq_device_result* res, const bfq_delivery_result* nest, const bfq_delivery_ordered_result* onest,
+                   const uint8_t* tenants, const int64_t* tenant_off, int32_t n_tenants, const uint8_t* d_topics,
+                   const int64_t* d_topic_off, const int64_t* d_pub_off, const uint8_t* d_pubpack_bytes,
+                   const int64_t* d_pubpack_off, uint8_t* d_out, int64_t out_cap, void* stream, const char* who,
+                   bfq_delivery_wire_result* out) {
+    if (!res || !res->lease || !nest || !out || out_cap < 0) return fail(BFQ_E_INVALID, "bad argument");
+    auto* L = static_cast<DeviceLease*>(res->lease);
+    cudaStream_t st = (cudaStream_t) stream;
+    cudaEvent_t ev = nullptr;
+    int32_t rc = lease_use(res, st, who, &ev);
+    if (rc != BFQ_OK) return rc;
+    RecordOnExit rec(ev, st);   // the write pass is still running when the call returns
+    if (!d_topics || !d_topic_off || !d_pub_off || !d_pubpack_bytes || !d_pubpack_off)
+        return fail(BFQ_E_INVALID, std::string(who) + ": NULL topic or publisher pack array");
+    if (n_tenants != L->ctx.n_tenants || (n_tenants > 0 && (!tenants || !tenant_off)))
+        return fail(BFQ_E_INVALID, std::string(who) + ": the tenant list must be the match's (" + std::to_string(L->ctx.n_tenants) + " tenants)");
+    Workspace* w = L->ws;
+    // the nesting must be the one the last delivery call on this result left in its workspace
+    if (nest->generation != L->snap->generation || nest->d_package_off != (const int64_t*) w->d_package_off.p ||
+        nest->d_match_off != (const int64_t*) w->d_match_off.p || w->dl_n_packs < 0 || nest->n_packs != w->dl_n_packs ||
+        nest->n_packages != w->dl_n_packages || nest->n_pairs != w->dl_n_pairs || w->dl_ordered != (onest != nullptr) ||
+        (onest && onest->d_pack_pub_off != (const int64_t*) w->d_pack_pub_off.p))
+        return fail(BFQ_E_RANGE, std::string(who) + ": the nesting is not the latest " +
+                                     (onest ? "bfq_delivery_device_ordered" : "bfq_delivery_device") + " result of this device result");
+    bfq_index* h = L->h;
+    std::shared_ptr<Snapshot::WireTable> wt;
+    if ((rc = ensure_wire_table(L->snap.get(), &wt)) != BFQ_OK) return rc;
+    const int64_t np = nest->n_pairs, nk = nest->n_packs, ng = nest->n_packages;
+    const uint32_t D = (uint32_t) nest->n_deliverers;
+    BFQ_CUDA_TRY(w->d_wr_pos.reserve((size_t) (np + 1 + nk + 1 + ng + 1)));
+    BFQ_CUDA_TRY(w->d_wr_check.reserve(4));
+    BFQ_CUDA_TRY(w->d_req_off.reserve((size_t) D + 1));
+    BFQ_CUDA_TRY(w->d_wr_tenant_off.reserve((size_t) n_tenants + 1));
+    const int64_t tbytes = n_tenants > 0 ? tenant_off[n_tenants] : 0;
+    BFQ_CUDA_TRY(w->d_wr_tenants.reserve((size_t) std::max<int64_t>(tbytes, 1)));
+    if (n_tenants > 0) {
+        BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_wr_tenant_off.p, tenant_off, ((size_t) n_tenants + 1) * 8, cudaMemcpyHostToDevice, st));
+        if (tbytes > 0) BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_wr_tenants.p, tenants, (size_t) tbytes, cudaMemcpyHostToDevice, st));
+    }
+    WireParams p{};
+    p.n_packages = ng;
+    p.n_packs = nk;
+    p.n_pairs = np;
+    p.n_deliverers = D;
+    p.package_off = (const long long*) nest->d_package_off;
+    p.package_tenant = nest->d_package_tenant;
+    p.pack_off = (const long long*) nest->d_pack_off;
+    p.pack_topic = nest->d_pack_topic;
+    p.match_off = (const long long*) nest->d_match_off;
+    p.match_rank = nest->d_match_rank;
+    p.match_member = nest->d_match_member;
+    p.pack_pub_off = onest ? (const long long*) onest->d_pack_pub_off : nullptr;
+    p.pack_pub = onest ? onest->d_pack_pub : nullptr;
+    p.tenants = w->d_wr_tenants.p;
+    p.tenant_off = w->d_wr_tenant_off.p;
+    p.topics = d_topics;
+    p.topic_off = (const long long*) d_topic_off;
+    p.n_topics = L->n;
+    p.pub_off = (const long long*) d_pub_off;
+    p.pubpack = d_pubpack_bytes;
+    p.pubpack_off = (const long long*) d_pubpack_off;
+    p.mi_first = wt->d_first.p;
+    p.mi_off = wt->d_off.p;
+    p.mi_bytes = wt->d_bytes.p;
+    p.pair_pos = w->d_wr_pos.p;
+    p.pack_pos = p.pair_pos + np + 1;
+    p.package_pos = p.pack_pos + nk + 1;
+    p.check = w->d_wr_check.p;
+    p.req_off = w->d_req_off.p;
+    p.out = d_out;
+    size_t tmp_bytes = 0;
+    BFQ_CUDA_TRY(launch_wire_size(p, nullptr, &tmp_bytes, st));
+    BFQ_CUDA_TRY(w->d_wr_tmp.reserve(tmp_bytes + 256));
+    BFQ_CUDA_TRY(launch_wire_size(p, w->d_wr_tmp.p, &tmp_bytes, st));
+    unsigned long long chk[4];
+    BFQ_CUDA_TRY(cudaMemcpyAsync(chk, w->d_wr_check.p, sizeof(chk), cudaMemcpyDeviceToHost, st));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
+    if (chk[0]) return fail(BFQ_E_INVALID, std::string(who) + ": d_pub_off / d_pubpack_off must start at 0 and never decrease, and "
+                                                               "every publisher of the nesting must be below d_pub_off[n_topics]");
+    const bool write = d_out && (int64_t) chk[1] <= out_cap;
+    if (write) BFQ_CUDA_TRY(launch_wire_write(p, st));
+    {
+        std::lock_guard<std::mutex> g(h->mu);
+        h->launches += write ? 10 : 8;
+    }
+    out->d_req_off = (const int64_t*) w->d_req_off.p;
+    out->n_bytes = (int64_t) chk[1];
+    out->n_match_infos = (int64_t) chk[2];
+    out->n_skipped = np - (int64_t) chk[2];
+    out->n_deliverers = (int32_t) D;
+    out->ordered_share_id = (int32_t) D - 1;
+    out->generation = L->snap->generation;
+    return BFQ_OK;
+}
+}  // namespace
+
+int32_t bfq_delivery_encode(const bfq_device_result* res, const bfq_delivery_result* nesting, const uint8_t* tenants,
+                            const int64_t* tenant_off, int32_t n_tenants, const uint8_t* d_topics, const int64_t* d_topic_off,
+                            const int64_t* d_pub_off, const uint8_t* d_pubpack_bytes, const int64_t* d_pubpack_off, uint8_t* d_out,
+                            int64_t out_cap, void* stream, bfq_delivery_wire_result* out) {
+    return run_encode(res, nesting, nullptr, tenants, tenant_off, n_tenants, d_topics, d_topic_off, d_pub_off, d_pubpack_bytes,
+                      d_pubpack_off, d_out, out_cap, stream, "bfq_delivery_encode", out);
+}
+
+int32_t bfq_delivery_encode_ordered(const bfq_device_result* res, const bfq_delivery_ordered_result* nesting, const uint8_t* tenants,
+                                    const int64_t* tenant_off, int32_t n_tenants, const uint8_t* d_topics, const int64_t* d_topic_off,
+                                    const int64_t* d_pub_off, const uint8_t* d_pubpack_bytes, const int64_t* d_pubpack_off,
+                                    uint8_t* d_out, int64_t out_cap, void* stream, bfq_delivery_wire_result* out) {
+    return run_encode(res, nesting ? &nesting->d : nullptr, nesting, tenants, tenant_off, n_tenants, d_topics, d_topic_off, d_pub_off,
+                      d_pubpack_bytes, d_pubpack_off, d_out, out_cap, stream, "bfq_delivery_encode_ordered", out);
 }
 
 int32_t bfq_fanout_deliverer(bfq_index* h, int32_t id, int32_t* sub_broker_id, uint8_t* key_out, int64_t key_cap, int64_t* key_len) {

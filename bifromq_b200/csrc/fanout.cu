@@ -713,7 +713,8 @@ bool split_receiver_url(sv url, int32_t* broker, sv* deliverer_key) {
     return true;
 }
 // RouteGroup { map<string, uint64> members = 1; }  (bifromq-dist-worker-schema/src/main/proto/distservice/RouteGroup.proto:27-29):
-// repeated field 1, each a nested message {1: string key, 2: varint value}. Calls f(receiverUrl) per member in wire order.
+// repeated field 1, each a nested message {1: string key, 2: varint value}. Calls f(receiverUrl, incarnation) per member in wire
+// order.
 template <typename F>
 bool for_each_group_member(sv b, F&& f) {
     size_t i = 0;
@@ -739,6 +740,7 @@ bool for_each_group_member(sv b, F&& f) {
         if (!varint(&len) || i + len > b.size()) return false;
         const size_t end = i + (size_t) len;
         sv key;
+        uint64_t value = 0;
         while (i < end) {
             uint64_t t2;
             if (!varint(&t2)) return false;
@@ -748,13 +750,12 @@ bool for_each_group_member(sv b, F&& f) {
                 key = b.substr(i, (size_t) kl);
                 i += (size_t) kl;
             } else if (t2 == (2u << 3)) {
-                uint64_t v;
-                if (!varint(&v)) return false;
+                if (!varint(&value)) return false;
             } else {
                 return false;
             }
         }
-        f(key);
+        f(key, value);
     }
     return true;
 }
@@ -801,7 +802,7 @@ bool build_tenant_fan(const KVBlob& kv, DelivererTable* table, TenantFan* out, s
         const bool ordered = d.flag == FLAG_ORDERED;
         out->gordered.push_back(ordered ? 1 : 0);
         bool ok = true;
-        const bool parsed = for_each_group_member(kv.val(r), [&](sv url) {
+        const bool parsed = for_each_group_member(kv.val(r), [&](sv url, uint64_t) {
             int32_t broker = 0;
             sv dk;
             if (!split_receiver_url(url, &broker, &dk)) {
@@ -818,6 +819,94 @@ bool build_tenant_fan(const KVBlob& kv, DelivererTable* table, TenantFan* out, s
         }
         out->gmem_off.push_back((uint32_t) out->gmem_deliv.size());
     }
+    return true;
+}
+
+// ------------------------------------------------------------------------------------------------ host: MatchInfo wire bytes
+namespace {
+void put_varint(std::string& s, uint64_t v) {
+    while (v >= 0x80) {
+        s.push_back((char) (uint8_t) (v | 0x80));
+        v >>= 7;
+    }
+    s.push_back((char) (uint8_t) v);
+}
+void put_len_field(std::string& s, uint8_t tag, sv bytes) {
+    s.push_back((char) tag);
+    put_varint(s, bytes.size());
+    s.append(bytes);
+}
+// RouteMatcher {type = 1, repeated filterLevel = 2, optional group = 3, mqttTopicFilter = 4} as RouteDetailCache.get builds it:
+// Normal (type left at 0) with the unescaped filter; UnorderedShare / OrderedShare with the group set and
+// "$share/<group>/<filter>" / "$oshare/<group>/<filter>". filterLevel = parse(escapedFilter, true): every NUL-separated level,
+// empty ones included.
+std::string route_matcher_bytes(const DecodedKey& d) {
+    std::string m;
+    const bool group = d.kind == KIND_GROUP;
+    if (group) {
+        m.push_back(0x08);
+        put_varint(m, d.flag == FLAG_ORDERED ? 2 : 1);
+    }
+    for_each_level(d.escaped_filter, '\0', [&](sv level) { put_len_field(m, 0x12, level); });
+    std::string filter(d.escaped_filter);
+    std::replace(filter.begin(), filter.end(), '\0', '/');
+    if (group) {
+        put_len_field(m, 0x1A, d.receiver);
+        filter = std::string(d.flag == FLAG_ORDERED ? "$oshare/" : "$share/") + std::string(d.receiver) + "/" + filter;
+    }
+    if (!filter.empty()) put_len_field(m, 0x22, filter);
+    return m;
+}
+// MatchInfo {matcher = 1, receiverId = 2, incarnation = 3} (NormalMatching), as DeliveryPack's matchInfo = 3 field. receiverId is
+// ReceiverCache's parts[1] of "<subBrokerId>\0<receiverId>\0<delivererKey>".
+bool put_match_info(std::string& out, const std::string& matcher, sv receiver_url, uint64_t incarnation) {
+    const size_t a = receiver_url.find('\0');
+    const size_t b = a == sv::npos ? sv::npos : receiver_url.find('\0', a + 1);
+    if (b == sv::npos) return false;
+    std::string mi;
+    put_len_field(mi, 0x0A, matcher);
+    if (b > a + 1) put_len_field(mi, 0x12, receiver_url.substr(a + 1, b - a - 1));
+    if (incarnation) {
+        mi.push_back(0x18);
+        put_varint(mi, incarnation);
+    }
+    put_len_field(out, 0x1A, mi);
+    return true;
+}
+}  // namespace
+
+bool build_tenant_wire(const KVBlob& kv, TenantWire* out, std::string* err) {
+    const int64_t n = kv.n();
+    out->first.assign((size_t) n, 0);
+    out->off.assign(1, 0);
+    out->bytes.clear();
+    auto fail_with = [&](const char* what) {
+        if (err) *err = what;
+        return false;
+    };
+    for (int64_t r = 0; r < n; r++) {
+        DecodedKey d;
+        if (!decode_route_key(kv.key(r), &d)) return fail_with("undecodable route key");
+        out->first[(size_t) r] = (uint32_t) (out->off.size() - 1);
+        const std::string matcher = route_matcher_bytes(d);
+        if (d.kind != KIND_GROUP) {
+            const sv v = kv.val(r);   // BSUtil.toLong: 8 bytes, big-endian
+            if (v.size() < 8) return fail_with("normal route value shorter than 8 bytes");
+            uint64_t inc = 0;
+            for (int i = 0; i < 8; i++) inc = inc << 8 | (uint8_t) v[(size_t) i];
+            if (!put_match_info(out->bytes, matcher, d.receiver, inc)) return fail_with("receiver url without a receiverId");
+            out->off.push_back(out->bytes.size());
+            continue;
+        }
+        bool ok = true;
+        const bool parsed = for_each_group_member(kv.val(r), [&](sv url, uint64_t inc) {
+            ok = ok && put_match_info(out->bytes, matcher, url, inc);
+            out->off.push_back(out->bytes.size());
+        });
+        if (!parsed) return fail_with("undecodable RouteGroup value");
+        if (!ok) return fail_with("member receiver url without a receiverId");
+    }
+    if (out->off.size() - 1 >= 0xFFFFFFFFull) return fail_with("2^32 or more MatchInfos in one tenant");
     return true;
 }
 

@@ -143,4 +143,56 @@ struct TenantFan {
 };
 bool build_tenant_fan(const KVBlob& kv, DelivererTable* table, TenantFan* out, std::string* err);
 
+// one tenant's MatchInfos as wire bytes (built once per tenant KV blob, like TenantFan): entry e is the whole `matchInfo = 3`
+// field of a DeliveryPack (tag, length, MatchInfo) as NormalMatching / GroupMatching build it from the route key and value
+// (DWS/cache/RouteDetailCache.java:53-109, ReceiverCache.java:32-36). One entry per normal route, one per member of a group in
+// the fan-out's member order; a member-less group has none.
+struct TenantWire {
+    std::vector<uint32_t> first;         // per local rank: its entry (a group's first member's)
+    std::vector<uint64_t> off;           // [entries + 1]: entry e is bytes[off[e] .. off[e + 1])
+    std::string bytes;
+};
+bool build_tenant_wire(const KVBlob& kv, TenantWire* out, std::string* err);
+
+// bfq_delivery_encode: a delivery nesting (launch_delivery's outputs) as one DeliveryRequest per deliverer (delivery_wire.cu)
+struct WireParams {
+    // the nesting
+    int64_t n_packages, n_packs, n_pairs;
+    uint32_t n_deliverers;               // the last id is ordered_share_id: its span is left empty
+    const long long* package_off;        // [n_deliverers + 1]
+    const uint32_t* package_tenant;      // [n_packages]
+    const long long* pack_off;           // [n_packages + 1]
+    const uint32_t* pack_topic;          // [n_packs]
+    const long long* match_off;          // [n_packs + 1]
+    const uint32_t* match_rank;          // [n_pairs]
+    const uint32_t* match_member;        // [n_pairs]
+    const long long* pack_pub_off;       // [n_packs + 1] or nullptr (every pack is whole)
+    const uint32_t* pack_pub;
+    // the batch: tenants (device copy of the match's list), topics, publisher packs
+    const uint8_t* tenants;
+    const long long* tenant_off;         // [n_tenants + 1]
+    const uint8_t* topics;
+    const long long* topic_off;          // [n_topics + 1]
+    int64_t n_topics;
+    const long long* pub_off;            // [n_topics + 1]
+    const uint8_t* pubpack;
+    const long long* pubpack_off;        // [n_pubs + 1], n_pubs = pub_off[n_topics]
+    // the snapshot's MatchInfo table
+    const uint32_t* mi_first;            // per rank
+    const unsigned long long* mi_off;    // [entries + 1]
+    const uint8_t* mi_bytes;
+    // scratch
+    unsigned long long* pair_pos;        // [n_pairs + 1] MatchInfo field bytes per pair, scanned
+    unsigned long long* pack_pos;        // [n_packs + 1] pack field bytes, scanned
+    unsigned long long* package_pos;     // [n_packages + 1] map entry field bytes, scanned
+    unsigned long long* check;           // [4]: bad pub_off / pubpack_off / pack_pub, total bytes, MatchInfos encoded
+    // outputs
+    long long* req_off;                  // [n_deliverers + 1]
+    uint8_t* out;
+};
+// pass 1 (sizes, req_off, check[]); d_tmp == nullptr: query the scan scratch size
+cudaError_t launch_wire_size(const WireParams& p, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream);
+// pass 2: the bytes (after pass 1 and a total that fits the caller's buffer)
+cudaError_t launch_wire_write(const WireParams& p, cudaStream_t stream);
+
 }  // namespace bfq

@@ -238,6 +238,24 @@ class DeviceResult:
                                                   d_pub_off_ptr, d_pub_hash_ptr, n_pubs, stream, C.byref(out)))
         return DeliveryResult(out.d, out)
 
+    def delivery_wire(self, nesting, tenants, d_topics_ptr, d_topic_off_ptr, d_pub_off_ptr, d_pubpack_ptr, d_pubpack_off_ptr,
+                      d_out_ptr, out_cap, stream=0):
+        """bfq_delivery_encode[_ordered]: `nesting` (the latest delivery() or delivery_ordered() of this result) as one
+        serialized DeliveryRequest per deliverer. tenants: the match's tenant list (or tenant_blob(...)); topics as the match
+        took them; d_pub_off_ptr: int64 [n_topics + 1] publisher packs per topic position, d_pubpack_ptr / d_pubpack_off_ptr
+        (int64 [n_pubs + 1]) their serialized TopicMessagePack.PublisherPack bytes (device). Bytes go to d_out_ptr only if they
+        fit out_cap (d_out_ptr = None only sizes). -> BfqDeliveryWireResult: deliverer d's request is
+        out[d_req_off[d] .. d_req_off[d + 1])"""
+        tb, toff, nt = GpuRouteIndex._tenants(tenants)
+        out = N.BfqDeliveryWireResult()
+        args = (N.ptr(tb), N.ptr(toff), nt, d_topics_ptr, d_topic_off_ptr, d_pub_off_ptr, d_pubpack_ptr, d_pubpack_off_ptr,
+                d_out_ptr, out_cap, stream, C.byref(out))
+        if nesting.ordered is not None:
+            N.check(N.lib.bfq_delivery_encode_ordered(C.byref(self.raw), C.byref(nesting.ordered), *args))
+        else:
+            N.check(N.lib.bfq_delivery_encode(C.byref(self.raw), C.byref(nesting.raw), *args))
+        return out
+
     def release(self):
         if getattr(self, "raw", None) is not None and self.raw.lease:
             N.lib.bfq_device_result_release(C.byref(self.raw))
@@ -295,12 +313,12 @@ class GpuRouteIndex:
         N.check(N.lib.bfq_index_commit(self._h))
 
     def stats(self):
-        s = np.zeros(22, np.int64)
+        s = np.zeros(23, np.int64)
         N.check(N.lib.bfq_index_stats(self._h, s.ctypes.data, len(s)))
         names = ["routes", "tenants", "nodes", "slots", "device_bytes", "max_nodes_per_depth", "launches",
                  "overflow_topics", "flagged_topics", "multi_segment_filters", "long_token_chunks", "deferred_topics",
                  "duplicate_topics", "full_commits", "delta_commits", "garbage_slots", "buffer_retries", "global_fanouts",
-                 "tag_usable_slots", "tag_used_slots", "tag_overflowed_blocks", "rebuilt_tenants"]
+                 "tag_usable_slots", "tag_used_slots", "tag_overflowed_blocks", "rebuilt_tenants", "wire_table_bytes"]
         return dict(zip(names, s.tolist()))
 
     def deliverer(self, deliverer_id):

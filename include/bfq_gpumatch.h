@@ -119,7 +119,8 @@ int32_t bfq_index_set_option(bfq_index* h, const char* name, int64_t value);
  * throttle buffer too small, grew it and re-ran the batch so far, 17 bfq_fanout_device calls that took the global-count
  * pass (rather than the shared-memory tile pass) so far, 18 usable tag-table slots (15 per block), 19 claimed tag-table
  * slots (children of wide nodes), 20 tag-table blocks whose overflow byte is set (all three of the current snapshot), 21 tenants
- * the last bfq_index_commit built (0 when nothing changed, every tenant after a full build) */
+ * the last bfq_index_commit built (0 when nothing changed, every tenant after a full build), 22 device bytes of the current
+ * snapshot's MatchInfo table (0 until the first bfq_delivery_encode[_ordered] on it) */
 int32_t bfq_index_stats(bfq_index* h, int64_t* stats, int32_t n);
 /* device time of the tier-0 (lane-per-topic) match kernel of the latest completed match call on this handle, measured with
  * CUDA events recorded on the launching stream around the launch (for roofline accounting) */
@@ -207,7 +208,7 @@ void bfq_result_free(bfq_result* r);
  * whatever else runs on the handle. Several matches may be in flight on one handle (and one stream) at a time.
  *   bfq_device_result_release  blocks until the match and everything the library enqueued for the result since
  *                           (bfq_expand_device, bfq_expand_device_budget, bfq_fanout_device, bfq_delivery_device,
- *                           bfq_delivery_device_ordered, bfq_exchange_gather), on every stream it was used on, has finished; then the workspace goes back
+ *                           bfq_delivery_device_ordered, bfq_delivery_encode[_ordered], bfq_exchange_gather), on every stream it was used on, has finished; then the workspace goes back
  *                           to the handle's pool, where the next match may take it. The caller's own work that reads the
  *                           result's arrays (or the CSR and fan-out arrays that live in its workspace) must be ordered
  *                           before the release by the caller. */
@@ -441,6 +442,59 @@ int32_t bfq_delivery_device_ordered(const bfq_device_result* res, const int64_t*
                                     int64_t n_pairs, const int32_t* d_topic_tenant, const int64_t* d_pub_off,
                                     const int32_t* d_pub_hash, int64_t n_pubs, void* stream,
                                     bfq_delivery_ordered_result* out);
+
+/* ------------------------------------------------------------------------------------------------
+ * Delivery requests as wire bytes: a nesting of bfq_delivery_device or bfq_delivery_device_ordered encoded as one serialized
+ * DeliveryRequest per deliverer, the message BatchDeliveryCall.execute (bifromq-deliverer/.../BatchDeliveryCall.java:91-108)
+ * builds and sends. Deliverer d's request is d_out[d_req_off[d] .. d_req_off[d + 1]): DeliveryRequest.parseFrom takes the
+ * slice as it is, so no MatchInfo or DeliveryRequest is ever built per pair on the host. Proto3, field numbers of
+ * subbroker/type.proto, commontype/MatchInfo.proto, RouteMatcher.proto and TopicMessage.proto, every length a minimal varint:
+ *   DeliveryRequest   package = 3: one map entry per package of the deliverer, in the nesting's tenant order; both entry fields
+ *                     are written (key = 1: tenantId, the match's tenant list entry; value = 2: DeliveryPackage)
+ *   DeliveryPackage   pack = 1 per pack, in the nesting's order
+ *   DeliveryPack      messagePack = 2, then matchInfo = 3 per MatchInfo of the pack, in the nesting's order
+ *   TopicMessagePack  topic = 1 (the topic position's topic, omitted when empty), message = 2 per publisher pack: every publisher
+ *                     pack of the topic position for a whole pack, the sub-pack's own (d_pack_pub, in order) for an $oshare
+ *                     sub-pack (DeliverExecutorGroup.java:271-273)
+ *   MatchInfo         as NormalMatching / GroupMatching build it (DWS/cache/): matcher = 1 always; receiverId = 2 (the second
+ *                     NUL-separated part of the receiverUrl, ReceiverCache) omitted when empty; incarnation = 3 (varint: the
+ *                     normal route's 8-byte big-endian value, or the member's value in the stored RouteGroup) omitted when 0.
+ *                     A $share / $oshare member carries the GROUP's RouteMatcher.
+ *   RouteMatcher      as RouteDetailCache.get builds it from the route key: type = 1 omitted for Normal, 1 UnorderedShare,
+ *                     2 OrderedShare; filterLevel = 2 for every NUL-separated level of the escaped filter, empty levels included;
+ *                     group = 3 for shared routes only; mqttTopicFilter = 4 the unescaped filter, prefixed "$share/<group>/" or
+ *                     "$oshare/<group>/" for groups (omitted when empty).
+ * Inputs: the nesting (the latest delivery call on THIS result: one from another result, snapshot or an earlier call is
+ * BFQ_E_RANGE; bfq_delivery_encode takes bfq_delivery_device's, bfq_delivery_encode_ordered bfq_delivery_device_ordered's);
+ * the match's own tenant list (host) and topics (device, as the match took them); per topic position its publisher packs as
+ * serialized TopicMessagePack.PublisherPack bytes (device): d_pub_off[n_topics + 1] as for bfq_delivery_device_ordered, and
+ * pack q's bytes are d_pubpack_bytes[d_pubpack_off[q] .. d_pubpack_off[q + 1]).
+ * Sizing follows bfq_expand_device: d_req_off [n_deliverers + 1] is always written; the bytes are written only if n_bytes fits
+ * out_cap (d_out = NULL only sizes). The span of ordered_share_id is empty: its MatchInfos (member-less groups, and with
+ * bfq_delivery_encode every $oshare pair) are counted in n_skipped and never encoded. d_req_off lives in the result's leased
+ * workspace until bfq_device_result_release, which waits for the encode; the next encode on the result overwrites it. The
+ * first call on a snapshot builds and uploads its MatchInfo table (bfq_index_stats slot 22); other calls never need it. The
+ * call synchronises `stream` once (to read n_bytes) and returns while the write pass may still run.
+ * Errors: BFQ_E_INVALID for a NULL array, a tenant list of another length than the match's, or a d_pub_off / d_pubpack_off
+ * that does not start at 0 and never decrease or a publisher position outside it (checked on the device: nothing is
+ * written); BFQ_E_STATE for a match that has not completed; BFQ_E_RANGE for a nesting that is not the result's latest.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+    const int64_t* d_req_off;       /* [n_deliverers + 1]: deliverer d's DeliveryRequest = d_out[d_req_off[d] .. d_req_off[d + 1]) */
+    int64_t n_bytes;                /* = d_req_off[n_deliverers] */
+    int64_t n_match_infos;          /* MatchInfos encoded */
+    int64_t n_skipped;              /* MatchInfos left under ordered_share_id: never encoded */
+    int32_t n_deliverers, ordered_share_id;
+    uint64_t generation;
+} bfq_delivery_wire_result;
+int32_t bfq_delivery_encode(const bfq_device_result* res, const bfq_delivery_result* nesting, const uint8_t* tenants,
+                            const int64_t* tenant_off, int32_t n_tenants, const uint8_t* d_topics, const int64_t* d_topic_off,
+                            const int64_t* d_pub_off, const uint8_t* d_pubpack_bytes, const int64_t* d_pubpack_off, uint8_t* d_out,
+                            int64_t out_cap, void* stream, bfq_delivery_wire_result* out);
+int32_t bfq_delivery_encode_ordered(const bfq_device_result* res, const bfq_delivery_ordered_result* nesting, const uint8_t* tenants,
+                                    const int64_t* tenant_off, int32_t n_tenants, const uint8_t* d_topics, const int64_t* d_topic_off,
+                                    const int64_t* d_pub_off, const uint8_t* d_pubpack_bytes, const int64_t* d_pubpack_off,
+                                    uint8_t* d_out, int64_t out_cap, void* stream, bfq_delivery_wire_result* out);
 
 /* ------------------------------------------------------------------------------------------------
  * Multi-GPU: the one exchange step of the tenant-sharded path (SURVEY.md 8e). Tenants are independent key ranges, so
