@@ -479,6 +479,9 @@ int32_t enqueue_core(const CoreCtx& c, const SubBatch& sb, CoreOut* out) {
     cudaStream_t stream = c.stream;
     const int64_t n = sb.n, b = sb.begin;
     MatchParams p = core_params(c, sb);
+    // tier 0's 16-byte sector stores: every inline run and spill block starts on a 32-byte boundary
+    if ((reinterpret_cast<uintptr_t>(p.ranges) % (RANGE_SECTOR * sizeof(uint2))) != 0 || p.dyn_base % RANGE_SECTOR != 0)
+        return fail(BFQ_E_STATE, "internal error: tier-0 range region not sector-aligned");
     if (c.s->l2_window_bytes > 0) {
         cudaStreamAttrValue attr{};
         attr.accessPolicyWindow.base_ptr = c.s->d_tags.p;
@@ -1699,7 +1702,8 @@ int32_t bfq_match(bfq_index* h, const uint8_t* tenants, const int64_t* tenant_of
         if (rc != BFQ_OK) return rc;
         BFQ_CUDA_TRY(w->d_ranges_c.reserve(w->d_ranges.cap));
         const uint64_t dyn_total = w->d_ranges.cap - (uint64_t) n * INLINE_RANGES;
-        const uint64_t dyn_slice = dyn_total / (uint64_t) C, thr_slice = w->d_throttled.cap / (uint64_t) C;
+        // whole spill blocks per slice: tier 0 writes a spill block in 32-byte sectors, so it must start on one
+        const uint64_t dyn_slice = dyn_total / (uint64_t) C / SPILL_RANGES * SPILL_RANGES, thr_slice = w->d_throttled.cap / (uint64_t) C;
         size_t tmp_bytes = 0;
         {
             CompactParams q{};

@@ -279,8 +279,8 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32) match_topics_kernel(const 
 //   * per step a lane reads the 28 bytes at its current level start (up to three aligned 16-byte granules, word select +
 //     funnel shift), finds the '/' with a SWAR zero-byte test — the level table is filled lazily, there is no tokenising
 //     pre-pass —, issues the exact-child slot read (4 x LDG.128) and the '+' child payload read (2 x LDG.128) together and
-//     writes the discovered ranges straight to the INLINE_RANGES inline slots of the topic's position in the work order:
-//     no staging, no output atomics;
+//     writes the discovered ranges to the INLINE_RANGES inline slots of the topic's position in the work order, one whole
+//     32-byte sector at a time from registers: no shared-memory staging, no output atomics;
 //   * a lane that finishes takes the next topic at once (warp-uniform refill from 32-topic chunks claimed with
 //     one atomicAdd per chunk), so a straggler never idles the other 31 lanes (a warp that waits for its whole batch of 32
 //     runs with a third of its lanes active);
@@ -311,8 +311,12 @@ struct LaneSmem {
     int32_t c_ord;
 };
 
+// 7 resident CTAs per SM (what the shared memory allows, and what a batch below LARGE_BATCH_TOPICS runs with) need <= 72
+// registers per thread; left to itself the compiler takes 76-80 since the sector buffer below
+constexpr int L_MIN_CTAS_PER_SM = 7;
+
 template <bool kRootStep, bool kPrefetch, bool kNA>
-__global__ void __launch_bounds__(L_WARPS * 32) match_topics_lane_kernel(const MatchParams p) {
+__global__ void __launch_bounds__(L_WARPS * 32, L_MIN_CTAS_PER_SM) match_topics_lane_kernel(const MatchParams p) {
     __shared__ LaneSmem sm[L_WARPS];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     LaneSmem& ws = sm[wid];
@@ -330,7 +334,12 @@ __global__ void __launch_bounds__(L_WARPS * 32) match_topics_lane_kernel(const M
     // matched persistent / group routes so far; bit 31 = "a node's saturated count byte was seen" (then the true sum is
     // unknown but large: the topic is flagged unless the cap is INT_MAX). <= INLINE_RANGES * 254 otherwise.
     uint32_t acc_p = 0, acc_g = 0;
-    uint2* rg_out = nullptr;   // next inline range slot of the lane's topic
+    // The ranges are written a whole 32-byte sector (4 ranges) at a time: rg_out is the first slot of the topic's current sector,
+    // s0..s2 hold its first n_rg % 4 ranges. A sector written piecemeal over a walk is partial whenever L2 evicts it in between
+    // (C4: range stores cost tier 0 71 us that way, issuing them ~0; see DESIGN §4). The inline runs (RANGE_SECTOR-aligned: INLINE_RANGES per
+    // position) and the spill blocks (RANGE_SECTOR-aligned offsets, see capi.cu) start on sector boundaries.
+    uint2* rg_out = nullptr;
+    uint2 s0 = make_uint2(0u, 0u), s1 = s0, s2 = s0;
     int64_t my_off = 0;
     int len = 0, level = 0, tenant = 0;
 
@@ -341,11 +350,12 @@ __global__ void __launch_bounds__(L_WARPS * 32) match_topics_lane_kernel(const M
             if (n_rg == INLINE_RANGES) {
                 const unsigned long long at = p.dyn_base + atomicAdd(&p.counters[CTR_RANGES], (unsigned long long) SPILL_RANGES);
                 if (at + SPILL_RANGES <= p.ranges_cap) {
-                    uint2* dst = p.ranges + at;
-                    const uint2* src = rg_out - INLINE_RANGES;
+                    // INLINE_RANGES is a whole number of sectors: all of them are written, none is pending
+                    uint4* dst = reinterpret_cast<uint4*>(p.ranges + at);
+                    const uint4* src = reinterpret_cast<const uint4*>(rg_out - INLINE_RANGES);
 #pragma unroll
-                    for (int j = 0; j < (int) INLINE_RANGES; j++) dst[j] = src[j];
-                    rg_out = dst + INLINE_RANGES;
+                    for (int j = 0; j < (int) INLINE_RANGES / 2; j++) dst[j] = src[j];
+                    rg_out = p.ranges + at + INLINE_RANGES;
                 } else {
                     bad = true;   // no room: the host grows the region and re-runs the batch
                 }
@@ -353,7 +363,20 @@ __global__ void __launch_bounds__(L_WARPS * 32) match_topics_lane_kernel(const M
                 bad = true;
             }
         }
-        if (!bad) *rg_out++ = make_uint2(first, multi ? (count | RANGE_MULTI) : count);
+        if (!bad) {
+            const uint2 r = make_uint2(first, multi ? (count | RANGE_MULTI) : count);
+            switch (n_rg & (RANGE_SECTOR - 1)) {
+            case 0: s0 = r; break;
+            case 1: s1 = r; break;
+            case 2: s2 = r; break;
+            default: {
+                uint4* o = reinterpret_cast<uint4*>(rg_out);
+                o[0] = make_uint4(s0.x, s0.y, s1.x, s1.y);
+                o[1] = make_uint4(s2.x, s2.y, r.x, r.y);
+                rg_out += RANGE_SECTOR;
+            }
+            }
+        }
         n_rg++;
         acc_r += count;
         const uint32_t cp = caps & 0xFFu, cg = (caps >> 8) & 0xFFu;
@@ -386,7 +409,13 @@ __global__ void __launch_bounds__(L_WARPS * 32) match_topics_lane_kernel(const M
                 const bool flag_g = maxG != 0x7FFFFFFF && acc_g > (uint32_t) (maxG < 0 ? 0 : maxG);
                 flagged = flag_p || flag_g;
             }
-            put_span((uint32_t) ((rg_out - n_rg) - p.ranges),   // the inline slots, or the spill block
+            if (n_rg & (RANGE_SECTOR - 1)) {
+                // the last, partial sector, written whole: the slots past n_rg hold stale ranges no reader looks at
+                uint4* o = reinterpret_cast<uint4*>(rg_out);
+                o[0] = make_uint4(s0.x, s0.y, s1.x, s1.y);
+                o[1] = make_uint4(s2.x, s2.y, s2.x, s2.y);
+            }
+            put_span((uint32_t) ((rg_out - (n_rg & ~(RANGE_SECTOR - 1))) - p.ranges),   // the inline slots, or the spill block
                      n_rg | (flagged ? SPAN_FLAGGED : 0u), acc_r, 0u);
             if (flagged) {
                 const unsigned long long idx = atomicAdd(&p.counters[CTR_FLAGGED], 1ull);

@@ -219,6 +219,11 @@ void launch_caps(const CapsParams& p, cudaStream_t stream);
 
 constexpr uint32_t INLINE_RANGES = 12;   // tier 0 writes the ranges of the topic at work-order position i at ranges[i * INLINE_RANGES ...)
 constexpr uint32_t SPILL_RANGES = 64;    // ... and moves a topic with more of them, once, to a block of this many ranges
+// Tier 0 writes its ranges one whole 32-byte sector (two 16-byte stores) at a time, so the inline runs and the spill blocks
+// start on sector boundaries: ranges[0] is 256-byte aligned, INLINE_RANGES and SPILL_RANGES are multiples of RANGE_SECTOR, and
+// the host cuts the cursor-allocated region into sub-batch slices of whole spill blocks.
+constexpr uint32_t RANGE_SECTOR = 4;
+static_assert(INLINE_RANGES % RANGE_SECTOR == 0 && SPILL_RANGES % RANGE_SECTOR == 0, "tier 0 writes whole 32-byte sectors");
 
 // Compaction for the host path: gathers the sparse (inline + dynamic) ranges into one dense array in topic order.
 // d_scan_tmp / tmp_bytes: scratch for the exclusive scan (query the size with d_scan_tmp == nullptr).
