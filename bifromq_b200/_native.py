@@ -61,6 +61,17 @@ class BfqDeliveryWireResult(C.Structure):
                 ("n_deliverers", C.c_int32), ("ordered_share_id", C.c_int32), ("generation", C.c_uint64)]
 
 
+class BfqStaleMatch(C.Structure):
+    _fields_ = [("deliverer", C.c_int32), ("tenant", C.c_int32), ("rank", C.c_uint32), ("member", C.c_uint32),
+                ("reply_off", C.c_int64), ("reply_len", C.c_int32), ("code", C.c_int32)]
+
+
+class BfqDeliveryReplyResult(C.Structure):
+    _fields_ = [("d_pair_code", C.c_void_p), ("d_status", C.c_void_p), ("d_stale", C.c_void_p), ("n_code", C.c_int64 * 8),
+                ("n_pairs", C.c_int64), ("n_stale", C.c_int64), ("n_fallback", C.c_int32), ("n_deliverers", C.c_int32),
+                ("ordered_share_id", C.c_int32), ("generation", C.c_uint64)]
+
+
 class BfqBudgetResult(C.Structure):
     _fields_ = [("d_delivered_persistent", C.c_void_p), ("d_topic_flags", C.c_void_p), ("n_delivered", C.c_int64),
                 ("n_dropped_bytes", C.c_int64), ("n_dropped_persistent_bandwidth", C.c_int64),
@@ -115,6 +126,8 @@ _SIGNATURES = {
                                    _vp, _vp, _i64, _vp, C.POINTER(BfqDeliveryWireResult)]),
     "bfq_delivery_encode_ordered": (_i32, [C.POINTER(BfqDeviceResult), C.POINTER(BfqDeliveryOrderedResult), _vp, _vp, _i32, _vp,
                                            _vp, _vp, _vp, _vp, _vp, _i64, _vp, C.POINTER(BfqDeliveryWireResult)]),
+    "bfq_delivery_reply": (_i32, [C.POINTER(BfqDeviceResult), C.POINTER(BfqDeliveryResult), _vp, _vp, _i32, _vp, _vp, _vp,
+                                  C.POINTER(BfqDeliveryReplyResult)]),
     "bfq_exchange_unique_id": (_i32, [_vp, _i32]),
     "bfq_exchange_create": (_i32, [_i32, _i32, _i32, _vp, C.POINTER(_vp)]),
     "bfq_exchange_destroy": (None, [_vp]),

@@ -60,12 +60,14 @@ struct Snapshot {
         DeviceBuf<uint32_t> d_first;             // per rank: its first entry
         DeviceBuf<unsigned long long> d_off;     // [entries + 1]
         DeviceBuf<uint8_t> d_bytes;
+        size_t n_entries = 0;
         int64_t bytes() const { return (int64_t) (d_first.bytes() + d_off.bytes() + d_bytes.bytes()); }
     };
     std::mutex fan_mu;
     std::shared_ptr<FanTable> fan;
     std::shared_ptr<UrlTable> urls;
     std::shared_ptr<WireTable> wire;
+    std::shared_ptr<DeviceBuf<uint32_t>> mi_hash;   // per MatchInfo table entry, for bfq_delivery_reply: built on its first call
     std::atomic<int64_t> wire_bytes{0};      // wire->bytes() once built (bfq_index_stats reads it without fan_mu)
     std::vector<TenantHost> th;
     uint64_t garbage_slots = 0;   // slots of regions that delta commits replaced (reclaimed by the next full build)
@@ -156,6 +158,15 @@ struct Workspace {
     DeviceBuf<unsigned long long> d_wr_pos, d_wr_check;
     DeviceBuf<long long> d_req_off, d_wr_tenant_off;
     DeviceBuf<uint8_t> d_wr_tenants, d_wr_tmp;
+    // DeliveryReply join (bfq_delivery_reply): per deliverer, per map entry slot (one per package), per chunk, the key table,
+    // per pair, the stale lists, and the outputs
+    DeviceBuf<unsigned long long> d_rp_ctr, d_rp_chunk_base, d_rp_slot_key, d_rp_slot_rpos, d_rp_pkg_stale;
+    DeviceBuf<uint8_t> d_rp_dl_fail, d_rp_ent_bad, d_rp_tmp, d_rp_pair_code, d_rp_status, d_rp_tenants;
+    DeviceBuf<int32_t> d_rp_dl_code;
+    DeviceBuf<uint32_t> d_rp_u32;
+    DeviceBuf<long long> d_rp_ent, d_rp_chunks, d_rp_tenant_off;
+    DeviceBuf<bfq_stale_match> d_rp_stale;
+    PinnedBuf<unsigned long long> h_rp_ctr;
     // pinned result buffers
     PinnedBuf<uint32_t> h_span_begin, h_span_count, h_route_count;
     PinnedBuf<uint2> h_ranges;
@@ -2587,10 +2598,19 @@ int32_t ensure_wire_table(Snapshot* s, std::shared_ptr<Snapshot::WireTable>* out
     BFQ_CUDA_TRY(cudaMemcpy(wt->d_first.p, first.data(), first.size() * 4, cudaMemcpyHostToDevice));
     BFQ_CUDA_TRY(cudaMemcpy(wt->d_off.p, off.data(), off.size() * 8, cudaMemcpyHostToDevice));
     if (!blob.empty()) BFQ_CUDA_TRY(cudaMemcpy(wt->d_bytes.p, blob.data(), blob.size(), cudaMemcpyHostToDevice));
+    wt->n_entries = entries;
     s->wire = wt;
     s->wire_bytes = wt->bytes();
     *out = wt;
     return BFQ_OK;
+}
+
+// the nesting is the one the last delivery call on this result left in its workspace (plain or ordered)
+bool latest_nesting(const DeviceLease* L, const bfq_delivery_result* nest) {
+    const Workspace* w = L->ws;
+    return nest->generation == L->snap->generation && nest->d_package_off == (const int64_t*) w->d_package_off.p &&
+           nest->d_match_off == (const int64_t*) w->d_match_off.p && w->dl_n_packs >= 0 && nest->n_packs == w->dl_n_packs &&
+           nest->n_packages == w->dl_n_packages && nest->n_pairs == w->dl_n_pairs;
 }
 
 // bfq_delivery_encode (oout == nullptr) and bfq_delivery_encode_ordered: nest is the nesting's plain part either way
@@ -2611,10 +2631,7 @@ int32_t run_encode(const bfq_device_result* res, const bfq_delivery_result* nest
     if (n_tenants != L->ctx.n_tenants || (n_tenants > 0 && (!tenants || !tenant_off)))
         return fail(BFQ_E_INVALID, std::string(who) + ": the tenant list must be the match's (" + std::to_string(L->ctx.n_tenants) + " tenants)");
     Workspace* w = L->ws;
-    // the nesting must be the one the last delivery call on this result left in its workspace
-    if (nest->generation != L->snap->generation || nest->d_package_off != (const int64_t*) w->d_package_off.p ||
-        nest->d_match_off != (const int64_t*) w->d_match_off.p || w->dl_n_packs < 0 || nest->n_packs != w->dl_n_packs ||
-        nest->n_packages != w->dl_n_packages || nest->n_pairs != w->dl_n_pairs || w->dl_ordered != (onest != nullptr) ||
+    if (!latest_nesting(L, nest) || w->dl_ordered != (onest != nullptr) ||
         (onest && onest->d_pack_pub_off != (const int64_t*) w->d_pack_pub_off.p))
         return fail(BFQ_E_RANGE, std::string(who) + ": the nesting is not the latest " +
                                      (onest ? "bfq_delivery_device_ordered" : "bfq_delivery_device") + " result of this device result");
@@ -2704,6 +2721,162 @@ int32_t bfq_delivery_encode_ordered(const bfq_device_result* res, const bfq_deli
                                     uint8_t* d_out, int64_t out_cap, void* stream, bfq_delivery_wire_result* out) {
     return run_encode(res, nesting ? &nesting->d : nullptr, nesting, tenants, tenant_off, n_tenants, d_topics, d_topic_off, d_pub_off,
                       d_pubpack_bytes, d_pubpack_off, d_out, out_cap, stream, "bfq_delivery_encode_ordered", out);
+}
+
+namespace {
+// the hash of every MatchInfo in the snapshot's table (bfq_delivery_reply's join key), built once per snapshot on `st`
+int32_t ensure_mi_hash(Snapshot* s, const Snapshot::WireTable& wt, cudaStream_t st, std::shared_ptr<DeviceBuf<uint32_t>>* out) {
+    std::lock_guard<std::mutex> g(s->fan_mu);
+    if (!s->mi_hash) {
+        auto hb = std::make_shared<DeviceBuf<uint32_t>>();
+        BFQ_CUDA_TRY(hb->reserve(std::max<size_t>(wt.n_entries, 1)));
+        BFQ_CUDA_TRY(launch_mi_hash(wt.d_bytes.p, wt.d_off.p, (int64_t) wt.n_entries, hb->p, st));
+        BFQ_CUDA_TRY(cudaStreamSynchronize(st));   // other streams read it from now on
+        s->mi_hash = hb;
+    }
+    *out = s->mi_hash;
+    return BFQ_OK;
+}
+}  // namespace
+
+int32_t bfq_delivery_reply(const bfq_device_result* res, const bfq_delivery_result* nest, const uint8_t* tenants,
+                           const int64_t* tenant_off, int32_t n_tenants, const uint8_t* d_reply, const int64_t* d_reply_off,
+                           void* stream, bfq_delivery_reply_result* out) {
+    const char* who = "bfq_delivery_reply";
+    if (!res || !res->lease || !nest || !out) return fail(BFQ_E_INVALID, "bad argument");
+    auto* L = static_cast<DeviceLease*>(res->lease);
+    cudaStream_t st = (cudaStream_t) stream;
+    cudaEvent_t ev = nullptr;
+    int32_t rc = lease_use(res, st, who, &ev);
+    if (rc != BFQ_OK) return rc;
+    RecordOnExit rec(ev, st);
+    if (!d_reply || !d_reply_off) return fail(BFQ_E_INVALID, std::string(who) + ": NULL reply array");
+    if (n_tenants != L->ctx.n_tenants || (n_tenants > 0 && (!tenants || !tenant_off)))
+        return fail(BFQ_E_INVALID, std::string(who) + ": the tenant list must be the match's (" + std::to_string(L->ctx.n_tenants) + " tenants)");
+    if (!latest_nesting(L, nest))
+        return fail(BFQ_E_RANGE, std::string(who) + ": the nesting is not the latest delivery nesting of this device result");
+    bfq_index* h = L->h;
+    Workspace* w = L->ws;
+    std::shared_ptr<Snapshot::WireTable> wt;
+    if ((rc = ensure_wire_table(L->snap.get(), &wt)) != BFQ_OK) return rc;
+    std::shared_ptr<DeviceBuf<uint32_t>> mh;
+    if ((rc = ensure_mi_hash(L->snap.get(), *wt, st, &mh)) != BFQ_OK) return rc;
+    const int64_t np = nest->n_pairs, nk = nest->n_packs, ng = nest->n_packages;
+    const uint32_t D = (uint32_t) nest->n_deliverers;
+    if (np >= (int64_t) 1 << 31) return fail(BFQ_E_RANGE, std::string(who) + ": 2^31 or more pairs in one nesting");
+    uint64_t T = 2;
+    while (T < 2 * (uint64_t) np) T <<= 1;
+    const int64_t cap = std::max<int64_t>(np, 1), G = std::max<int64_t>(ng, 1);
+    const uint64_t nch = RP_MAX_CHUNKS + (uint64_t) ng;
+    BFQ_CUDA_TRY(w->d_rp_ctr.reserve(RP_CTR_N));
+    BFQ_CUDA_TRY(w->h_rp_ctr.reserve(RP_CTR_N));
+    BFQ_CUDA_TRY(w->d_rp_chunk_base.reserve((size_t) ng + 1));
+    BFQ_CUDA_TRY(w->d_rp_slot_key.reserve(T));
+    BFQ_CUDA_TRY(w->d_rp_slot_rpos.reserve(T));
+    BFQ_CUDA_TRY(w->d_rp_pkg_stale.reserve(2 * ((size_t) ng + 1)));
+    BFQ_CUDA_TRY(w->d_rp_dl_fail.reserve(D));
+    BFQ_CUDA_TRY(w->d_rp_ent_bad.reserve((size_t) G));
+    BFQ_CUDA_TRY(w->d_rp_pair_code.reserve((size_t) cap));
+    BFQ_CUDA_TRY(w->d_rp_status.reserve(D));
+    BFQ_CUDA_TRY(w->d_rp_dl_code.reserve(D));
+    BFQ_CUDA_TRY(w->d_rp_u32.reserve((size_t) D + 2 * (size_t) G + 3 * T + (size_t) cap * 6));
+    BFQ_CUDA_TRY(w->d_rp_ent.reserve(4 * (size_t) G));
+    BFQ_CUDA_TRY(w->d_rp_chunks.reserve(3 * nch));
+    BFQ_CUDA_TRY(w->d_rp_stale.reserve((size_t) cap));
+    BFQ_CUDA_TRY(w->d_rp_tenant_off.reserve((size_t) n_tenants + 1));
+    const int64_t tbytes = n_tenants > 0 ? tenant_off[n_tenants] : 0;
+    BFQ_CUDA_TRY(w->d_rp_tenants.reserve((size_t) std::max<int64_t>(tbytes, 1)));
+    if (n_tenants > 0) {
+        BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_rp_tenant_off.p, tenant_off, ((size_t) n_tenants + 1) * 8, cudaMemcpyHostToDevice, st));
+        if (tbytes > 0) BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_rp_tenants.p, tenants, (size_t) tbytes, cudaMemcpyHostToDevice, st));
+    }
+    ReplyParams p{};
+    p.n_packages = ng;
+    p.n_packs = nk;
+    p.n_pairs = np;
+    p.n_deliverers = D;
+    p.package_off = (const long long*) nest->d_package_off;
+    p.package_tenant = nest->d_package_tenant;
+    p.pack_off = (const long long*) nest->d_pack_off;
+    p.match_off = (const long long*) nest->d_match_off;
+    p.match_rank = nest->d_match_rank;
+    p.match_member = nest->d_match_member;
+    p.tenants = w->d_rp_tenants.p;
+    p.tenant_off = w->d_rp_tenant_off.p;
+    p.mi_first = wt->d_first.p;
+    p.mi_off = wt->d_off.p;
+    p.mi_bytes = wt->d_bytes.p;
+    p.mi_hash = mh->p;
+    p.reply = d_reply;
+    p.reply_off = (const long long*) d_reply_off;
+    p.ctr = w->d_rp_ctr.p;
+    p.dl_fail = w->d_rp_dl_fail.p;
+    p.dl_code = w->d_rp_dl_code.p;
+    uint32_t* u = w->d_rp_u32.p;
+    p.dl_entries = u;
+    u += D;
+    p.ent_pkg = u;
+    u += G;
+    p.pkg_claimed = u;
+    u += G;
+    p.slot_pair = u;
+    u += T;
+    p.slot_code = u;
+    u += T;
+    p.slot_rlen = u;
+    u += T;
+    p.pair_slot = u;
+    u += cap;
+    p.stale_list = u;
+    u += cap;
+    p.sort_key_in = u;
+    u += cap;
+    p.sort_key_out = u;
+    u += cap;
+    p.sort_val_in = u;
+    u += cap;
+    p.sort_val_out = u;
+    p.ent_s = w->d_rp_ent.p;
+    p.ent_e = p.ent_s + G;
+    p.ent_vs = p.ent_e + G;
+    p.ent_ve = p.ent_vs + G;
+    p.ent_bad = w->d_rp_ent_bad.p;
+    p.chunk_base = w->d_rp_chunk_base.p;
+    p.ch_guess = w->d_rp_chunks.p;
+    p.ch_exit = p.ch_guess + nch;
+    p.ch_start = p.ch_exit + nch;
+    p.slot_key = w->d_rp_slot_key.p;
+    p.slot_rpos = w->d_rp_slot_rpos.p;
+    p.table_mask = T - 1;
+    p.pkg_stale = w->d_rp_pkg_stale.p;
+    p.pkg_cursor = p.pkg_stale + ng + 1;
+    p.stale_cap = cap;
+    p.pair_code = w->d_rp_pair_code.p;
+    p.status = w->d_rp_status.p;
+    p.stale = w->d_rp_stale.p;
+    size_t tmp_bytes = 0;
+    BFQ_CUDA_TRY(launch_reply(p, nullptr, &tmp_bytes, st));
+    BFQ_CUDA_TRY(w->d_rp_tmp.reserve(tmp_bytes + 256));
+    BFQ_CUDA_TRY(launch_reply(p, w->d_rp_tmp.p, &tmp_bytes, st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(w->h_rp_ctr.p, w->d_rp_ctr.p, RP_CTR_N * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
+    {
+        std::lock_guard<std::mutex> g(h->mu);
+        h->launches += 17;
+    }
+    const unsigned long long* c = w->h_rp_ctr.p;
+    if (c[RP_BAD_OFF]) return fail(BFQ_E_INVALID, std::string(who) + ": d_reply_off must never decrease");
+    out->d_pair_code = w->d_rp_pair_code.p;
+    out->d_status = w->d_rp_status.p;
+    out->d_stale = w->d_rp_stale.p;
+    for (int i = 0; i < 8; i++) out->n_code[i] = (int64_t) c[RP_N_CODE + i];
+    out->n_pairs = np;
+    out->n_stale = (int64_t) c[RP_N_STALE];
+    out->n_fallback = (int32_t) c[RP_N_FALLBACK];
+    out->n_deliverers = (int32_t) D;
+    out->ordered_share_id = (int32_t) D - 1;
+    out->generation = L->snap->generation;
+    return BFQ_OK;
 }
 
 int32_t bfq_fanout_deliverer(bfq_index* h, int32_t id, int32_t* sub_broker_id, uint8_t* key_out, int64_t key_cap, int64_t* key_len) {

@@ -9,6 +9,7 @@
 #include <utility>
 #include <vector>
 
+#include "../../include/bfq_gpumatch.h"
 #include "codec.h"
 #include "index_builder.h"
 
@@ -194,5 +195,62 @@ struct WireParams {
 cudaError_t launch_wire_size(const WireParams& p, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream);
 // pass 2: the bytes (after pass 1 and a total that fits the caller's buffer)
 cudaError_t launch_wire_write(const WireParams& p, cudaStream_t stream);
+
+// bfq_delivery_reply: every deliverer's DeliveryReply joined back to the pairs of a nesting (delivery_reply.cu)
+enum { RP_BAD_OFF = 0, RP_VALUE_BYTES = 1, RP_N_FALLBACK = 2, RP_N_STALE = 3, RP_N_CODE = 4, RP_CTR_N = 12 };
+enum { RP_NO_RESULT = 5, RP_NOT_SENT = 6, RP_UNDECIDED = 7 };
+// DeliveryResults spans are cut into chunks of RP_CHUNK_MIN bytes, or more when the replies' results exceed RP_MAX_CHUNKS of them
+constexpr long long RP_CHUNK_MIN = 2048;
+constexpr unsigned long long RP_MAX_CHUNKS = 1ull << 20;
+struct ReplyParams {
+    // the nesting
+    int64_t n_packages, n_packs, n_pairs;
+    uint32_t n_deliverers;               // the last id is ordered_share_id: its pairs were never sent
+    const long long* package_off;        // [n_deliverers + 1]
+    const uint32_t* package_tenant;      // [n_packages]
+    const long long* pack_off;           // [n_packages + 1]
+    const long long* match_off;          // [n_packs + 1]
+    const uint32_t* match_rank;          // [n_pairs]
+    const uint32_t* match_member;        // [n_pairs]
+    // device copy of the match's tenant list
+    const uint8_t* tenants;
+    const long long* tenant_off;         // [n_tenants + 1]
+    // the snapshot's MatchInfo table and the hash of every entry's MatchInfo
+    const uint32_t* mi_first;
+    const unsigned long long* mi_off;
+    const uint8_t* mi_bytes;
+    const uint32_t* mi_hash;
+    // the replies
+    const uint8_t* reply;
+    const long long* reply_off;          // [n_deliverers + 1]
+    // scratch
+    unsigned long long* ctr;             // [RP_CTR_N]
+    uint8_t* dl_fail;                    // per deliverer
+    int32_t* dl_code;                    // per deliverer: the reply code
+    uint32_t* dl_entries;                // per deliverer: its map entries, at slots package_off[d] ..
+    long long *ent_s, *ent_e;            // per entry slot [n_packages]: the map entry's bytes
+    long long *ent_vs, *ent_ve;          // its DeliveryResults bytes
+    uint32_t* ent_pkg;                   // the package its tenant key names
+    uint8_t* ent_bad;                    // its results could not be walked
+    uint32_t* pkg_claimed;               // per package: a map entry named it
+    unsigned long long* chunk_base;      // [n_packages + 1] chunks per entry slot, scanned
+    long long *ch_guess, *ch_exit, *ch_start;   // per chunk [RP_MAX_CHUNKS + n_packages]
+    unsigned long long* slot_key;        // [table_mask + 1]: package << 32 | MatchInfo entry, ~0 empty
+    uint32_t *slot_pair, *slot_code, *slot_rlen;
+    unsigned long long* slot_rpos;
+    uint64_t table_mask;
+    uint32_t* pair_slot;                 // [n_pairs]
+    unsigned long long *pkg_stale, *pkg_cursor;   // [n_packages + 1]
+    uint32_t *stale_list, *sort_key_in, *sort_key_out, *sort_val_in, *sort_val_out;   // [stale_cap]
+    int64_t stale_cap;
+    // outputs
+    uint8_t* pair_code;                  // [n_pairs]
+    uint8_t* status;                     // [n_deliverers]
+    bfq_stale_match* stale;              // [stale_cap]
+};
+// the MatchInfo hash of every table entry (once per snapshot)
+cudaError_t launch_mi_hash(const uint8_t* bytes, const unsigned long long* off, int64_t n_entries, uint32_t* out, cudaStream_t stream);
+// every stage of the join; d_tmp == nullptr: query the scan / sort scratch size
+cudaError_t launch_reply(const ReplyParams& p, void* d_tmp, size_t* tmp_bytes, cudaStream_t stream);
 
 }  // namespace bfq

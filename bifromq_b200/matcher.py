@@ -256,6 +256,17 @@ class DeviceResult:
             N.check(N.lib.bfq_delivery_encode(C.byref(self.raw), C.byref(nesting.raw), *args))
         return out
 
+    def delivery_reply(self, nesting, tenants, d_reply_ptr, d_reply_off_ptr, stream=0):
+        """bfq_delivery_reply: every deliverer's serialized DeliveryReply (device bytes; deliverer d's is
+        reply[reply_off[d] .. reply_off[d + 1]), int64 offsets) joined back to the pairs of `nesting` (the latest delivery() or
+        delivery_ordered() of this result, the one its requests were encoded from). tenants: the match's tenant list.
+        -> BfqDeliveryReplyResult: d_pair_code per pair, d_status per deliverer, d_stale (BfqStaleMatch) per stale MatchInfo"""
+        tb, toff, nt = GpuRouteIndex._tenants(tenants)
+        out = N.BfqDeliveryReplyResult()
+        N.check(N.lib.bfq_delivery_reply(C.byref(self.raw), C.byref(nesting.raw), N.ptr(tb), N.ptr(toff), nt, d_reply_ptr,
+                                         d_reply_off_ptr, stream, C.byref(out)))
+        return out
+
     def release(self):
         if getattr(self, "raw", None) is not None and self.raw.lease:
             N.lib.bfq_device_result_release(C.byref(self.raw))

@@ -208,7 +208,7 @@ void bfq_result_free(bfq_result* r);
  * whatever else runs on the handle. Several matches may be in flight on one handle (and one stream) at a time.
  *   bfq_device_result_release  blocks until the match and everything the library enqueued for the result since
  *                           (bfq_expand_device, bfq_expand_device_budget, bfq_fanout_device, bfq_delivery_device,
- *                           bfq_delivery_device_ordered, bfq_delivery_encode[_ordered], bfq_exchange_gather), on every stream it was used on, has finished; then the workspace goes back
+ *                           bfq_delivery_device_ordered, bfq_delivery_encode[_ordered], bfq_delivery_reply, bfq_exchange_gather), on every stream it was used on, has finished; then the workspace goes back
  *                           to the handle's pool, where the next match may take it. The caller's own work that reads the
  *                           result's arrays (or the CSR and fan-out arrays that live in its workspace) must be ordered
  *                           before the release by the caller. */
@@ -495,6 +495,72 @@ int32_t bfq_delivery_encode_ordered(const bfq_device_result* res, const bfq_deli
                                     const int64_t* tenant_off, int32_t n_tenants, const uint8_t* d_topics, const int64_t* d_topic_off,
                                     const int64_t* d_pub_off, const uint8_t* d_pubpack_bytes, const int64_t* d_pubpack_off,
                                     uint8_t* d_out, int64_t out_cap, void* stream, bfq_delivery_wire_result* out);
+
+/* ------------------------------------------------------------------------------------------------
+ * Delivery replies: every deliverer's serialized DeliveryReply joined back to the pairs of its request, as the reply branch
+ * of BatchDeliveryCall.execute (bifromq-deliverer/.../BatchDeliveryCall.java:108-172) with TypeUtil.toMap does it, so the
+ * host never builds a MatchInfo per pair to key the join. subbroker/type.proto:41-63:
+ *   DeliveryReply     code = 1 (0 OK, 1 BACK_PRESSURE_REJECTED, 2 ERROR); result = 2: map<tenantId, DeliveryResults>
+ *   DeliveryResults   result = 1: repeated DeliveryResult
+ *   DeliveryResult    matchInfo = 1; code = 2 (0 OK, 1 NO_SUB, 2 NO_RECEIVER)
+ * Inputs: `nesting` is the latest delivery nesting of this result, the one bfq_delivery_encode[_ordered] encodes (for an ordered
+ * nesting pass &ordered.d; an $oshare sub-pack's MatchInfo is its (rank, winning member)); anything else is BFQ_E_RANGE. The
+ * match's own tenant list (host). Deliverer d's reply is d_reply[d_reply_off[d] .. d_reply_off[d + 1]) (device; the offsets
+ * never decrease and need not start at 0): a failed call is the bytes 08 02 (the ERROR reply `.exceptionally` makes), an empty
+ * slice a default reply (OK, no results). The slices of deliverers with an empty request (ordered_share_id among them) are
+ * never read.
+ * A deliverer is decided on the device only when its answer is certainly the reference's: its reply is well-formed protobuf
+ * (known fields in any order; unknown fields of wire types 0, 1, 2 and 5 skipped at every level), every DeliveryResult's
+ * matchInfo equals, byte for byte, a MatchInfo the deliverer's request carries under that map entry's tenant (the encode's
+ * canonical bytes; for these messages canonical bytes are equal exactly when the messages are), and no MatchInfo appears
+ * twice under a tenant (where toMap throws). A singular field or a tenant key given twice, a tenant key that is not valid
+ * UTF-8 or not in the request, a MatchInfo that does not resolve (a non-canonical encoding of a requested one included),
+ * truncated bytes or a wrong wire type on a known field make it FALLBACK instead: the host runs execute's loop on its request
+ * and reply slices. Sub-brokers that echo the request's MatchInfo objects (LocalDistService.dist, DeliveryPipeline.deliver)
+ * never cause it. Other deliverers of the call are unaffected.
+ * Outputs (device arrays in the result's leased workspace until bfq_device_result_release, which waits for this call; the next
+ * call on the result overwrites them):
+ *   d_pair_code[nesting->n_pairs]  per pair of the nesting (aligned with d_match_rank / d_match_member), DeliveryCallResult:
+ *                           0 OK, 1 NO_SUB, 2 NO_RECEIVER, 3 BACK_PRESSURE_REJECTED, 4 ERROR (also a DeliveryResult code
+ *                           outside 0-2, which is not stale), and 5 NO_RESULT (no result for it: the reference completes it OK
+ *                           and logs "No deliver result"), 6 NOT_SENT (the pairs under ordered_share_id), 7 UNDECIDED (its
+ *                           deliverer is FALLBACK)
+ *   d_status[n_deliverers]  0 OK, 3 BACK_PRESSURE_REJECTED, 4 ERROR (the reply code is ERROR or any value but 0 and 1),
+ *                           6 NOT_SENT (an empty request), 7 FALLBACK
+ *   d_stale[n_stale]        execute's staleMatchInfos: one entry per distinct (deliverer, tenant index, rank, member) whose code
+ *                           is NO_SUB or NO_RECEIVER, sorted by those four fields, with the offset and length of its MatchInfo
+ *                           in d_reply (MatchInfo.parseFrom of those bytes gives removeRoute's matcher, receiverId and
+ *                           incarnation; delivererKey and subBrokerId come from bfq_fanout_deliverer)
+ * The plain and the ordered nesting share the result's buffers and the nesting struct does not say which call made it: a
+ * bfq_delivery_result copied before a later delivery call whose counts happen to equal it is taken for that later nesting, so
+ * pass the struct of the latest call (it is what the requests were encoded from).
+ * The first call on a snapshot also hashes its MatchInfo table (uploading the table first if no encode did). Workspace: the
+ * key table has a power of two of at least 2 * nesting->n_pairs slots of 28 bytes, and the per-pair and stale arrays take
+ * about 60 bytes per pair (all sized from n_pairs, an upper bound on the distinct keys, because the count is only known on the
+ * device); about 3 GB at 23.6 M pairs, kept by the workspace for its next calls. The call synchronises `stream` once, to read
+ * the counts.
+ * Errors: BFQ_E_INVALID for a NULL array, a tenant list of another length than the match's, or a decreasing d_reply_off
+ * (checked on the device: nothing is written); BFQ_E_STATE for a match that has not completed; BFQ_E_RANGE for a nesting that
+ * is not the result's latest.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct {
+    int32_t deliverer, tenant;      /* deliverer id; tenant index in the match's list */
+    uint32_t rank, member;          /* as in d_match_rank / d_match_member */
+    int64_t reply_off;              /* the MatchInfo message: d_reply[reply_off .. reply_off + reply_len) */
+    int32_t reply_len, code;        /* code: 1 NO_SUB or 2 NO_RECEIVER */
+} bfq_stale_match;
+typedef struct {
+    const uint8_t* d_pair_code;     /* [n_pairs] */
+    const uint8_t* d_status;        /* [n_deliverers] */
+    const bfq_stale_match* d_stale; /* [n_stale] */
+    int64_t n_code[8];              /* pairs per code of d_pair_code */
+    int64_t n_pairs, n_stale;
+    int32_t n_fallback, n_deliverers, ordered_share_id;
+    uint64_t generation;
+} bfq_delivery_reply_result;
+int32_t bfq_delivery_reply(const bfq_device_result* res, const bfq_delivery_result* nesting, const uint8_t* tenants,
+                           const int64_t* tenant_off, int32_t n_tenants, const uint8_t* d_reply, const int64_t* d_reply_off,
+                           void* stream, bfq_delivery_reply_result* out);
 
 /* ------------------------------------------------------------------------------------------------
  * Multi-GPU: the one exchange step of the tenant-sharded path (SURVEY.md 8e). Tenants are independent key ranges, so
