@@ -17,201 +17,11 @@
 #include "codec.h"
 #include "cuda_buf.h"
 #include "index_builder.h"
+#include "index_state.h"
 #include "fanout.h"
-#include "lease.h"
 #include "match_kernels.cuh"
 
 using namespace bfq;
-
-// ------------------------------------------------------------------------------------------------ snapshots
-// One committed state of the index: device arrays + the host-side tables results are resolved against (segment table,
-// route kinds, raw KV). Immutable once published and reference counted: every match pins the snapshot it ran on, so a
-// result's ranks always resolve against the KV order they were produced from, whatever is committed meanwhile.
-struct Snapshot {
-    int device = 0;
-    uint64_t generation = 0;
-    DeviceBuf<Slot> d_slots, d_roots;
-    DeviceBuf<uint32_t> d_segs, d_pfxP, d_pfxG;
-    DeviceBuf<uint8_t> d_rkind, d_tags;
-    FlatIndex flat;          // host copy (segs / tenant map / tenant table / statistics; the uploaded arrays are dropped)
-    // per tenant, aligned with flat.tenants (key order): the committed KV (route lookups; shared with the staging area and
-    // with the neighbouring snapshots, a delta commit replaces only the touched tenants') and the route kinds
-    struct TenantHost {
-        std::shared_ptr<const KVBlob> kv;
-        std::shared_ptr<const std::vector<uint8_t>> rkind;
-        std::shared_ptr<const TenantFan> fan;   // routes -> deliverer ids, built on the first fan-out that sees this blob
-        std::shared_ptr<const TenantWire> wire; // routes -> MatchInfo bytes, built on the first encode that sees this blob
-    };
-    // fan-out tables of the whole snapshot (device), assembled from the tenants' on first use
-    struct FanTable {
-        DeviceBuf<uint32_t> d_rdeliv, d_gmem_off, d_gmem_deliv;
-        DeviceBuf<uint8_t> d_gordered;
-        uint32_t n_deliverers = 0;   // incl. the reserved last id (ordered shared subscriptions)
-    };
-    // receiverUrls of the ordered groups' members (device), for the $oshare pick: built on the first ordered delivery call
-    struct UrlTable {
-        DeviceBuf<unsigned long long> d_words;   // member m: its url at byte 4 of words d_word[m] .., zero-padded
-        DeviceBuf<long long> d_word;             // [members of the fan table]
-        DeviceBuf<uint32_t> d_len;
-        uint32_t member_bits = 1;                // bits of the largest ordered group's size
-    };
-    // every route's MatchInfo bytes (device), for bfq_delivery_encode: built on the first encode call
-    struct WireTable {
-        DeviceBuf<uint32_t> d_first;             // per rank: its first entry
-        DeviceBuf<unsigned long long> d_off;     // [entries + 1]
-        DeviceBuf<uint8_t> d_bytes;
-        size_t n_entries = 0;
-        int64_t bytes() const { return (int64_t) (d_first.bytes() + d_off.bytes() + d_bytes.bytes()); }
-    };
-    std::mutex fan_mu;
-    std::shared_ptr<FanTable> fan;
-    std::shared_ptr<UrlTable> urls;
-    std::shared_ptr<WireTable> wire;
-    std::shared_ptr<DeviceBuf<uint32_t>> mi_hash;   // per MatchInfo table entry, for bfq_delivery_reply: built on its first call
-    std::atomic<int64_t> wire_bytes{0};      // wire->bytes() once built (bfq_index_stats reads it without fan_mu)
-    std::vector<TenantHost> th;
-    uint64_t garbage_slots = 0;   // slots of regions that delta commits replaced (reclaimed by the next full build)
-    int64_t delta_commits = 0;    // delta commits since the last full build
-    size_t l2_window_bytes = 0;
-    // rank -> (index into flat.tenants, rank inside the tenant); false if out of range
-    bool locate(int64_t rank, size_t* ti, int64_t* local) const {
-        if (rank < 0 || rank >= flat.n_routes || flat.tenants.empty()) return false;
-        size_t lo = 0, hi = flat.tenants.size();
-        while (hi - lo > 1) {
-            const size_t mid = (lo + hi) / 2;
-            if (flat.tenants[mid].lo <= rank) lo = mid;
-            else hi = mid;
-        }
-        *ti = lo;
-        *local = rank - flat.tenants[lo].lo;
-        return *local < flat.tenants[lo].n_routes;
-    }
-    int64_t device_bytes() const {
-        return (int64_t) (d_slots.bytes() + d_tags.bytes() + d_roots.bytes() + d_segs.bytes() + d_rkind.bytes() + d_pfxP.bytes() + d_pfxG.bytes());
-    }
-    ~Snapshot() { cudaSetDevice(device); }   // runs before the members are destroyed: the buffers are freed on this device
-};
-
-constexpr int MAX_CHUNKS = 8;
-
-// Everything ONE match in flight needs: streams, device scratch, pinned result buffers. A workspace is leased from the
-// index's pool for the duration of a call AND of the result it produced (the result's arrays live in it), so concurrent
-// matches on one handle never share a buffer. Returned to the pool by bfq_result_free / bfq_device_result_release.
-struct Workspace {
-    int device = 0;
-    cudaStream_t stream = nullptr, copy_stream = nullptr, work_stream[2] = {nullptr, nullptr};
-    cudaEvent_t ev[2] = {nullptr, nullptr};
-    cudaEvent_t ev_h2d[MAX_CHUNKS] = {};
-    cudaEvent_t evk[2] = {nullptr, nullptr};
-    cudaEvent_t ev_done = nullptr;   // device path: recorded behind the last thing a match enqueued (what wait() waits for)
-    std::vector<cudaEvent_t> ev_use; // device path: one per stream the result was used on after the match (lease.h), created on demand
-    // resolved tenant table of the previous call on this workspace (reused when the same list comes again)
-    uint64_t tab_generation = ~0ull;
-    std::vector<uint8_t> tab_blob;
-    std::vector<int64_t> tab_off;
-    std::vector<int32_t> tab_caps;
-    int32_t tab_n = -1;
-    bool any_cap = true;
-    DeviceBuf<int32_t> d_tenant_tab;   // root | maxP | maxG, 3 x n_tenants
-    PinnedBuf<int32_t> h_tenant_tab;
-    // per-call device buffers
-    DeviceBuf<uint8_t> d_topics;
-    DeviceBuf<int64_t> d_topic_off;
-    DeviceBuf<int32_t> d_topic_tenant;
-    DeviceBuf<uint32_t> d_span_begin, d_span_count, d_route_count, d_overflow, d_flagged, d_kept, d_defer;
-    DeviceBuf<uint2> d_ranges, d_scratch, d_ranges_c;
-    DeviceBuf<uint8_t> d_scan_tmp;
-    DeviceBuf<uint32_t> d_cnt, d_new_begin, d_final_begin, d_final_count;
-    // locality order + dedup (launch_order): per compute-stream slot (two sub-batches can be in flight)
-    DeviceBuf<uint32_t> d_ord_keys, d_leader, d_order;
-    DeviceBuf<SpanRecord> d_pos_rec;            // tier 0's span record per work-order position (MatchParams::pos_rec)
-    DeviceBuf<unsigned long long> d_hash_tab;   // 2 x hash_stride
-    DeviceBuf<uint32_t> d_hist;                 // 2 x hist_stride (launch_order's scratch)
-    size_t hash_stride = 0, hist_stride = 0;
-    DeviceBuf<uint3> d_throttled;
-    DeviceBuf<unsigned long long> d_counters;
-    PinnedBuf<unsigned long long> h_counters;
-    DeviceBuf<unsigned long long> d_exp_counts;
-    // delivery budgets (bfq_expand_device_budget)
-    DeviceBuf<long long> d_bud_bytes;
-    DeviceBuf<uint8_t> d_bud_bw, d_bud_flags;
-    DeviceBuf<uint32_t> d_bud_dp, d_bud_list;
-    DeviceBuf<unsigned long long> d_bud_ctr;
-    // fan-out expansion (fanout.cu)
-    DeviceBuf<uint32_t> d_fo_counts, d_fo_base, d_pack_topic, d_pack_rank, d_pack_member;
-    DeviceBuf<long long> d_pack_offsets;
-    DeviceBuf<uint8_t> d_fo_tmp;
-    // delivery nesting (fanout.cu: launch_delivery): scratch per topic (6 words each + 2) and per pair (10 words each + 2), the outputs
-    DeviceBuf<uint32_t> d_dl_topic_tmp, d_dl_pair_tmp, d_dl_pcount, d_package_tenant, d_dl_pack_topic, d_match_rank, d_match_member;
-    DeviceBuf<unsigned long long> d_dl_totals;
-    DeviceBuf<long long> d_package_off, d_dl_pack_off, d_match_off;
-    DeviceBuf<uint8_t> d_dl_tmp;
-    // $oshare resolution (bfq_delivery_device_ordered): per CSR pair flags and item counts, the check words, the sort keys of
-    // pairs and items, the per-item / per-emit-position words, and the publisher outputs
-    DeviceBuf<uint32_t> d_os_flag, d_os_u32, d_pack_pub;
-    DeviceBuf<unsigned long long> d_os_items, d_os_check, d_os_key;
-    DeviceBuf<long long> d_pack_pub_off;
-    // the nesting the last delivery call left in the buffers above (n_packs < 0: none, or a call that failed)
-    int64_t dl_n_pairs = -1, dl_n_packages = -1, dl_n_packs = -1;
-    bool dl_ordered = false;
-    // DeliveryRequest encoding (bfq_delivery_encode): the size scans (pairs, packs, packages), the checks, the offsets
-    DeviceBuf<unsigned long long> d_wr_pos, d_wr_check;
-    DeviceBuf<long long> d_req_off, d_wr_tenant_off;
-    DeviceBuf<uint8_t> d_wr_tenants, d_wr_tmp;
-    // DeliveryReply join (bfq_delivery_reply): per deliverer, per map entry slot (one per package), per chunk, the key table,
-    // per pair, the stale lists, and the outputs
-    DeviceBuf<unsigned long long> d_rp_ctr, d_rp_chunk_base, d_rp_slot_key, d_rp_slot_rpos, d_rp_pkg_stale;
-    DeviceBuf<uint8_t> d_rp_dl_fail, d_rp_ent_bad, d_rp_tmp, d_rp_pair_code, d_rp_status, d_rp_tenants;
-    DeviceBuf<int32_t> d_rp_dl_code;
-    DeviceBuf<uint32_t> d_rp_u32;
-    DeviceBuf<long long> d_rp_ent, d_rp_chunks, d_rp_tenant_off;
-    DeviceBuf<bfq_stale_match> d_rp_stale;
-    PinnedBuf<unsigned long long> h_rp_ctr;
-    // pinned result buffers
-    PinnedBuf<uint32_t> h_span_begin, h_span_count, h_route_count;
-    PinnedBuf<uint2> h_ranges;
-    PinnedBuf<uint3> h_throttled;
-
-    cudaError_t init(int dev) {
-        device = dev;
-        cudaError_t e = cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking);
-        if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking);
-        for (auto& w : work_stream)
-            if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&w, cudaStreamNonBlocking);
-        for (auto& x : ev)
-            if (e == cudaSuccess) e = cudaEventCreate(&x);
-        for (auto& x : evk)
-            if (e == cudaSuccess) e = cudaEventCreate(&x);
-        for (auto& x : ev_h2d)
-            if (e == cudaSuccess) e = cudaEventCreateWithFlags(&x, cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev_done, cudaEventDisableTiming);
-        return e;
-    }
-    ~Workspace() {
-        cudaSetDevice(device);   // the buffers are freed after this body, on this device
-        for (auto& e : ev) if (e) cudaEventDestroy(e);
-        for (auto& e : evk) if (e) cudaEventDestroy(e);
-        for (auto& e : ev_h2d) if (e) cudaEventDestroy(e);
-        if (ev_done) cudaEventDestroy(ev_done);
-        for (auto& e : ev_use) cudaEventDestroy(e);
-        if (copy_stream) cudaStreamDestroy(copy_stream);
-        for (auto& w : work_stream) if (w) cudaStreamDestroy(w);
-        if (stream) cudaStreamDestroy(stream);
-    }
-};
-
-// idle workspaces of one index. Shared with every result / lease in flight, so that freeing a result after its index was
-// destroyed (a garbage-collected host language decides the order) still has a valid place to return its workspace to.
-struct Pool {
-    std::mutex mu;
-    std::vector<Workspace*> idle;
-    int device = 0;
-    bool closed = false;
-    ~Pool() {
-        cudaSetDevice(device);
-        for (Workspace* w : idle) delete w;
-    }
-};
 
 struct bfq_result {
     bfq_index* owner = nullptr;
@@ -223,42 +33,6 @@ struct bfq_result {
     const bfq_range* ranges = nullptr;
     const bfq_throttled* throttled = nullptr;
     double ms[4] = {0, 0, 0, 0};
-};
-
-struct bfq_index {
-    int device = 0;
-    std::mutex mu;         // current snapshot pointer, workspace pool, statistics
-    std::mutex stage_mu;   // staging area: reset / load / apply and the (long) host-side rebuild of commit
-    Staging staging;
-    std::shared_ptr<Snapshot> snap;
-    uint64_t next_generation = 1;
-    std::shared_ptr<Pool> pool = std::make_shared<Pool>();   // idle workspaces
-    std::shared_ptr<DelivererTable> deliverers = std::make_shared<DelivererTable>();   // (subBrokerId, delivererKey) -> id, append-only
-    int64_t order_min = 32768;           // batches smaller than this are matched in arrival order (BFQ_ORDER=0: never order)
-    bool dedup = true;                   // BFQ_DEDUP=0: match duplicates of a (tenant, topic) pair separately
-    int32_t tier0_ctas_per_sm = 0;       // bfq_index_set_option("tier0_ctas_per_sm"): 0 = as many as fit
-    int32_t dedup_hash_bits = 64;        // bfq_index_set_option("dedup_hash_bits"): test knob, < 64 forces de-dup hash collisions
-    bool fanout_global = false;          // bfq_index_set_option("fanout_global"): test knob, every fan-out takes the global pass
-    double last_kernel_ms = 0;
-    int64_t launches = 0, overflow_topics = 0, flagged_topics = 0, deferred_topics = 0, duplicate_topics = 0, buffer_retries = 0;
-    int64_t global_fanouts = 0;
-    int64_t full_commits = 0, delta_commits = 0;
-    int64_t rebuilt_tenants = 0;         // tenants the last commit built (bfq_index_stats slot 21)
-    // Releases the host image of a full build (2.3 GB of records at 10M filters: 0.4 s of page freeing) off the committing
-    // thread. Touched under stage_mu only (commits are serialised); joined before the next one starts and at destroy.
-    std::thread janitor;
-
-    ~bfq_index() {
-        if (janitor.joinable()) janitor.join();
-        cudaSetDevice(device);
-        std::vector<Workspace*> idle;
-        {
-            std::lock_guard<std::mutex> g(pool->mu);
-            pool->closed = true;   // workspaces still leased are freed when they come back
-            idle.swap(pool->idle);
-        }
-        for (Workspace* w : idle) delete w;
-    }
 };
 
 namespace {
@@ -305,11 +79,6 @@ void give_back(const std::shared_ptr<Pool>& pool, Workspace* w) {
     delete w;
 }
 
-struct CoreOut {
-    int64_t n_ranges = 0, n_throttled = 0, n_overflow = 0, n_flagged = 0, n_launches = 0, n_deferred = 0, n_leaders = 0;
-    uint64_t want_dyn = 0, want_thr = 0;
-    int64_t chunk_throttled[MAX_CHUNKS] = {};
-};
 
 // tenant ids -> root ordinals of this snapshot + caps, uploaded to the workspace (skipped when the previous call on this
 // workspace carried the same list against the same snapshot: compared byte for byte, not by fingerprint)
@@ -413,16 +182,6 @@ SubBatch whole_batch(Workspace* w, int64_t n) {
     return sb;
 }
 
-struct CoreCtx {
-    bfq_index* h;
-    Workspace* w;
-    const Snapshot* s;
-    const uint8_t* d_topics;
-    const int64_t* d_topic_off;
-    const int32_t* d_topic_tenant;
-    int32_t n_tenants;
-    cudaStream_t stream;
-};
 
 MatchParams core_params(const CoreCtx& c, const SubBatch& sb) {
     Workspace* w = c.w;
@@ -674,23 +433,6 @@ int32_t grow_for_retry(Workspace* w, const CoreOut& co, int64_t n, int C) {
     return BFQ_OK;
 }
 
-// A device-side match in flight (bfq_match_device_async .. bfq_device_result_wait .. bfq_device_result_release)
-struct DeviceLease {
-    bfq_index* h = nullptr;
-    std::shared_ptr<Pool> pool;
-    std::shared_ptr<Snapshot> snap;
-    Workspace* ws = nullptr;
-    CoreCtx ctx{};
-    int64_t n = 0;
-    bool done = false;
-    int32_t rc = BFQ_OK;
-    CoreOut co;
-    double tier0_ms = 0;
-    // streams the result was used on after the match; stream i's last use is recorded on ws->ev_use[i] (lease.h). One event
-    // per stream: re-recording covers that stream's earlier uses, but not another stream's.
-    std::mutex use_mu;
-    std::vector<cudaStream_t> used_on;
-};
 
 void fill_device_result(const DeviceLease* L, bfq_device_result* out) {
     Workspace* w = L->ws;
@@ -2017,877 +1759,6 @@ int32_t bfq_match_device(bfq_index* h, const uint8_t* tenants, const int64_t* te
     rc = bfq_device_result_wait(out);
     if (rc != BFQ_OK) bfq_device_result_release(out);
     return rc;
-}
-
-}  // extern "C"
-
-int32_t bfq::lease_use(const bfq_device_result* res, cudaStream_t stream, const char* who, cudaEvent_t* ev) {
-    if (!res || !res->lease) return fail(BFQ_E_INVALID, std::string(who) + ": no match in flight behind this result");
-    auto* L = static_cast<DeviceLease*>(res->lease);
-    if (!L->done || L->rc != BFQ_OK) return fail(BFQ_E_STATE, std::string(who) + " needs a completed match (bfq_device_result_wait)");
-    BFQ_CUDA_TRY(cudaSetDevice(L->h->device));
-    std::lock_guard<std::mutex> g(L->use_mu);
-    size_t i = 0;
-    while (i < L->used_on.size() && L->used_on[i] != stream) i++;
-    if (i == L->used_on.size()) {
-        Workspace* w = L->ws;
-        if (w->ev_use.size() == i) {
-            cudaEvent_t e = nullptr;
-            BFQ_CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-            w->ev_use.push_back(e);
-        }
-        L->used_on.push_back(stream);
-    }
-    *ev = L->ws->ev_use[i];
-    return BFQ_OK;
-}
-
-namespace {
-// the expand's inputs for a completed device match (its workspace, snapshot and caps) and the caller's CSR outputs
-ExpandParams expand_params(const DeviceLease* L, int64_t* d_offsets, int64_t* d_ranks, int64_t rank_cap) {
-    const Workspace* w = L->ws;
-    const Snapshot* s = L->snap.get();
-    const size_t nt = (size_t) std::max(L->ctx.n_tenants, 1);
-    ExpandParams p{};
-    p.n_topics = L->n;
-    p.span_begin = w->d_span_begin.p;
-    p.span_count = w->d_span_count.p;
-    p.route_count = w->d_route_count.p;
-    p.kept_count = w->d_kept.p;
-    p.ranges = w->d_ranges.p;
-    p.segs = s->d_segs.p;
-    p.counts = w->d_exp_counts.p;
-    p.offsets = d_offsets;
-    p.ranks = d_ranks;
-    p.rank_cap = d_ranks ? rank_cap : 0;
-    p.flagged_list = w->d_flagged.p;
-    p.n_flagged = L->co.n_flagged;
-    p.topic_tenant = L->ctx.d_topic_tenant;
-    p.max_pfanout = w->d_tenant_tab.p + nt;
-    p.max_gfanout = w->d_tenant_tab.p + 2 * nt;
-    p.rkind = s->d_rkind.p;
-    p.pfx_persistent = s->d_pfxP.p;
-    p.pfx_group = s->d_pfxG.p;
-    return p;
-}
-}  // namespace
-
-extern "C" {
-
-int32_t bfq_expand_device(const bfq_device_result* res, int64_t* d_offsets, int64_t* d_ranks, int64_t rank_cap, void* stream,
-                          int64_t* n_ranks) {
-    if (!res || !res->lease || !d_offsets) return fail(BFQ_E_INVALID, "bad argument");
-    auto* L = static_cast<DeviceLease*>(res->lease);
-    cudaStream_t st = (cudaStream_t) stream;
-    cudaEvent_t ev = nullptr;
-    const int32_t rc = lease_use(res, st, "bfq_expand_device", &ev);
-    if (rc != BFQ_OK) return rc;
-    RecordOnExit rec(ev, st);   // phase 2 is still running when the call returns
-    bfq_index* h = L->h;
-    Workspace* w = L->ws;
-    const int64_t n_topics = L->n;
-    BFQ_CUDA_TRY(w->d_exp_counts.reserve((size_t) n_topics + 1));
-    const ExpandParams p = expand_params(L, d_offsets, d_ranks, rank_cap);
-    size_t tmp_bytes = 0;
-    BFQ_CUDA_TRY(launch_expand(p, nullptr, &tmp_bytes, st, 1));
-    BFQ_CUDA_TRY(w->d_scan_tmp.reserve(tmp_bytes + 256));
-    BFQ_CUDA_TRY(launch_expand(p, w->d_scan_tmp.p, &tmp_bytes, st, 1));
-    long long total = 0;
-    BFQ_CUDA_TRY(cudaMemcpyAsync(&total, d_offsets + n_topics, sizeof(long long), cudaMemcpyDeviceToHost, st));
-    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
-    if (n_ranks) *n_ranks = (int64_t) total;
-    int64_t launches = 2;
-    if (d_ranks && total <= rank_cap) {
-        BFQ_CUDA_TRY(launch_expand(p, w->d_scan_tmp.p, &tmp_bytes, st, 2));
-        launches += 2;
-    }
-    std::lock_guard<std::mutex> g(h->mu);
-    h->launches += launches;
-    return BFQ_OK;
-}
-
-int32_t bfq_expand_device_budget(const bfq_device_result* res, const int32_t* d_msg_bytes, const int64_t* max_pfanout_bytes,
-                                 const uint8_t* tenant_bandwidth, int64_t* d_offsets, int64_t* d_ranks, int64_t rank_cap,
-                                 void* stream, bfq_budget_result* out) {
-    if (!res || !res->lease || !d_offsets || !out) return fail(BFQ_E_INVALID, "bad argument");
-    auto* L = static_cast<DeviceLease*>(res->lease);
-    cudaStream_t st = (cudaStream_t) stream;
-    cudaEvent_t ev = nullptr;
-    const int32_t rc = lease_use(res, st, "bfq_expand_device_budget", &ev);
-    if (rc != BFQ_OK) return rc;
-    RecordOnExit rec(ev, st);   // phase 2 is still running when the call returns
-    const int64_t n_topics = L->n;
-    const int32_t n_tenants = L->ctx.n_tenants;
-    if (n_topics > 0 && !d_msg_bytes) return fail(BFQ_E_INVALID, "NULL d_msg_bytes");
-    if (n_tenants > 0 && (!max_pfanout_bytes || !tenant_bandwidth)) return fail(BFQ_E_INVALID, "NULL per-tenant budget table");
-    for (int32_t i = 0; i < n_tenants; i++)
-        if (max_pfanout_bytes[i] <= 0)
-            return fail(BFQ_E_INVALID, "max_pfanout_bytes[" + std::to_string(i) + "] = " + std::to_string(max_pfanout_bytes[i]) +
-                                           ": MaxPersistentFanoutBytes must be > 0");
-    bfq_index* h = L->h;
-    Workspace* w = L->ws;
-    const size_t nn = (size_t) std::max<int64_t>(n_topics, 1), nt = (size_t) std::max(n_tenants, 1);
-    BFQ_CUDA_TRY(w->d_exp_counts.reserve(nn + 1));
-    BFQ_CUDA_TRY(w->d_bud_bytes.reserve(nt));
-    BFQ_CUDA_TRY(w->d_bud_bw.reserve(nt));
-    BFQ_CUDA_TRY(w->d_bud_flags.reserve(nn));
-    BFQ_CUDA_TRY(w->d_bud_dp.reserve(nn));
-    BFQ_CUDA_TRY(w->d_bud_list.reserve(nn));
-    BFQ_CUDA_TRY(w->d_bud_ctr.reserve(BUD_CTR_COUNT));
-    if (n_tenants > 0) {
-        BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_bud_bytes.p, max_pfanout_bytes, (size_t) n_tenants * sizeof(long long), cudaMemcpyHostToDevice, st));
-        BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_bud_bw.p, tenant_bandwidth, (size_t) n_tenants, cudaMemcpyHostToDevice, st));
-    }
-    BFQ_CUDA_TRY(cudaMemsetAsync(w->d_bud_ctr.p, 0, BUD_CTR_COUNT * sizeof(unsigned long long), st));
-    BudgetParams q{};
-    q.e = expand_params(L, d_offsets, d_ranks, rank_cap);
-    q.n_tenants = n_tenants;
-    q.msg_bytes = d_msg_bytes;
-    q.max_bytes = w->d_bud_bytes.p;
-    q.bandwidth = w->d_bud_bw.p;
-    q.delivered_p = w->d_bud_dp.p;
-    q.flags = w->d_bud_flags.p;
-    q.list = w->d_bud_list.p;
-    q.ctr = w->d_bud_ctr.p;
-    size_t tmp_bytes = 0;
-    BFQ_CUDA_TRY(launch_budget(q, nullptr, &tmp_bytes, st, 1));
-    BFQ_CUDA_TRY(w->d_scan_tmp.reserve(tmp_bytes + 256));
-    BFQ_CUDA_TRY(launch_budget(q, w->d_scan_tmp.p, &tmp_bytes, st, 1));
-    long long total = 0;
-    unsigned long long ctr[BUD_CTR_COUNT];
-    BFQ_CUDA_TRY(cudaMemcpyAsync(&total, d_offsets + n_topics, sizeof(long long), cudaMemcpyDeviceToHost, st));
-    BFQ_CUDA_TRY(cudaMemcpyAsync(ctr, w->d_bud_ctr.p, sizeof(ctr), cudaMemcpyDeviceToHost, st));
-    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
-    int64_t launches = 2;
-    const bool ok = ctr[BUD_BAD_SIZE] == 0;
-    if (ok && d_ranks && total <= rank_cap) {
-        q.n_listed = (int64_t) ctr[BUD_LISTED];
-        BFQ_CUDA_TRY(launch_budget(q, w->d_scan_tmp.p, &tmp_bytes, st, 2));
-        launches += 2;
-    }
-    {
-        std::lock_guard<std::mutex> g(h->mu);
-        h->launches += launches;
-    }
-    if (!ok) return fail(BFQ_E_INVALID, std::to_string(ctr[BUD_BAD_SIZE]) + " negative d_msg_bytes entries");
-    out->d_delivered_persistent = w->d_bud_dp.p;
-    out->d_topic_flags = w->d_bud_flags.p;
-    out->n_delivered = (int64_t) total;
-    out->n_dropped_bytes = (int64_t) ctr[BUD_DROP_BYTES];
-    out->n_dropped_persistent_bandwidth = (int64_t) ctr[BUD_DROP_PBW];
-    out->n_dropped_transient_bandwidth = (int64_t) ctr[BUD_DROP_TBW];
-    return BFQ_OK;
-}
-
-// ---------------------------------------------------------------- fan-out expansion (fanout.cu)
-namespace {
-// the snapshot's fan-out tables: every tenant's routes resolved to deliverer ids (cached per tenant blob: a delta commit
-// re-resolves only the tenants it rebuilt), concatenated in rank order and uploaded once per snapshot
-int32_t ensure_fan_table(bfq_index* h, Snapshot* s, std::shared_ptr<Snapshot::FanTable>* out) {
-    std::lock_guard<std::mutex> g(s->fan_mu);
-    if (s->fan) {
-        *out = s->fan;
-        return BFQ_OK;
-    }
-    const size_t T = s->th.size();
-    std::vector<std::string> errs(T);
-    {
-        std::atomic<size_t> cursor{0};
-        auto worker = [&]() {
-            while (true) {
-                const size_t i = cursor.fetch_add(1);
-                if (i >= T) break;
-                if (s->th[i].fan) continue;
-                auto tf = std::make_shared<TenantFan>();
-                if (build_tenant_fan(*s->th[i].kv, h->deliverers.get(), tf.get(), &errs[i])) s->th[i].fan = std::move(tf);
-            }
-        };
-        const unsigned nt = (unsigned) std::max<size_t>(1, std::min<size_t>(std::min<size_t>(std::thread::hardware_concurrency(), 64), T));
-        std::vector<std::thread> th;
-        for (unsigned t = 1; t < nt; t++) th.emplace_back(worker);
-        worker();
-        for (auto& x : th) x.join();
-    }
-    for (size_t i = 0; i < T; i++)
-        if (!s->th[i].fan) return fail(BFQ_E_INVALID, "fan-out tables: " + errs[i]);
-    std::vector<uint32_t> rdeliv((size_t) std::max<int64_t>(s->flat.n_routes, 1), 0), gmem_off(1, 0), gmem_deliv;
-    std::vector<uint8_t> gordered;
-    for (size_t i = 0; i < T; i++) {
-        const TenantFan& tf = *s->th[i].fan;
-        const uint32_t gbase = (uint32_t) gordered.size(), mbase = (uint32_t) gmem_deliv.size();
-        const int64_t lo = s->flat.tenants[i].lo;
-        for (size_t r = 0; r < tf.rdeliv.size(); r++)
-            rdeliv[(size_t) lo + r] = (tf.rdeliv[r] & FO_GROUP_BIT) ? (FO_GROUP_BIT | ((tf.rdeliv[r] & ~FO_GROUP_BIT) + gbase)) : tf.rdeliv[r];
-        for (size_t k = 1; k < tf.gmem_off.size(); k++) gmem_off.push_back(tf.gmem_off[k] + mbase);
-        gmem_deliv.insert(gmem_deliv.end(), tf.gmem_deliv.begin(), tf.gmem_deliv.end());
-        gordered.insert(gordered.end(), tf.gordered.begin(), tf.gordered.end());
-    }
-    auto ft = std::make_shared<Snapshot::FanTable>();
-    {
-        std::lock_guard<std::mutex> gd(h->deliverers->mu);
-        ft->n_deliverers = (uint32_t) h->deliverers->list.size() + 1;
-    }
-    // ids share rdeliv[] with FO_GROUP_BIT, and n_deliverers and the global pass's n_deliverers + 1 counts are int32
-    if (ft->n_deliverers > 0x7FFFFFFEu) return fail(BFQ_E_RANGE, "more than 2^31 - 3 distinct (subBrokerId, delivererKey) pairs on one handle");
-    BFQ_CUDA_TRY(ft->d_rdeliv.reserve(rdeliv.size()));
-    BFQ_CUDA_TRY(ft->d_gmem_off.reserve(gmem_off.size()));
-    BFQ_CUDA_TRY(ft->d_gmem_deliv.reserve(std::max<size_t>(gmem_deliv.size(), 1)));
-    BFQ_CUDA_TRY(ft->d_gordered.reserve(std::max<size_t>(gordered.size(), 1)));
-    BFQ_CUDA_TRY(cudaMemcpy(ft->d_rdeliv.p, rdeliv.data(), rdeliv.size() * 4, cudaMemcpyHostToDevice));
-    BFQ_CUDA_TRY(cudaMemcpy(ft->d_gmem_off.p, gmem_off.data(), gmem_off.size() * 4, cudaMemcpyHostToDevice));
-    if (!gmem_deliv.empty()) BFQ_CUDA_TRY(cudaMemcpy(ft->d_gmem_deliv.p, gmem_deliv.data(), gmem_deliv.size() * 4, cudaMemcpyHostToDevice));
-    if (!gordered.empty()) BFQ_CUDA_TRY(cudaMemcpy(ft->d_gordered.p, gordered.data(), gordered.size(), cudaMemcpyHostToDevice));
-    s->fan = ft;
-    *out = ft;
-    return BFQ_OK;
-}
-
-// the snapshot's ordered-group member urls, from the tenants' fan-out tables (call after ensure_fan_table), in the fan table's
-// member order: each url at byte 4 of its own run of 8-byte words, so the pick reads LE32(hash) ‖ url as whole words
-int32_t ensure_url_table(Snapshot* s, std::shared_ptr<Snapshot::UrlTable>* out) {
-    std::lock_guard<std::mutex> g(s->fan_mu);
-    if (s->urls) {
-        *out = s->urls;
-        return BFQ_OK;
-    }
-    std::vector<unsigned long long> words;
-    std::vector<long long> word;
-    std::vector<uint32_t> len;
-    uint32_t largest = 0;
-    for (const auto& th : s->th) {
-        const TenantFan& tf = *th.fan;
-        for (size_t m = 0; m + 1 < tf.ourl_off.size(); m++) {
-            const uint32_t a = tf.ourl_off[m], n = tf.ourl_off[m + 1] - a;
-            word.push_back((long long) words.size());
-            len.push_back(n);
-            if (n == 0) continue;
-            const size_t w0 = words.size();
-            words.resize(w0 + (4 + (size_t) n + 7) / 8, 0);
-            memcpy(reinterpret_cast<uint8_t*>(words.data() + w0) + 4, tf.ourl.data() + a, n);
-        }
-        for (size_t k = 0; k < tf.gordered.size(); k++)
-            if (tf.gordered[k]) largest = std::max(largest, tf.gmem_off[k + 1] - tf.gmem_off[k]);
-    }
-    auto ut = std::make_shared<Snapshot::UrlTable>();
-    ut->member_bits = largest ? 32u - (uint32_t) __builtin_clz(largest) : 1u;
-    BFQ_CUDA_TRY(ut->d_words.reserve(std::max<size_t>(words.size(), 1)));
-    BFQ_CUDA_TRY(ut->d_word.reserve(std::max<size_t>(word.size(), 1)));
-    BFQ_CUDA_TRY(ut->d_len.reserve(std::max<size_t>(len.size(), 1)));
-    if (!words.empty()) BFQ_CUDA_TRY(cudaMemcpy(ut->d_words.p, words.data(), words.size() * 8, cudaMemcpyHostToDevice));
-    if (!word.empty()) BFQ_CUDA_TRY(cudaMemcpy(ut->d_word.p, word.data(), word.size() * 8, cudaMemcpyHostToDevice));
-    if (!len.empty()) BFQ_CUDA_TRY(cudaMemcpy(ut->d_len.p, len.data(), len.size() * 4, cudaMemcpyHostToDevice));
-    s->urls = ut;
-    *out = ut;
-    return BFQ_OK;
-}
-}  // namespace
-
-int32_t bfq_fanout_device(const bfq_device_result* res, const int64_t* d_offsets, const int64_t* d_ranks, int64_t n_pairs, void* stream,
-                          bfq_fanout_result* out) {
-    if (!res || !res->lease || !out || !d_offsets || n_pairs < 0 || (n_pairs > 0 && !d_ranks)) return fail(BFQ_E_INVALID, "bad argument");
-    auto* L = static_cast<DeviceLease*>(res->lease);
-    cudaStream_t st = (cudaStream_t) stream;
-    cudaEvent_t ev = nullptr;
-    int32_t rc = lease_use(res, st, "bfq_fanout_device", &ev);
-    if (rc != BFQ_OK) return rc;
-    RecordOnExit rec(ev, st);   // the call never synchronises: every pass is still queued when it returns
-    if (n_pairs >= (int64_t) 0xFFFFFFF0ll) return fail(BFQ_E_RANGE, "more than 2^32 (topic, route) pairs in one batch; split the batch");
-    bfq_index* h = L->h;
-    Workspace* w = L->ws;
-    std::shared_ptr<Snapshot::FanTable> ft;
-    rc = ensure_fan_table(h, L->snap.get(), &ft);
-    if (rc != BFQ_OK) return rc;
-    bool force_global;
-    {
-        std::lock_guard<std::mutex> g(h->mu);
-        force_global = h->fanout_global;
-    }
-    const bool tiled = !force_global && fanout_tiled(ft->n_deliverers, n_pairs);
-    const size_t words = fanout_scratch_words(ft->n_deliverers, n_pairs, tiled);
-    BFQ_CUDA_TRY(w->d_fo_counts.reserve(words));
-    BFQ_CUDA_TRY(w->d_fo_base.reserve(words));
-    BFQ_CUDA_TRY(w->d_pack_offsets.reserve((size_t) ft->n_deliverers + 1));
-    BFQ_CUDA_TRY(w->d_pack_topic.reserve((size_t) std::max<int64_t>(n_pairs, 1)));
-    BFQ_CUDA_TRY(w->d_pack_rank.reserve((size_t) std::max<int64_t>(n_pairs, 1)));
-    BFQ_CUDA_TRY(w->d_pack_member.reserve((size_t) std::max<int64_t>(n_pairs, 1)));
-    FanoutParams p{};
-    p.n_topics = L->n;
-    p.offsets = d_offsets;
-    p.n_pairs = n_pairs;
-    p.ranks = d_ranks;
-    p.rdeliv = ft->d_rdeliv.p;
-    p.gmem_off = ft->d_gmem_off.p;
-    p.gmem_deliv = ft->d_gmem_deliv.p;
-    p.gordered = ft->d_gordered.p;
-    p.n_deliverers = ft->n_deliverers;
-    p.counts = w->d_fo_counts.p;
-    p.base = w->d_fo_base.p;
-    p.pack_offsets = w->d_pack_offsets.p;
-    p.pack_topic = w->d_pack_topic.p;
-    p.pack_rank = w->d_pack_rank.p;
-    p.pack_member = w->d_pack_member.p;
-    size_t tmp_bytes = 0;
-    BFQ_CUDA_TRY(launch_fanout(p, tiled, nullptr, &tmp_bytes, st));
-    BFQ_CUDA_TRY(w->d_fo_tmp.reserve(tmp_bytes + 256));
-    BFQ_CUDA_TRY(launch_fanout(p, tiled, w->d_fo_tmp.p, &tmp_bytes, st));
-    out->d_pack_offsets = (const int64_t*) w->d_pack_offsets.p;
-    out->d_pack_topic = w->d_pack_topic.p;
-    out->d_pack_rank = w->d_pack_rank.p;
-    out->d_pack_member = w->d_pack_member.p;
-    out->n_pairs = n_pairs;
-    out->n_deliverers = (int32_t) ft->n_deliverers;
-    out->ordered_share_id = (int32_t) ft->n_deliverers - 1;
-    out->generation = L->snap->generation;
-    std::lock_guard<std::mutex> g(h->mu);
-    h->launches += 5;
-    if (!tiled) h->global_fanouts++;
-    return BFQ_OK;
-}
-
-namespace {
-struct PublisherPacks {   // bfq_delivery_device_ordered's publisher arrays
-    const int64_t* pub_off;
-    const int32_t* pub_hash;
-    int64_t n_pubs;
-};
-
-// bfq_delivery_device (pubs == nullptr) and bfq_delivery_device_ordered (pubs and oout set)
-int32_t run_delivery_call(const bfq_device_result* res, const int64_t* d_offsets, const int64_t* d_ranks, int64_t n_pairs,
-                          const int32_t* d_topic_tenant, void* stream, const char* who, const PublisherPacks* pubs,
-                          bfq_delivery_result* out, bfq_delivery_ordered_result* oout) {
-    auto* L = static_cast<DeviceLease*>(res->lease);
-    cudaStream_t st = (cudaStream_t) stream;
-    cudaEvent_t ev = nullptr;
-    int32_t rc = lease_use(res, st, who, &ev);
-    if (rc != BFQ_OK) return rc;
-    RecordOnExit rec(ev, st);   // the call synchronises after its last launch, but an error return may come before that
-    if (L->n > 0 && !d_topic_tenant) return fail(BFQ_E_INVALID, "NULL d_topic_tenant");
-    if (pubs && !pubs->pub_off) return fail(BFQ_E_INVALID, "NULL d_pub_off");
-    if (pubs && (pubs->n_pubs < 0 || (pubs->n_pubs > 0 && !pubs->pub_hash))) return fail(BFQ_E_INVALID, "bad d_pub_hash / n_pubs");
-    if (n_pairs >= (int64_t) 0xFFFFFFF0ll) return fail(BFQ_E_RANGE, "more than 2^32 (topic, route) pairs in one batch; split the batch");
-    bfq_index* h = L->h;
-    Workspace* w = L->ws;
-    w->dl_n_packs = -1;   // the buffers below are about to change
-    std::shared_ptr<Snapshot::FanTable> ft;
-    rc = ensure_fan_table(h, L->snap.get(), &ft);
-    if (rc != BFQ_OK) return rc;
-    std::shared_ptr<Snapshot::UrlTable> ut;
-    if (pubs && (rc = ensure_url_table(L->snap.get(), &ut)) != BFQ_OK) return rc;
-    const int64_t T = L->n;
-    DeliveryParams q{};
-    q.f.n_topics = T;
-    q.f.offsets = d_offsets;
-    q.f.n_pairs = n_pairs;
-    q.f.ranks = d_ranks;
-    q.f.rdeliv = ft->d_rdeliv.p;
-    q.f.gmem_off = ft->d_gmem_off.p;
-    q.f.gmem_deliv = ft->d_gmem_deliv.p;
-    q.f.gordered = ft->d_gordered.p;
-    q.f.n_deliverers = ft->n_deliverers;
-    q.topic_tenant = d_topic_tenant;
-    q.n_tenants = L->ctx.n_tenants;
-    int64_t n_items = 0;
-    if (pubs) {
-        // phase 1: which pairs are $oshare pairs to resolve, how many (pair, publisher) items, and the d_pub_off check
-        q.oshare = true;
-        q.o.pub_off = pubs->pub_off;
-        q.o.pub_hash = pubs->pub_hash;
-        q.o.n_pubs = pubs->n_pubs;
-        q.o.url_words = ut->d_words.p;
-        q.o.url_word = ut->d_word.p;
-        q.o.url_len = ut->d_len.p;
-        q.o.member_bits = ut->member_bits;
-        BFQ_CUDA_TRY(w->d_os_flag.reserve((size_t) n_pairs + 1));
-        BFQ_CUDA_TRY(w->d_os_items.reserve((size_t) n_pairs + 1));
-        BFQ_CUDA_TRY(w->d_os_check.reserve(4));
-        q.o.oflag = w->d_os_flag.p;
-        q.o.oitems = w->d_os_items.p;
-        q.o.check = w->d_os_check.p;
-        size_t tmp_bytes = 0;
-        BFQ_CUDA_TRY(launch_oshare_count(q, nullptr, &tmp_bytes, st));
-        BFQ_CUDA_TRY(w->d_dl_tmp.reserve(tmp_bytes + 256));
-        BFQ_CUDA_TRY(launch_oshare_count(q, w->d_dl_tmp.p, &tmp_bytes, st));
-        unsigned long long chk[4];
-        BFQ_CUDA_TRY(cudaMemcpyAsync(chk, w->d_os_check.p, sizeof(chk), cudaMemcpyDeviceToHost, st));
-        BFQ_CUDA_TRY(cudaStreamSynchronize(st));
-        if ((int64_t) chk[3] != n_pairs)
-            return fail(BFQ_E_INVALID, "n_pairs = " + std::to_string(n_pairs) + " but d_offsets[n_topics] = " + std::to_string((int64_t) chk[3]));
-        if (chk[2]) return fail(BFQ_E_INVALID, "d_pub_off must run from 0 to n_pubs = " + std::to_string(pubs->n_pubs) + " without decreasing");
-        if (chk[1] >= 0xFFFFFFF0ull || (uint64_t) n_pairs + chk[1] >= 0xFFFFFFF0ull)
-            return fail(BFQ_E_RANGE, "more than 2^32 pairs and ($oshare pair, publisher) items in one batch; split the batch");
-        q.o.n_opairs = (int64_t) chk[0];
-        n_items = (int64_t) chk[1];
-        q.o.n_items = n_items;
-    }
-    const size_t np = (size_t) std::max<int64_t>(n_pairs + n_items, 1);
-    BFQ_CUDA_TRY(w->d_dl_topic_tmp.reserve(6 * (size_t) T + 2));
-    BFQ_CUDA_TRY(w->d_dl_pair_tmp.reserve(10 * np + 2));
-    BFQ_CUDA_TRY(w->d_dl_pcount.reserve((size_t) ft->n_deliverers + 1));
-    BFQ_CUDA_TRY(w->d_dl_totals.reserve(5));
-    BFQ_CUDA_TRY(w->d_package_off.reserve((size_t) ft->n_deliverers + 1));
-    BFQ_CUDA_TRY(w->d_package_tenant.reserve(np));
-    BFQ_CUDA_TRY(w->d_dl_pack_off.reserve(np + 1));
-    BFQ_CUDA_TRY(w->d_dl_pack_topic.reserve(np));
-    BFQ_CUDA_TRY(w->d_match_off.reserve(np + 1));
-    BFQ_CUDA_TRY(w->d_match_rank.reserve(np));
-    BFQ_CUDA_TRY(w->d_match_member.reserve(np));
-    uint32_t* tt = w->d_dl_topic_tmp.p;
-    q.tkey[0] = tt;
-    q.tkey[1] = tt + T;
-    q.tval[0] = tt + 2 * T;
-    q.tval[1] = tt + 3 * T;
-    q.tcount = tt + 4 * T;
-    q.tstart = tt + 5 * T + 1;
-    uint32_t* pt = w->d_dl_pair_tmp.p;
-    q.key[0] = pt;
-    q.key[1] = pt + np;
-    q.val[0] = pt + 2 * np;
-    q.val[1] = pt + 3 * np;
-    q.e_topic = pt + 4 * np;
-    q.e_rank = pt + 5 * np;
-    q.e_member = pt + 6 * np;
-    q.s_topic = pt + 7 * np;
-    q.package_head = pt + 8 * np;
-    q.pack_head = pt + 9 * np + 1;
-    q.pcount = w->d_dl_pcount.p;
-    q.totals = w->d_dl_totals.p;
-    q.package_off = w->d_package_off.p;
-    q.package_tenant = w->d_package_tenant.p;
-    q.pack_off = w->d_dl_pack_off.p;
-    q.pack_topic = w->d_dl_pack_topic.p;
-    q.match_off = w->d_match_off.p;
-    q.match_rank = w->d_match_rank.p;
-    q.match_member = w->d_match_member.p;
-    if (pubs) {
-        const size_t O = (size_t) q.o.n_opairs, I = (size_t) n_items;
-        BFQ_CUDA_TRY(w->d_os_key.reserve(std::max<size_t>(2 * O + 2 * I, 1)));
-        BFQ_CUDA_TRY(w->d_os_u32.reserve((O + 1) + 2 * I + 2 * (I + 1) + I + 3 * np + 1));
-        BFQ_CUDA_TRY(w->d_pack_pub.reserve(std::max<size_t>(I, 1)));
-        BFQ_CUDA_TRY(w->d_pack_pub_off.reserve(np + 1));
-        unsigned long long* kp = w->d_os_key.p;
-        q.o.okey[0] = kp;
-        q.o.okey[1] = kp + O;
-        q.o.ikey[0] = kp + 2 * O;
-        q.o.ikey[1] = kp + 2 * O + I;
-        uint32_t* up = w->d_os_u32.p;
-        q.o.istart = up;
-        up += O + 1;
-        q.o.ival[0] = up;
-        q.o.ival[1] = up + I;
-        up += 2 * I;
-        q.o.ihead = up;
-        up += I + 1;
-        q.o.sub_start = up;
-        up += I + 1;
-        q.o.sub_pack = up;
-        up += I;
-        q.o.e_sub = up;
-        q.o.s_sub = up + np;
-        q.o.pub_count = up + 2 * np;
-        q.o.pack_pub_off = w->d_pack_pub_off.p;
-        q.o.pack_pub = w->d_pack_pub.p;
-    }
-    size_t tmp_bytes = 0;
-    BFQ_CUDA_TRY(launch_delivery(q, nullptr, &tmp_bytes, st));
-    BFQ_CUDA_TRY(w->d_dl_tmp.reserve(tmp_bytes + 256));
-    BFQ_CUDA_TRY(launch_delivery(q, w->d_dl_tmp.p, &tmp_bytes, st));
-    unsigned long long tot[5] = {0, 0, 0, 0, 0};
-    BFQ_CUDA_TRY(cudaMemcpyAsync(tot, w->d_dl_totals.p, (pubs ? 5 : 4) * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
-    {
-        std::lock_guard<std::mutex> g(h->mu);
-        h->launches += pubs ? 25 : 11;
-    }
-    if ((int64_t) tot[3] != n_pairs)
-        return fail(BFQ_E_INVALID, "n_pairs = " + std::to_string(n_pairs) + " but d_offsets[n_topics] = " + std::to_string((int64_t) tot[3]));
-    out->d_package_off = (const int64_t*) w->d_package_off.p;
-    out->d_package_tenant = w->d_package_tenant.p;
-    out->d_pack_off = (const int64_t*) w->d_dl_pack_off.p;
-    out->d_pack_topic = w->d_dl_pack_topic.p;
-    out->d_match_off = (const int64_t*) w->d_match_off.p;
-    out->d_match_rank = w->d_match_rank.p;
-    out->d_match_member = w->d_match_member.p;
-    out->n_pairs = (int64_t) tot[0];
-    out->n_packages = (int64_t) tot[1];
-    out->n_packs = (int64_t) tot[2];
-    out->n_deliverers = (int32_t) ft->n_deliverers;
-    out->ordered_share_id = (int32_t) ft->n_deliverers - 1;
-    out->generation = L->snap->generation;
-    w->dl_n_pairs = out->n_pairs;
-    w->dl_n_packages = out->n_packages;
-    w->dl_n_packs = out->n_packs;
-    w->dl_ordered = pubs != nullptr;
-    if (oout) {
-        oout->d_pack_pub_off = (const int64_t*) w->d_pack_pub_off.p;
-        oout->d_pack_pub = w->d_pack_pub.p;
-        oout->n_pack_pubs = n_items;
-        oout->n_ordered_packs = (int64_t) tot[4];
-    }
-    return BFQ_OK;
-}
-}  // namespace
-
-int32_t bfq_delivery_device(const bfq_device_result* res, const int64_t* d_offsets, const int64_t* d_ranks, int64_t n_pairs,
-                            const int32_t* d_topic_tenant, void* stream, bfq_delivery_result* out) {
-    if (!res || !res->lease || !out || !d_offsets || n_pairs < 0 || (n_pairs > 0 && !d_ranks)) return fail(BFQ_E_INVALID, "bad argument");
-    return run_delivery_call(res, d_offsets, d_ranks, n_pairs, d_topic_tenant, stream, "bfq_delivery_device", nullptr, out, nullptr);
-}
-
-int32_t bfq_delivery_device_ordered(const bfq_device_result* res, const int64_t* d_offsets, const int64_t* d_ranks, int64_t n_pairs,
-                                    const int32_t* d_topic_tenant, const int64_t* d_pub_off, const int32_t* d_pub_hash, int64_t n_pubs,
-                                    void* stream, bfq_delivery_ordered_result* out) {
-    if (!res || !res->lease || !out || !d_offsets || n_pairs < 0 || (n_pairs > 0 && !d_ranks)) return fail(BFQ_E_INVALID, "bad argument");
-    const PublisherPacks pubs{d_pub_off, d_pub_hash, n_pubs};
-    return run_delivery_call(res, d_offsets, d_ranks, n_pairs, d_topic_tenant, stream, "bfq_delivery_device_ordered", &pubs, &out->d,
-                             out);
-}
-
-namespace {
-// the snapshot's MatchInfo table: every tenant's entries (cached per tenant blob, so a delta commit re-encodes only the tenants it
-// rebuilt), concatenated in rank order and uploaded once per snapshot
-int32_t ensure_wire_table(Snapshot* s, std::shared_ptr<Snapshot::WireTable>* out) {
-    std::lock_guard<std::mutex> g(s->fan_mu);
-    if (s->wire) {
-        *out = s->wire;
-        return BFQ_OK;
-    }
-    const size_t T = s->th.size();
-    std::vector<std::string> errs(T);
-    {
-        std::atomic<size_t> cursor{0};
-        auto worker = [&]() {
-            while (true) {
-                const size_t i = cursor.fetch_add(1);
-                if (i >= T) break;
-                if (s->th[i].wire) continue;
-                auto tw = std::make_shared<TenantWire>();
-                if (build_tenant_wire(*s->th[i].kv, tw.get(), &errs[i])) s->th[i].wire = std::move(tw);
-            }
-        };
-        const unsigned nt = (unsigned) std::max<size_t>(1, std::min<size_t>(std::min<size_t>(std::thread::hardware_concurrency(), 64), T));
-        std::vector<std::thread> th;
-        for (unsigned t = 1; t < nt; t++) th.emplace_back(worker);
-        worker();
-        for (auto& x : th) x.join();
-    }
-    size_t entries = 0, bytes = 0;
-    for (size_t i = 0; i < T; i++) {
-        if (!s->th[i].wire) return fail(BFQ_E_INVALID, "MatchInfo table: " + errs[i]);
-        entries += s->th[i].wire->off.size() - 1;
-        bytes += s->th[i].wire->bytes.size();
-    }
-    if (entries >= 0xFFFFFFFFull) return fail(BFQ_E_RANGE, "2^32 or more MatchInfos in one snapshot");
-    std::vector<uint32_t> first((size_t) std::max<int64_t>(s->flat.n_routes, 1), 0);
-    std::vector<unsigned long long> off(1, 0);
-    off.reserve(entries + 1);
-    std::vector<uint8_t> blob;
-    blob.reserve(bytes);
-    for (size_t i = 0; i < T; i++) {
-        const TenantWire& tw = *s->th[i].wire;
-        const uint32_t ebase = (uint32_t) (off.size() - 1);
-        const unsigned long long bbase = blob.size();
-        const int64_t lo = s->flat.tenants[i].lo;
-        for (size_t r = 0; r < tw.first.size(); r++) first[(size_t) lo + r] = tw.first[r] + ebase;
-        for (size_t e = 1; e < tw.off.size(); e++) off.push_back(tw.off[e] + bbase);
-        blob.insert(blob.end(), tw.bytes.begin(), tw.bytes.end());
-    }
-    auto wt = std::make_shared<Snapshot::WireTable>();
-    BFQ_CUDA_TRY(wt->d_first.reserve(first.size()));
-    BFQ_CUDA_TRY(wt->d_off.reserve(off.size()));
-    BFQ_CUDA_TRY(wt->d_bytes.reserve(std::max<size_t>(blob.size(), 1)));
-    BFQ_CUDA_TRY(cudaMemcpy(wt->d_first.p, first.data(), first.size() * 4, cudaMemcpyHostToDevice));
-    BFQ_CUDA_TRY(cudaMemcpy(wt->d_off.p, off.data(), off.size() * 8, cudaMemcpyHostToDevice));
-    if (!blob.empty()) BFQ_CUDA_TRY(cudaMemcpy(wt->d_bytes.p, blob.data(), blob.size(), cudaMemcpyHostToDevice));
-    wt->n_entries = entries;
-    s->wire = wt;
-    s->wire_bytes = wt->bytes();
-    *out = wt;
-    return BFQ_OK;
-}
-
-// the nesting is the one the last delivery call on this result left in its workspace (plain or ordered)
-bool latest_nesting(const DeviceLease* L, const bfq_delivery_result* nest) {
-    const Workspace* w = L->ws;
-    return nest->generation == L->snap->generation && nest->d_package_off == (const int64_t*) w->d_package_off.p &&
-           nest->d_match_off == (const int64_t*) w->d_match_off.p && w->dl_n_packs >= 0 && nest->n_packs == w->dl_n_packs &&
-           nest->n_packages == w->dl_n_packages && nest->n_pairs == w->dl_n_pairs;
-}
-
-// bfq_delivery_encode (oout == nullptr) and bfq_delivery_encode_ordered: nest is the nesting's plain part either way
-int32_t run_encode(const bfq_device_result* res, const bfq_delivery_result* nest, const bfq_delivery_ordered_result* onest,
-                   const uint8_t* tenants, const int64_t* tenant_off, int32_t n_tenants, const uint8_t* d_topics,
-                   const int64_t* d_topic_off, const int64_t* d_pub_off, const uint8_t* d_pubpack_bytes,
-                   const int64_t* d_pubpack_off, uint8_t* d_out, int64_t out_cap, void* stream, const char* who,
-                   bfq_delivery_wire_result* out) {
-    if (!res || !res->lease || !nest || !out || out_cap < 0) return fail(BFQ_E_INVALID, "bad argument");
-    auto* L = static_cast<DeviceLease*>(res->lease);
-    cudaStream_t st = (cudaStream_t) stream;
-    cudaEvent_t ev = nullptr;
-    int32_t rc = lease_use(res, st, who, &ev);
-    if (rc != BFQ_OK) return rc;
-    RecordOnExit rec(ev, st);   // the write pass is still running when the call returns
-    if (!d_topics || !d_topic_off || !d_pub_off || !d_pubpack_bytes || !d_pubpack_off)
-        return fail(BFQ_E_INVALID, std::string(who) + ": NULL topic or publisher pack array");
-    if (n_tenants != L->ctx.n_tenants || (n_tenants > 0 && (!tenants || !tenant_off)))
-        return fail(BFQ_E_INVALID, std::string(who) + ": the tenant list must be the match's (" + std::to_string(L->ctx.n_tenants) + " tenants)");
-    Workspace* w = L->ws;
-    if (!latest_nesting(L, nest) || w->dl_ordered != (onest != nullptr) ||
-        (onest && onest->d_pack_pub_off != (const int64_t*) w->d_pack_pub_off.p))
-        return fail(BFQ_E_RANGE, std::string(who) + ": the nesting is not the latest " +
-                                     (onest ? "bfq_delivery_device_ordered" : "bfq_delivery_device") + " result of this device result");
-    bfq_index* h = L->h;
-    std::shared_ptr<Snapshot::WireTable> wt;
-    if ((rc = ensure_wire_table(L->snap.get(), &wt)) != BFQ_OK) return rc;
-    const int64_t np = nest->n_pairs, nk = nest->n_packs, ng = nest->n_packages;
-    const uint32_t D = (uint32_t) nest->n_deliverers;
-    BFQ_CUDA_TRY(w->d_wr_pos.reserve((size_t) (np + 1 + nk + 1 + ng + 1)));
-    BFQ_CUDA_TRY(w->d_wr_check.reserve(4));
-    BFQ_CUDA_TRY(w->d_req_off.reserve((size_t) D + 1));
-    BFQ_CUDA_TRY(w->d_wr_tenant_off.reserve((size_t) n_tenants + 1));
-    const int64_t tbytes = n_tenants > 0 ? tenant_off[n_tenants] : 0;
-    BFQ_CUDA_TRY(w->d_wr_tenants.reserve((size_t) std::max<int64_t>(tbytes, 1)));
-    if (n_tenants > 0) {
-        BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_wr_tenant_off.p, tenant_off, ((size_t) n_tenants + 1) * 8, cudaMemcpyHostToDevice, st));
-        if (tbytes > 0) BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_wr_tenants.p, tenants, (size_t) tbytes, cudaMemcpyHostToDevice, st));
-    }
-    WireParams p{};
-    p.n_packages = ng;
-    p.n_packs = nk;
-    p.n_pairs = np;
-    p.n_deliverers = D;
-    p.package_off = (const long long*) nest->d_package_off;
-    p.package_tenant = nest->d_package_tenant;
-    p.pack_off = (const long long*) nest->d_pack_off;
-    p.pack_topic = nest->d_pack_topic;
-    p.match_off = (const long long*) nest->d_match_off;
-    p.match_rank = nest->d_match_rank;
-    p.match_member = nest->d_match_member;
-    p.pack_pub_off = onest ? (const long long*) onest->d_pack_pub_off : nullptr;
-    p.pack_pub = onest ? onest->d_pack_pub : nullptr;
-    p.tenants = w->d_wr_tenants.p;
-    p.tenant_off = w->d_wr_tenant_off.p;
-    p.topics = d_topics;
-    p.topic_off = (const long long*) d_topic_off;
-    p.n_topics = L->n;
-    p.pub_off = (const long long*) d_pub_off;
-    p.pubpack = d_pubpack_bytes;
-    p.pubpack_off = (const long long*) d_pubpack_off;
-    p.mi_first = wt->d_first.p;
-    p.mi_off = wt->d_off.p;
-    p.mi_bytes = wt->d_bytes.p;
-    p.pair_pos = w->d_wr_pos.p;
-    p.pack_pos = p.pair_pos + np + 1;
-    p.package_pos = p.pack_pos + nk + 1;
-    p.check = w->d_wr_check.p;
-    p.req_off = w->d_req_off.p;
-    p.out = d_out;
-    size_t tmp_bytes = 0;
-    BFQ_CUDA_TRY(launch_wire_size(p, nullptr, &tmp_bytes, st));
-    BFQ_CUDA_TRY(w->d_wr_tmp.reserve(tmp_bytes + 256));
-    BFQ_CUDA_TRY(launch_wire_size(p, w->d_wr_tmp.p, &tmp_bytes, st));
-    unsigned long long chk[4];
-    BFQ_CUDA_TRY(cudaMemcpyAsync(chk, w->d_wr_check.p, sizeof(chk), cudaMemcpyDeviceToHost, st));
-    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
-    if (chk[0]) return fail(BFQ_E_INVALID, std::string(who) + ": d_pub_off / d_pubpack_off must start at 0 and never decrease, and "
-                                                               "every publisher of the nesting must be below d_pub_off[n_topics]");
-    const bool write = d_out && (int64_t) chk[1] <= out_cap;
-    if (write) BFQ_CUDA_TRY(launch_wire_write(p, st));
-    {
-        std::lock_guard<std::mutex> g(h->mu);
-        h->launches += write ? 10 : 8;
-    }
-    out->d_req_off = (const int64_t*) w->d_req_off.p;
-    out->n_bytes = (int64_t) chk[1];
-    out->n_match_infos = (int64_t) chk[2];
-    out->n_skipped = np - (int64_t) chk[2];
-    out->n_deliverers = (int32_t) D;
-    out->ordered_share_id = (int32_t) D - 1;
-    out->generation = L->snap->generation;
-    return BFQ_OK;
-}
-}  // namespace
-
-int32_t bfq_delivery_encode(const bfq_device_result* res, const bfq_delivery_result* nesting, const uint8_t* tenants,
-                            const int64_t* tenant_off, int32_t n_tenants, const uint8_t* d_topics, const int64_t* d_topic_off,
-                            const int64_t* d_pub_off, const uint8_t* d_pubpack_bytes, const int64_t* d_pubpack_off, uint8_t* d_out,
-                            int64_t out_cap, void* stream, bfq_delivery_wire_result* out) {
-    return run_encode(res, nesting, nullptr, tenants, tenant_off, n_tenants, d_topics, d_topic_off, d_pub_off, d_pubpack_bytes,
-                      d_pubpack_off, d_out, out_cap, stream, "bfq_delivery_encode", out);
-}
-
-int32_t bfq_delivery_encode_ordered(const bfq_device_result* res, const bfq_delivery_ordered_result* nesting, const uint8_t* tenants,
-                                    const int64_t* tenant_off, int32_t n_tenants, const uint8_t* d_topics, const int64_t* d_topic_off,
-                                    const int64_t* d_pub_off, const uint8_t* d_pubpack_bytes, const int64_t* d_pubpack_off,
-                                    uint8_t* d_out, int64_t out_cap, void* stream, bfq_delivery_wire_result* out) {
-    return run_encode(res, nesting ? &nesting->d : nullptr, nesting, tenants, tenant_off, n_tenants, d_topics, d_topic_off, d_pub_off,
-                      d_pubpack_bytes, d_pubpack_off, d_out, out_cap, stream, "bfq_delivery_encode_ordered", out);
-}
-
-namespace {
-// the hash of every MatchInfo in the snapshot's table (bfq_delivery_reply's join key), built once per snapshot on `st`
-int32_t ensure_mi_hash(Snapshot* s, const Snapshot::WireTable& wt, cudaStream_t st, std::shared_ptr<DeviceBuf<uint32_t>>* out) {
-    std::lock_guard<std::mutex> g(s->fan_mu);
-    if (!s->mi_hash) {
-        auto hb = std::make_shared<DeviceBuf<uint32_t>>();
-        BFQ_CUDA_TRY(hb->reserve(std::max<size_t>(wt.n_entries, 1)));
-        BFQ_CUDA_TRY(launch_mi_hash(wt.d_bytes.p, wt.d_off.p, (int64_t) wt.n_entries, hb->p, st));
-        BFQ_CUDA_TRY(cudaStreamSynchronize(st));   // other streams read it from now on
-        s->mi_hash = hb;
-    }
-    *out = s->mi_hash;
-    return BFQ_OK;
-}
-}  // namespace
-
-int32_t bfq_delivery_reply(const bfq_device_result* res, const bfq_delivery_result* nest, const uint8_t* tenants,
-                           const int64_t* tenant_off, int32_t n_tenants, const uint8_t* d_reply, const int64_t* d_reply_off,
-                           void* stream, bfq_delivery_reply_result* out) {
-    const char* who = "bfq_delivery_reply";
-    if (!res || !res->lease || !nest || !out) return fail(BFQ_E_INVALID, "bad argument");
-    auto* L = static_cast<DeviceLease*>(res->lease);
-    cudaStream_t st = (cudaStream_t) stream;
-    cudaEvent_t ev = nullptr;
-    int32_t rc = lease_use(res, st, who, &ev);
-    if (rc != BFQ_OK) return rc;
-    RecordOnExit rec(ev, st);
-    if (!d_reply || !d_reply_off) return fail(BFQ_E_INVALID, std::string(who) + ": NULL reply array");
-    if (n_tenants != L->ctx.n_tenants || (n_tenants > 0 && (!tenants || !tenant_off)))
-        return fail(BFQ_E_INVALID, std::string(who) + ": the tenant list must be the match's (" + std::to_string(L->ctx.n_tenants) + " tenants)");
-    if (!latest_nesting(L, nest))
-        return fail(BFQ_E_RANGE, std::string(who) + ": the nesting is not the latest delivery nesting of this device result");
-    bfq_index* h = L->h;
-    Workspace* w = L->ws;
-    std::shared_ptr<Snapshot::WireTable> wt;
-    if ((rc = ensure_wire_table(L->snap.get(), &wt)) != BFQ_OK) return rc;
-    std::shared_ptr<DeviceBuf<uint32_t>> mh;
-    if ((rc = ensure_mi_hash(L->snap.get(), *wt, st, &mh)) != BFQ_OK) return rc;
-    const int64_t np = nest->n_pairs, nk = nest->n_packs, ng = nest->n_packages;
-    const uint32_t D = (uint32_t) nest->n_deliverers;
-    if (np >= (int64_t) 1 << 31) return fail(BFQ_E_RANGE, std::string(who) + ": 2^31 or more pairs in one nesting");
-    uint64_t T = 2;
-    while (T < 2 * (uint64_t) np) T <<= 1;
-    const int64_t cap = std::max<int64_t>(np, 1), G = std::max<int64_t>(ng, 1);
-    const uint64_t nch = RP_MAX_CHUNKS + (uint64_t) ng;
-    BFQ_CUDA_TRY(w->d_rp_ctr.reserve(RP_CTR_N));
-    BFQ_CUDA_TRY(w->h_rp_ctr.reserve(RP_CTR_N));
-    BFQ_CUDA_TRY(w->d_rp_chunk_base.reserve((size_t) ng + 1));
-    BFQ_CUDA_TRY(w->d_rp_slot_key.reserve(T));
-    BFQ_CUDA_TRY(w->d_rp_slot_rpos.reserve(T));
-    BFQ_CUDA_TRY(w->d_rp_pkg_stale.reserve(2 * ((size_t) ng + 1)));
-    BFQ_CUDA_TRY(w->d_rp_dl_fail.reserve(D));
-    BFQ_CUDA_TRY(w->d_rp_ent_bad.reserve((size_t) G));
-    BFQ_CUDA_TRY(w->d_rp_pair_code.reserve((size_t) cap));
-    BFQ_CUDA_TRY(w->d_rp_status.reserve(D));
-    BFQ_CUDA_TRY(w->d_rp_dl_code.reserve(D));
-    BFQ_CUDA_TRY(w->d_rp_u32.reserve((size_t) D + 2 * (size_t) G + 3 * T + (size_t) cap * 6));
-    BFQ_CUDA_TRY(w->d_rp_ent.reserve(4 * (size_t) G));
-    BFQ_CUDA_TRY(w->d_rp_chunks.reserve(3 * nch));
-    BFQ_CUDA_TRY(w->d_rp_stale.reserve((size_t) cap));
-    BFQ_CUDA_TRY(w->d_rp_tenant_off.reserve((size_t) n_tenants + 1));
-    const int64_t tbytes = n_tenants > 0 ? tenant_off[n_tenants] : 0;
-    BFQ_CUDA_TRY(w->d_rp_tenants.reserve((size_t) std::max<int64_t>(tbytes, 1)));
-    if (n_tenants > 0) {
-        BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_rp_tenant_off.p, tenant_off, ((size_t) n_tenants + 1) * 8, cudaMemcpyHostToDevice, st));
-        if (tbytes > 0) BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_rp_tenants.p, tenants, (size_t) tbytes, cudaMemcpyHostToDevice, st));
-    }
-    ReplyParams p{};
-    p.n_packages = ng;
-    p.n_packs = nk;
-    p.n_pairs = np;
-    p.n_deliverers = D;
-    p.package_off = (const long long*) nest->d_package_off;
-    p.package_tenant = nest->d_package_tenant;
-    p.pack_off = (const long long*) nest->d_pack_off;
-    p.match_off = (const long long*) nest->d_match_off;
-    p.match_rank = nest->d_match_rank;
-    p.match_member = nest->d_match_member;
-    p.tenants = w->d_rp_tenants.p;
-    p.tenant_off = w->d_rp_tenant_off.p;
-    p.mi_first = wt->d_first.p;
-    p.mi_off = wt->d_off.p;
-    p.mi_bytes = wt->d_bytes.p;
-    p.mi_hash = mh->p;
-    p.reply = d_reply;
-    p.reply_off = (const long long*) d_reply_off;
-    p.ctr = w->d_rp_ctr.p;
-    p.dl_fail = w->d_rp_dl_fail.p;
-    p.dl_code = w->d_rp_dl_code.p;
-    uint32_t* u = w->d_rp_u32.p;
-    p.dl_entries = u;
-    u += D;
-    p.ent_pkg = u;
-    u += G;
-    p.pkg_claimed = u;
-    u += G;
-    p.slot_pair = u;
-    u += T;
-    p.slot_code = u;
-    u += T;
-    p.slot_rlen = u;
-    u += T;
-    p.pair_slot = u;
-    u += cap;
-    p.stale_list = u;
-    u += cap;
-    p.sort_key_in = u;
-    u += cap;
-    p.sort_key_out = u;
-    u += cap;
-    p.sort_val_in = u;
-    u += cap;
-    p.sort_val_out = u;
-    p.ent_s = w->d_rp_ent.p;
-    p.ent_e = p.ent_s + G;
-    p.ent_vs = p.ent_e + G;
-    p.ent_ve = p.ent_vs + G;
-    p.ent_bad = w->d_rp_ent_bad.p;
-    p.chunk_base = w->d_rp_chunk_base.p;
-    p.ch_guess = w->d_rp_chunks.p;
-    p.ch_exit = p.ch_guess + nch;
-    p.ch_start = p.ch_exit + nch;
-    p.slot_key = w->d_rp_slot_key.p;
-    p.slot_rpos = w->d_rp_slot_rpos.p;
-    p.table_mask = T - 1;
-    p.pkg_stale = w->d_rp_pkg_stale.p;
-    p.pkg_cursor = p.pkg_stale + ng + 1;
-    p.stale_cap = cap;
-    p.pair_code = w->d_rp_pair_code.p;
-    p.status = w->d_rp_status.p;
-    p.stale = w->d_rp_stale.p;
-    size_t tmp_bytes = 0;
-    BFQ_CUDA_TRY(launch_reply(p, nullptr, &tmp_bytes, st));
-    BFQ_CUDA_TRY(w->d_rp_tmp.reserve(tmp_bytes + 256));
-    BFQ_CUDA_TRY(launch_reply(p, w->d_rp_tmp.p, &tmp_bytes, st));
-    BFQ_CUDA_TRY(cudaMemcpyAsync(w->h_rp_ctr.p, w->d_rp_ctr.p, RP_CTR_N * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
-    {
-        std::lock_guard<std::mutex> g(h->mu);
-        h->launches += 17;
-    }
-    const unsigned long long* c = w->h_rp_ctr.p;
-    if (c[RP_BAD_OFF]) return fail(BFQ_E_INVALID, std::string(who) + ": d_reply_off must never decrease");
-    out->d_pair_code = w->d_rp_pair_code.p;
-    out->d_status = w->d_rp_status.p;
-    out->d_stale = w->d_rp_stale.p;
-    for (int i = 0; i < 8; i++) out->n_code[i] = (int64_t) c[RP_N_CODE + i];
-    out->n_pairs = np;
-    out->n_stale = (int64_t) c[RP_N_STALE];
-    out->n_fallback = (int32_t) c[RP_N_FALLBACK];
-    out->n_deliverers = (int32_t) D;
-    out->ordered_share_id = (int32_t) D - 1;
-    out->generation = L->snap->generation;
-    return BFQ_OK;
-}
-
-int32_t bfq_fanout_deliverer(bfq_index* h, int32_t id, int32_t* sub_broker_id, uint8_t* key_out, int64_t key_cap, int64_t* key_len) {
-    if (!h || id < 0) return fail(BFQ_E_INVALID, "bad argument");
-    std::lock_guard<std::mutex> g(h->deliverers->mu);
-    if ((size_t) id >= h->deliverers->list.size()) return fail(BFQ_E_RANGE, "deliverer id out of range (the last id of a fan-out result is the ordered-share marker)");
-    const auto& e = h->deliverers->list[(size_t) id];
-    if (sub_broker_id) *sub_broker_id = e.first;
-    if (key_len) *key_len = (int64_t) e.second.size();
-    if (key_out && (int64_t) e.second.size() <= key_cap) memcpy(key_out, e.second.data(), e.second.size());
-    return BFQ_OK;
 }
 
 // ---------------------------------------------------------------- codec exports

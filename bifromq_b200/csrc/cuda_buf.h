@@ -93,6 +93,33 @@ using PinnedBuf = CudaBuf<T, true>;
 
 inline int32_t fail(int32_t code, const std::string& msg) { return set_error(code, msg); }
 
+// Typed arrays placed one after another in one block, each at a 256-byte boundary. With base == nullptr it only counts the
+// bytes; with base set it hands out the pointers.
+struct Carve {
+    uint8_t* base = nullptr;
+    size_t bytes = 0;
+    template <typename T>
+    T* take(size_t n) {
+        bytes = (bytes + 255) & ~(size_t) 255;
+        T* p = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
+        bytes += n * sizeof(T);
+        return p;
+    }
+};
+
+// A layout written once (layout(Carve&) takes every array of a call) and run twice: to size `arena` (contents not kept), then
+// to hand out the arrays in it. `what` names the arena in the error message.
+template <typename Layout>
+int32_t carve(DeviceBuf<uint8_t>& arena, const char* what, Layout&& layout) {
+    Carve count;
+    layout(count);
+    const cudaError_t e = arena.reserve(count.bytes);
+    if (e != cudaSuccess) return fail(BFQ_E_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
+    Carve place{arena.p};
+    layout(place);
+    return BFQ_OK;
+}
+
 }  // namespace bfq
 
 // returns BFQ_E_CUDA from the enclosing function, with the failed expression and CUDA's message in bfq_last_error()

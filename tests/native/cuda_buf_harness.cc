@@ -117,6 +117,41 @@ int main() {
         put("try_error", quoted(bfq_last_error()));
         put("try_buffer_empty", (long) (e.p == nullptr && e.cap == 0));
         put("try_ok_rc", (long) reserve_or_fail(e, 64));
+
+        // ---- carve: one layout sizes the arena and hands out its arrays, each at a 256-byte boundary
+        DeviceBuf<uint8_t> arena;
+        uint8_t* a8 = nullptr;
+        unsigned long long* a64 = nullptr;
+        uint32_t* a32 = nullptr;
+        uint16_t* a16 = nullptr;
+        size_t n64 = 5;
+        auto layout = [&](bfq::Carve& c) {
+            a8 = c.take<uint8_t>(3);
+            a64 = c.take<unsigned long long>(n64);
+            a32 = c.take<uint32_t>(0);
+            a16 = c.take<uint16_t>(2);
+        };
+        auto offsets = [&]() {
+            const uint8_t* b = arena.p;
+            return "[" + std::to_string((const uint8_t*) a8 - b) + ", " + std::to_string((const uint8_t*) a64 - b) + ", " +
+                   std::to_string((const uint8_t*) a32 - b) + ", " + std::to_string((const uint8_t*) a16 - b) + "]";
+        };
+        m = st.log.size();
+        put("carve_rc", (long) bfq::carve(arena, "arena", layout));
+        put("carve_log", since(m));
+        put("carve_offsets", offsets());
+        m = st.log.size();
+        bfq::carve(arena, "arena", layout);
+        put("carve_fits_log", since(m));
+        n64 = 100;
+        m = st.log.size();
+        bfq::carve(arena, "arena", layout);
+        put("carve_grow_log", since(m));
+        put("carve_grow_offsets", offsets());
+        n64 = 1000;
+        st.fail_next_alloc = true;
+        put("carve_failed_rc", (long) bfq::carve(arena, "test arena", layout));
+        put("carve_failed_error", quoted(bfq_last_error()));
     }
     // every buffer above is out of scope: each allocation has been freed exactly once
     put("device_allocs", st.device_allocs);

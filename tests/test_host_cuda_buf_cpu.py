@@ -50,6 +50,13 @@ def test_cuda_buf_allocation_rules(tmp_path):
     assert o["try_rc"] == BFQ_E_CUDA and o["try_error"] == "buf.reserve(n): out of memory"
     assert o["try_buffer_empty"] == 1 and o["try_ok_rc"] == 0
 
+    # carve: the counting pass sizes the arena (3 bytes, 5 x 8 at 256, an empty array and 2 x 2 at 512); the placing pass
+    # hands out those offsets. Arrays never overlap and each starts on a 256-byte boundary.
+    assert o["carve_rc"] == 0 and o["carve_log"] == ["malloc 516"] and o["carve_offsets"] == [0, 256, 512, 512]
+    assert o["carve_fits_log"] == []
+    assert o["carve_grow_log"] == ["free", "malloc 1284"] and o["carve_grow_offsets"] == [0, 256, 1280, 1280]
+    assert o["carve_failed_rc"] == BFQ_E_CUDA and o["carve_failed_error"] == "test arena: out of memory"
+
     # every allocation was freed exactly once
     assert o["device_allocs"] == o["device_frees"] > 0
     assert o["pinned_allocs"] == o["pinned_frees"] == 2
