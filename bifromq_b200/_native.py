@@ -32,6 +32,12 @@ class BfqDeviceResult(C.Structure):
                 ("tier0_ms", C.c_double), ("generation", C.c_uint64), ("lease", C.c_void_p)]
 
 
+class BfqRDeviceResult(C.Structure):
+    _fields_ = [("d_offsets", C.c_void_p), ("d_ids", C.c_void_p), ("d_total", C.c_void_p), ("n_filters", C.c_int64),
+                ("n_ids", C.c_int64), ("n_ranges", C.c_int64), ("n_overflow_filters", C.c_int64), ("generation", C.c_uint64),
+                ("device_ms", C.c_double), ("kernel_ms", C.c_double), ("lease", C.c_void_p)]
+
+
 class BfqGathered(C.Structure):
     _fields_ = [("d_route_count", C.c_void_p), ("d_span_count", C.c_void_p), ("d_ranges", C.c_void_p),
                 ("topic_base", C.POINTER(C.c_int64)), ("range_base", C.POINTER(C.c_int64)), ("topic_count", C.POINTER(C.c_int64)),
@@ -155,7 +161,11 @@ _SIGNATURES = {
     "bfq_rresult_ids": (_vp, [_vp, C.POINTER(_i64)]),
     "bfq_rresult_total_matches": (_vp, [_vp]),
     "bfq_rresult_timings": (_i32, [_vp, _vp, _i32]),
+    "bfq_rresult_generation": (C.c_uint64, [_vp]),
     "bfq_rresult_free": (None, [_vp]),
+    "bfq_rmatch_device": (_i32, [_vp, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp, _vp, C.POINTER(BfqRDeviceResult)]),
+    "bfq_rdevice_result_release": (None, [C.POINTER(BfqRDeviceResult)]),
+    "bfq_rretain_keys_device": (_i32, [_vp, C.POINTER(BfqRDeviceResult), _vp, _vp, _i64, _vp, C.POINTER(_i64)]),
 }
 
 _lib = None

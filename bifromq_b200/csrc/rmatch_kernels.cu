@@ -22,12 +22,14 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <atomic>
 #include <chrono>
 #include <cstring>
 #include <map>
 #include <memory>
 #include <mutex>
 #include <set>
+#include <shared_mutex>
 #include <string>
 #include <tuple>
 #include <unordered_map>
@@ -40,6 +42,7 @@
 #include "cuda_buf.h"
 #include "trie_layout.h"
 #include "hash_probe.cuh"
+#include "lease.h"
 #include "match_kernels.cuh"
 
 using namespace bfq;
@@ -490,16 +493,134 @@ __global__ void __launch_bounds__(256) rinsert_edges_kernel(const Slot* __restri
     }
 }
 
+// *bad = 1 if some filter_tenant of a device-resident batch lies outside [0, n_tenants): the match kernel indexes the tenant
+// table with it, so the call fails before that kernel runs
+__global__ void rcheck_tenants_kernel(int64_t n, const int32_t* filter_tenant, int32_t n_tenants, unsigned long long* bad) {
+    const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && (filter_tenant[i] < 0 || filter_tenant[i] >= n_tenants)) *bad = 1;
+}
+
+// len[i] = length of the retain key of ids[i] (key_off: the id table's device key offsets)
+__global__ void rkey_len_kernel(int64_t n, const int64_t* ids, const int64_t* key_off, int64_t* len) {
+    const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) {
+        const int64_t id = ids[i];
+        len[i] = key_off[id + 1] - key_off[id];
+    }
+}
+
+// one warp per id: its retain key to out[out_off[i] ..)
+__global__ void __launch_bounds__(256) rkey_copy_kernel(int64_t n, const int64_t* ids, const int64_t* key_off,
+                                                        const uint8_t* key_bytes, const int64_t* out_off, uint8_t* out) {
+    const int lane = threadIdx.x & 31;
+    const int64_t i = ((int64_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= n) return;
+    const int64_t id = ids[i];
+    const int64_t b = key_off[id], len = key_off[id + 1] - b;
+    const uint8_t* src = key_bytes + b;
+    uint8_t* dst = out + out_off[i];
+    for (int64_t x = lane; x < len; x += 32) dst[x] = src[x];
+}
+
 }  // namespace
 
+// The retain keys of an id table on the device: key i is bytes[off[i] .. off[i + 1]). Buffers that must grow are replaced, not
+// reallocated: a gather still running on another stream keeps reading the old ones, which its result holds until released.
+struct KeyBufs {
+    int device = 0;
+    DeviceBuf<uint8_t> bytes;
+    DeviceBuf<int64_t> off;
+    ~KeyBufs() { cudaSetDevice(device); }   // runs before the members are destroyed: the buffers are freed on this device
+};
+
 // id -> (tenant, topic); tombstones keep their slot. bfq_rindex_reset starts a new table, so ids restart at 0 there while the
-// snapshot and its results still name ids of the old one.
-using IdTable = std::vector<std::pair<std::string, std::string>>;
+// snapshot and its results still name ids of the old one. Append-only: add / load_keys push_back under the handle lock held
+// exclusive, and every host reader of `e` (a match's result, key calls, lookup) holds it shared, so no reader sees a
+// reallocation. The device key table belongs to the id table and goes with it.
+struct IdTable {
+    std::vector<std::pair<std::string, std::string>> e;
+    std::mutex key_mu;                    // the key table below
+    std::shared_ptr<KeyBufs> keys;        // built on the first key call, extended for ids added since
+    int64_t key_ids = 0, key_bytes = 0;   // ids and bytes it holds
+    std::atomic<int64_t> key_device_bytes{0};
+};
 
 struct bfq_rresult {
     std::vector<int64_t> offsets, ids, totals;
     double ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    std::shared_ptr<const IdTable> by_id;   // the id table of the snapshot the match ran on
+    uint64_t generation = 0;
+    std::shared_ptr<IdTable> by_id;   // the id table of the snapshot the match ran on
+};
+
+// Everything ONE inverse match in flight needs: its stream, device scratch and outputs, pinned counters. Leased from the
+// handle's pool for a call, and for a device result until bfq_rdevice_result_release (its arrays live here), so concurrent
+// matches on one handle never share a buffer.
+struct RWorkspace {
+    int device = 0;
+    cudaStream_t stream = nullptr;
+    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};   // [0,1] around all kernels of a match, [2,3] around rmatch_kernel
+    cudaEvent_t ev_in = nullptr;        // device path: recorded on the caller's stream, where the batch was written
+    std::vector<cudaEvent_t> ev_use;    // device result: one per stream a key gather ran on (RLease::used_on), created on demand
+    std::atomic<int64_t> bytes_held{0}; // device_bytes() when the last call on it ended (bfq_rindex_stats)
+    DeviceBuf<uint8_t> d_in, d_scan_tmp, d_key_tmp;   // d_in: the host path's batch, one block
+    PinnedBuf<int32_t> h_tenant_root;
+    PinnedBuf<unsigned long long> h_small;   // [0, RC_COUNT) the match counters, [RC_COUNT] a total read back
+    DeviceBuf<int64_t> d_ids, d_key_len;
+    DeviceBuf<int32_t> d_tenant_root;
+    DeviceBuf<uint32_t> d_span_begin, d_span_count, d_overflow;
+    DeviceBuf<unsigned long long> d_total, d_kept, d_offsets, d_counters;
+    DeviceBuf<uint2> d_ranges, d_scratch;
+    // locality order of a batch of filters (match_kernels.cu: launch_order, without de-duplication)
+    DeviceBuf<uint32_t> d_ord_keys, d_ord_leader, d_order, d_hist;
+    DeviceBuf<unsigned long long> d_ord_ctr;
+
+    cudaError_t init(int dev) {
+        device = dev;
+        cudaError_t e = cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking);
+        for (auto& x : ev)
+            if (e == cudaSuccess) e = cudaEventCreate(&x);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev_in, cudaEventDisableTiming);
+        return e;
+    }
+    int64_t device_bytes() const {
+        return (int64_t) (d_in.bytes() + d_scan_tmp.bytes() + d_key_tmp.bytes() + d_ids.bytes() + d_key_len.bytes() +
+                          d_tenant_root.bytes() + d_span_begin.bytes() + d_span_count.bytes() + d_overflow.bytes() +
+                          d_total.bytes() + d_kept.bytes() + d_offsets.bytes() + d_counters.bytes() + d_ranges.bytes() +
+                          d_scratch.bytes() + d_ord_keys.bytes() + d_ord_leader.bytes() + d_order.bytes() + d_hist.bytes() +
+                          d_ord_ctr.bytes());
+    }
+    ~RWorkspace() {
+        cudaSetDevice(device);   // the buffers are freed after this body, on this device
+        for (auto& e : ev) if (e) cudaEventDestroy(e);
+        if (ev_in) cudaEventDestroy(ev_in);
+        for (auto& e : ev_use) cudaEventDestroy(e);
+        if (stream) cudaStreamDestroy(stream);
+    }
+};
+
+// the workspaces of one handle. Shared with every device result in flight, so that releasing a result after its handle was
+// destroyed still has a place to return its workspace to.
+struct RPool {
+    std::mutex mu;
+    std::vector<RWorkspace*> idle;
+    std::vector<RWorkspace*> held;   // every workspace alive: idle and leased
+    int device = 0;
+    bool closed = false;
+    ~RPool() {
+        cudaSetDevice(device);
+        for (RWorkspace* w : idle) delete w;
+    }
+};
+
+// a device result (bfq_rmatch_device .. bfq_rdevice_result_release)
+struct RLease {
+    bfq_rindex* h = nullptr;
+    std::shared_ptr<RPool> pool;
+    RWorkspace* ws = nullptr;
+    std::shared_ptr<IdTable> by_id;   // the id table of the snapshot the match ran on
+    std::mutex use_mu;                // key gathers on this result, one at a time (they share the workspace's scratch)
+    std::vector<cudaStream_t> used_on;              // ws->ev_use[i]: the last gather on used_on[i]
+    std::vector<std::shared_ptr<KeyBufs>> keys;     // key buffers the gathers read, held until release
 };
 
 // where a live tenant's trie sits in the snapshot (see the layout comment above rebuild_full)
@@ -511,10 +632,12 @@ struct TenantRegion {
 
 struct bfq_rindex {
     int device = 0;
-    std::mutex mu;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};   // [0,1] around all kernels of a match, [2,3] around rmatch_kernel
-    PinnedBuf<unsigned long long> h_small;   // pinned scalars
+    // Matches hold it shared from reading the snapshot's tables until their device reads of them have finished (a commit
+    // patches the device tables in place); add / load_keys / remove / reset / commit hold it exclusive.
+    std::shared_mutex mu;
+    std::mutex gate;   // a writer holds it while it waits for and holds mu: matches arriving meanwhile queue behind it
+    cudaStream_t stream = nullptr;   // commits
+    std::shared_ptr<RPool> pool = std::make_shared<RPool>();
     // staging: (tenant, topic) -> id ; id -> (tenant, topic)
     std::map<std::pair<std::string, std::string>, int64_t> staged;
     std::shared_ptr<IdTable> by_id = std::make_shared<IdTable>();   // staging: add / load_keys append here
@@ -522,7 +645,8 @@ struct bfq_rindex {
     std::set<std::string> dirty;   // tenants whose staged topic set changed since the last commit
     bool need_full = true;         // the next commit is a full build (no snapshot yet, reset, bulk load onto an empty handle)
     bool have_snapshot = false;
-    std::shared_ptr<const IdTable> committed;   // the table by_id was when the snapshot was built (append-only since)
+    uint64_t generation = 0;       // successful commits so far: the snapshot's generation
+    std::shared_ptr<IdTable> committed;   // the table by_id was when the snapshot was built (append-only since)
     // snapshot
     std::unordered_map<std::string, int32_t> tenant_root;
     std::unordered_map<std::string, TenantRegion> regions;   // the live tenants' regions
@@ -540,35 +664,40 @@ struct bfq_rindex {
     DeviceBuf<int64_t> d_dfs_to_id, d_bfs_to_id;
     DeviceBuf<Slot> d_new_slots;                // slot images of a delta commit
     DeviceBuf<unsigned long long> d_ins_ctr;
-    // workspace
-    DeviceBuf<uint8_t> d_filters, d_scan_tmp;
-    DeviceBuf<int64_t> d_filter_off, d_limit, d_ids;
-    DeviceBuf<int32_t> d_filter_tenant, d_tenant_root;
-    DeviceBuf<uint32_t> d_span_begin, d_span_count, d_overflow;
-    DeviceBuf<unsigned long long> d_total, d_kept, d_offsets, d_counters;
-    DeviceBuf<uint2> d_ranges, d_scratch;
-    // locality order of a batch of filters (match_kernels.cu: launch_order, without de-duplication)
-    DeviceBuf<uint32_t> d_ord_keys, d_ord_leader, d_order, d_hist;
-    DeviceBuf<unsigned long long> d_ord_ctr;
-    int64_t launches = 0;
+    std::atomic<int64_t> launches{0};
 
-    int64_t device_bytes() const {
+    int64_t snapshot_bytes() const {
         return (int64_t) (d_nodes.bytes() + d_slots.bytes() + d_tags.bytes() + d_dfs_to_id.bytes() + d_bfs_to_id.bytes() +
-                          d_filters.bytes() + d_scan_tmp.bytes() + d_filter_off.bytes() + d_limit.bytes() + d_ids.bytes() +
-                          d_filter_tenant.bytes() + d_tenant_root.bytes() + d_span_begin.bytes() + d_span_count.bytes() +
-                          d_overflow.bytes() + d_total.bytes() + d_kept.bytes() + d_offsets.bytes() + d_counters.bytes() +
-                          d_ranges.bytes() + d_scratch.bytes() + d_ord_keys.bytes() + d_ord_leader.bytes() + d_order.bytes() +
-                          d_hist.bytes() + d_ord_ctr.bytes() + d_new_slots.bytes() + d_ins_ctr.bytes());
+                          d_new_slots.bytes() + d_ins_ctr.bytes());
     }
 
     ~bfq_rindex() {
         cudaSetDevice(device);   // the buffers are freed after this body, on this device
-        for (auto& e : ev) if (e) cudaEventDestroy(e);
+        std::vector<RWorkspace*> idle;
+        {
+            std::lock_guard<std::mutex> g(pool->mu);
+            pool->closed = true;   // workspaces still leased are freed when they come back
+            idle.swap(pool->idle);
+            pool->held.clear();
+        }
+        for (RWorkspace* w : idle) delete w;
         if (stream) cudaStreamDestroy(stream);
     }
 };
 
 namespace {
+
+// The handle lock for matches and for writers. std::shared_mutex lets new readers in while a writer waits, so a steady stream
+// of matches could hold a commit off indefinitely; the gate makes matches that arrive after a waiting writer wait behind it.
+std::shared_lock<std::shared_mutex> read_lock(bfq_rindex* h) {
+    { std::lock_guard<std::mutex> wait_for_writers(h->gate); }
+    return std::shared_lock<std::shared_mutex>(h->mu);
+}
+struct WriteLock {
+    std::lock_guard<std::mutex> gate;
+    std::unique_lock<std::shared_mutex> g;
+    explicit WriteLock(bfq_rindex* h) : gate(h->gate), g(h->mu) {}
+};
 
 struct HNode {  // host build node
     std::map<std::string, uint32_t> children;   // name -> host node index (sorted => '$' children form one run)
@@ -937,6 +1066,274 @@ int32_t commit_delta(bfq_rindex* h) {
     return BFQ_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ workspaces
+constexpr size_t POOL_KEEP = 4;   // idle workspaces kept for reuse; more are freed when they come back
+
+int32_t acquire(bfq_rindex* h, RWorkspace** out) {
+    RPool& pool = *h->pool;
+    {
+        std::lock_guard<std::mutex> g(pool.mu);
+        if (!pool.idle.empty()) {
+            *out = pool.idle.back();
+            pool.idle.pop_back();
+            return BFQ_OK;
+        }
+    }
+    auto* w = new RWorkspace();
+    const cudaError_t e = w->init(h->device);
+    if (e != cudaSuccess) {
+        delete w;
+        return fail(BFQ_E_CUDA, std::string("workspace: ") + cudaGetErrorString(e));
+    }
+    std::lock_guard<std::mutex> g(pool.mu);
+    pool.held.push_back(w);
+    *out = w;
+    return BFQ_OK;
+}
+
+// the caller has waited for everything enqueued on w
+void give_back(const std::shared_ptr<RPool>& pool, RWorkspace* w) {
+    if (!w) return;
+    w->bytes_held = w->device_bytes();
+    {
+        std::lock_guard<std::mutex> g(pool->mu);
+        if (!pool->closed && pool->idle.size() < POOL_KEEP) {
+            pool->idle.push_back(w);
+            return;
+        }
+        pool->held.erase(std::remove(pool->held.begin(), pool->held.end(), w), pool->held.end());
+    }
+    cudaSetDevice(pool->device);
+    delete w;
+}
+
+// a workspace for the length of one call: back to the pool on every return, after its stream has drained
+struct CallLease {
+    std::shared_ptr<RPool> pool;
+    RWorkspace* w = nullptr;
+    ~CallLease() {
+        if (w) {
+            cudaStreamSynchronize(w->stream);
+            give_back(pool, w);
+        }
+    }
+};
+
+// ------------------------------------------------------------------------------------------------ retain keys on the device
+// Brings the device key table of t up to every id t holds and returns its buffers. The caller holds the handle lock (the ids
+// are read here); uploads run on st and are finished on return.
+int32_t extend_keys(IdTable& t, int device, cudaStream_t st, std::shared_ptr<KeyBufs>* out) {
+    std::lock_guard<std::mutex> g(t.key_mu);
+    const int64_t n = (int64_t) t.e.size();
+    if (t.keys && t.key_ids == n) {
+        *out = t.keys;
+        return BFQ_OK;
+    }
+    std::string blob;
+    std::vector<int64_t> ends;   // off[key_ids + 1 .. n]
+    ends.reserve((size_t) (n - t.key_ids));
+    for (int64_t i = t.key_ids; i < n; i++) {
+        blob += make_retain_key(t.e[(size_t) i].first, t.e[(size_t) i].second);
+        ends.push_back(t.key_bytes + (int64_t) blob.size());
+    }
+    const int64_t n_bytes = t.key_bytes + (int64_t) blob.size();
+    std::shared_ptr<KeyBufs> kb = t.keys;
+    if (!kb || kb->off.cap < (size_t) n + 1 || kb->bytes.cap < (size_t) std::max<int64_t>(n_bytes, 1)) {
+        auto nb = std::make_shared<KeyBufs>();
+        nb->device = device;
+        const size_t want_off = std::max((size_t) n + 1, kb ? kb->off.cap + kb->off.cap / 2 : 0);
+        const size_t want_bytes = std::max((size_t) std::max<int64_t>(n_bytes, 1), kb ? kb->bytes.cap + kb->bytes.cap / 2 : 0);
+        BFQ_CUDA_TRY(nb->off.reserve(want_off));
+        BFQ_CUDA_TRY(nb->bytes.reserve(want_bytes));
+        if (kb) {
+            BFQ_CUDA_TRY(cudaMemcpyAsync(nb->off.p, kb->off.p, (size_t) (t.key_ids + 1) * 8, cudaMemcpyDeviceToDevice, st));
+            if (t.key_bytes)
+                BFQ_CUDA_TRY(cudaMemcpyAsync(nb->bytes.p, kb->bytes.p, (size_t) t.key_bytes, cudaMemcpyDeviceToDevice, st));
+        } else {
+            BFQ_CUDA_TRY(cudaMemsetAsync(nb->off.p, 0, 8, st));   // off[0]
+        }
+        kb = nb;
+    }
+    // appended past what earlier gathers read: they keep running on the same buffers
+    if (!ends.empty())
+        BFQ_CUDA_TRY(cudaMemcpyAsync(kb->off.p + t.key_ids + 1, ends.data(), ends.size() * 8, cudaMemcpyHostToDevice, st));
+    if (!blob.empty()) BFQ_CUDA_TRY(cudaMemcpyAsync(kb->bytes.p + t.key_bytes, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
+    t.keys = kb;
+    t.key_ids = n;
+    t.key_bytes = n_bytes;
+    t.key_device_bytes = (int64_t) (kb->bytes.bytes() + kb->off.bytes());
+    *out = kb;
+    return BFQ_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ the match
+struct RCoreIn {
+    const uint8_t* tenants;
+    const int64_t* tenant_off;
+    int32_t n_tenants;
+    const uint8_t* d_filters;
+    const int64_t* d_filter_off;
+    const int32_t* d_filter_tenant;
+    int64_t n;
+    const int64_t* d_limit;      // nullptr = unlimited
+    bool check_tenants;          // filter_tenant has not been range-checked on the host
+};
+struct RCoreOut {
+    unsigned long long n_ids = 0, n_ranges = 0, n_overflow = 0;
+};
+
+// The match of a batch resident on the device, enqueued on w->stream: tenant roots, locality order, rmatch_kernel (re-run
+// while the range buffer grows), the limit, the id offsets and rexpand_kernel. On return the ids are enqueued to
+// w->d_ids, d_offsets[n + 1] / d_total[n] hold offsets and totals, and ev[1] follows the last kernel. The caller holds h->mu
+// shared and keeps it until w->stream has drained: rexpand_kernel is the last to read the snapshot's tables.
+int32_t rmatch_core(bfq_rindex* h, RWorkspace* w, const RCoreIn& in, RCoreOut* out) {
+    cudaStream_t st = w->stream;
+    const int64_t n = in.n;
+    const int32_t n_tenants = in.n_tenants;
+    const size_t nn = (size_t) std::max<int64_t>(n, 1), nt = (size_t) std::max(n_tenants, 1);
+    unsigned long long* hc = nullptr;
+    BFQ_CUDA_TRY(w->h_small.reserve(RC_COUNT + 1));
+    hc = w->h_small.p;
+    BFQ_CUDA_TRY(w->d_offsets.reserve(nn + 1));
+    if (n == 0) {
+        BFQ_CUDA_TRY(cudaMemsetAsync(w->d_offsets.p, 0, 8, st));
+        return BFQ_OK;
+    }
+    BFQ_CUDA_TRY(w->h_tenant_root.reserve(nt));
+    for (int32_t t = 0; t < n_tenants; t++) {
+        auto it = h->tenant_root.find(std::string((const char*) in.tenants + in.tenant_off[t], (size_t) (in.tenant_off[t + 1] - in.tenant_off[t])));
+        w->h_tenant_root.p[t] = it != h->tenant_root.end() ? it->second : -1;
+    }
+    BFQ_CUDA_TRY(w->d_tenant_root.reserve(nt));
+    BFQ_CUDA_TRY(w->d_span_begin.reserve(nn));
+    BFQ_CUDA_TRY(w->d_span_count.reserve(nn));
+    BFQ_CUDA_TRY(w->d_overflow.reserve(nn));
+    BFQ_CUDA_TRY(w->d_total.reserve(nn));
+    BFQ_CUDA_TRY(w->d_kept.reserve(nn + 1));
+    BFQ_CUDA_TRY(w->d_counters.reserve(RC_COUNT));
+    if (w->d_ranges.cap == 0) BFQ_CUDA_TRY(w->d_ranges.reserve(std::max<size_t>(1 << 18, 8 * nn)));
+    if (n_tenants > 0)
+        BFQ_CUDA_TRY(cudaMemcpyAsync(w->d_tenant_root.p, w->h_tenant_root.p, (size_t) n_tenants * 4, cudaMemcpyHostToDevice, st));
+    BFQ_CUDA_TRY(cudaEventRecord(w->ev[0], st));   // the inputs are (enqueued to be) resident: device time of the kernels from here
+    if (in.check_tenants) {
+        BFQ_CUDA_TRY(cudaMemsetAsync(w->d_counters.p, 0, RC_COUNT * sizeof(unsigned long long), st));
+        rcheck_tenants_kernel<<<(unsigned) ((n + 255) / 256), 256, 0, st>>>(n, in.d_filter_tenant, n_tenants, w->d_counters.p + RC_COUNT - 1);
+        h->launches++;
+        BFQ_CUDA_TRY(cudaGetLastError());
+        BFQ_CUDA_TRY(cudaMemcpyAsync(hc + RC_COUNT - 1, w->d_counters.p + RC_COUNT - 1, 8, cudaMemcpyDeviceToHost, st));
+        BFQ_CUDA_TRY(cudaStreamSynchronize(st));
+        if (hc[RC_COUNT - 1] != 0) return fail(BFQ_E_RANGE, "filter_tenant out of range");
+    }
+
+    RMatchParams p{};
+    p.nodes = h->d_nodes.p;
+    p.slots = h->d_slots.p;
+    p.tags = reinterpret_cast<const uint4*>(h->d_tags.p);
+    p.n_blocks = h->n_blocks;
+    p.filters = in.d_filters;
+    p.filter_off = in.d_filter_off;
+    p.filter_tenant = in.d_filter_tenant;
+    p.tenant_root = w->d_tenant_root.p;
+    p.n_filters = n;
+    p.span_begin = w->d_span_begin.p;
+    p.span_count = w->d_span_count.p;
+    p.total = w->d_total.p;
+    p.overflow_list = w->d_overflow.p;
+    p.counters = w->d_counters.p;
+    const int sms = device_sm_count();
+    int ctas_per_sm = 4;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, rmatch_kernel<false>, R_WARPS * 32, 0);
+    ctas_per_sm = std::max(1, ctas_per_sm);
+    // filters that share a tenant and leading levels walk the same part of the topic trie: group them so that the warps
+    // running at the same time hit the same node records in L2 (the forward path's locality order, reused)
+    const uint32_t* order = nullptr;
+    if (n >= 4096) {
+        BFQ_CUDA_TRY(w->d_ord_keys.reserve(nn));
+        BFQ_CUDA_TRY(w->d_ord_leader.reserve(nn));
+        BFQ_CUDA_TRY(w->d_order.reserve(nn));
+        BFQ_CUDA_TRY(w->d_hist.reserve(order_scratch_words(n, n_tenants)));
+        BFQ_CUDA_TRY(w->d_ord_ctr.reserve(CTR_COUNT));
+        OrderParams q{};
+        q.n_topics = n;
+        q.topics = in.d_filters;
+        q.topic_off = in.d_filter_off;
+        q.topic_tenant = in.d_filter_tenant;
+        q.n_tenants = n_tenants;
+        q.keys = w->d_ord_keys.p;
+        q.leader = w->d_ord_leader.p;
+        q.order = w->d_order.p;
+        q.hash_tab = nullptr;
+        q.hash_mask = 0;
+        q.hist = w->d_hist.p;
+        q.dedup = 0;
+        q.counters = w->d_ord_ctr.p;
+        BFQ_CUDA_TRY(launch_order(q, st));
+        h->launches += 3;
+        order = q.order;
+    }
+    for (int attempt = 0; attempt < 8; attempt++) {
+        p.ranges = w->d_ranges.p;
+        p.ranges_cap = w->d_ranges.cap;
+        p.work_list = order;
+        p.n_work = 0;
+        BFQ_CUDA_TRY(cudaMemsetAsync(w->d_counters.p, 0, RC_COUNT * sizeof(unsigned long long), st));
+        int64_t ctas = std::min<int64_t>((n + R_WARPS - 1) / R_WARPS, (int64_t) sms * ctas_per_sm);
+        BFQ_CUDA_TRY(cudaEventRecord(w->ev[2], st));
+        rmatch_kernel<false><<<(unsigned) std::max<int64_t>(ctas, 1), R_WARPS * 32, 0, st>>>(p);
+        BFQ_CUDA_TRY(cudaEventRecord(w->ev[3], st));
+        h->launches++;
+        BFQ_CUDA_TRY(cudaGetLastError());
+        BFQ_CUDA_TRY(cudaMemcpyAsync(hc, w->d_counters.p, RC_COUNT * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+        BFQ_CUDA_TRY(cudaStreamSynchronize(st));
+        if (hc[RC_OVERFLOW] > 0) {
+            const uint64_t capF = (uint64_t) h->max_nodes_per_depth + 2;
+            const uint64_t capR = 3 * ((uint64_t) h->n_nodes + 2) + 2;
+            const uint64_t per_warp = 2 * capF + capR;
+            uint64_t warps = std::min<uint64_t>(hc[RC_OVERFLOW], std::max<uint64_t>(8, (1ull << 31) / (per_warp * sizeof(uint2))));
+            warps = std::min<uint64_t>((warps + 7) / 8 * 8, (uint64_t) sms * 8);
+            BFQ_CUDA_TRY(w->d_scratch.reserve((size_t) (warps * per_warp)));
+            p.scratch = w->d_scratch.p;
+            p.scratch_frontier_cap = capF;
+            p.scratch_ranges_cap = capR;
+            p.work_list = w->d_overflow.p;
+            p.n_work = (int64_t) hc[RC_OVERFLOW];
+            rmatch_kernel<true><<<(unsigned) (warps / 8), R_WARPS * 32, 0, st>>>(p);
+            h->launches++;
+            BFQ_CUDA_TRY(cudaGetLastError());
+            BFQ_CUDA_TRY(cudaMemcpyAsync(hc, w->d_counters.p, RC_COUNT * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+            BFQ_CUDA_TRY(cudaStreamSynchronize(st));
+            if (hc[RC_ERROR] != 0) return fail(BFQ_E_STATE, "tier-2 scratch exhausted");
+        }
+        if (hc[RC_RANGES] <= w->d_ranges.cap) break;
+        const size_t want = (size_t) (hc[RC_RANGES] + hc[RC_RANGES] / 4 + 1024);
+        if (want >= 0xFFFFFFF0ull || attempt == 7) return fail(BFQ_E_RANGE, "too many matched ranges in one batch; split the batch");
+        BFQ_CUDA_TRY(w->d_ranges.reserve(want));
+    }
+    out->n_ranges = hc[RC_RANGES];
+    out->n_overflow = hc[RC_OVERFLOW];
+    // kept = min(total, limit), kept[n] = 0; exclusive scan over n + 1, so offsets[n] is the grand total; expand to ids
+    rkept_kernel<<<(unsigned) ((n + 255) / 256), 256, 0, st>>>(n, w->d_total.p, in.d_limit, w->d_kept.p);
+    BFQ_CUDA_TRY(cudaMemsetAsync(w->d_kept.p + n, 0, 8, st));
+    size_t tmp_bytes = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, w->d_kept.p, w->d_offsets.p, (int) (n + 1), st);
+    BFQ_CUDA_TRY(w->d_scan_tmp.reserve(tmp_bytes));
+    cub::DeviceScan::ExclusiveSum(w->d_scan_tmp.p, tmp_bytes, w->d_kept.p, w->d_offsets.p, (int) (n + 1), st);
+    h->launches += 2;
+    // only the grand total is needed on the host before the expansion (to size the id buffer)
+    BFQ_CUDA_TRY(cudaMemcpyAsync(hc + RC_COUNT, w->d_offsets.p + n, 8, cudaMemcpyDeviceToHost, st));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
+    out->n_ids = hc[RC_COUNT];
+    BFQ_CUDA_TRY(w->d_ids.reserve((size_t) std::max<unsigned long long>(out->n_ids, 1)));
+    rexpand_kernel<<<(unsigned) ((n * 32 + 255) / 256), 256, 0, st>>>(n, w->d_span_begin.p, w->d_span_count.p, w->d_ranges.p,
+                                                                      w->d_offsets.p, w->d_kept.p, h->d_dfs_to_id.p,
+                                                                      h->d_bfs_to_id.p, w->d_ids.p);
+    h->launches++;
+    BFQ_CUDA_TRY(cudaGetLastError());
+    BFQ_CUDA_TRY(cudaEventRecord(w->ev[1], st));
+    return BFQ_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -951,6 +1348,7 @@ int32_t bfq_rindex_create(int32_t device_ordinal, bfq_rindex** out) {
     BFQ_CUDA_TRY(cudaSetDevice(device_ordinal));
     auto* h = new bfq_rindex();
     h->device = device_ordinal;
+    h->pool->device = device_ordinal;
     if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) {
         delete h;
         return fail(BFQ_E_CUDA, "cudaStreamCreate failed");
@@ -962,7 +1360,7 @@ void bfq_rindex_destroy(bfq_rindex* h) { delete h; }
 
 int32_t bfq_rindex_reset(bfq_rindex* h) {
     if (!h) return fail(BFQ_E_INVALID, "handle is NULL");
-    std::lock_guard<std::mutex> g(h->mu);
+    WriteLock g(h);
     h->staged.clear();
     h->by_id = std::make_shared<IdTable>();   // the committed table stays with the snapshot and its results
     h->alive.clear();
@@ -974,7 +1372,7 @@ int32_t bfq_rindex_reset(bfq_rindex* h) {
 int32_t bfq_rindex_add(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_off, int32_t n_tenants,
                        const uint8_t* topics, const int64_t* topic_off, const int32_t* topic_tenant, int64_t n, int64_t* ids_out) {
     if (!h || n < 0 || n_tenants < 0) return fail(BFQ_E_INVALID, "bad argument");
-    std::lock_guard<std::mutex> g(h->mu);
+    WriteLock g(h);
     std::vector<std::string> ts((size_t) n_tenants);
     for (int32_t t = 0; t < n_tenants; t++) ts[(size_t) t].assign((const char*) tenants + tenant_off[t], (size_t) (tenant_off[t + 1] - tenant_off[t]));
     for (int64_t i = 0; i < n; i++) {
@@ -984,8 +1382,8 @@ int32_t bfq_rindex_add(bfq_rindex* h, const uint8_t* tenants, const int64_t* ten
         auto it = h->staged.find(key);
         int64_t id;
         if (it == h->staged.end()) {
-            id = (int64_t) h->by_id->size();
-            h->by_id->push_back(key);
+            id = (int64_t) h->by_id->e.size();
+            h->by_id->e.push_back(key);
             h->alive.push_back(1);
             h->dirty.insert(key.first);
             h->staged.emplace(std::move(key), id);
@@ -1003,7 +1401,7 @@ int32_t bfq_rindex_add(bfq_rindex* h, const uint8_t* tenants, const int64_t* ten
 // and skips an unparsable entry).
 int32_t bfq_rindex_load_keys(bfq_rindex* h, const uint8_t* keys, const int64_t* key_off, int64_t n, int64_t* ids_out) {
     if (!h || n < 0 || (n > 0 && (!keys || !key_off))) return fail(BFQ_E_INVALID, "bad argument");
-    std::lock_guard<std::mutex> g(h->mu);
+    WriteLock g(h);
     if (h->staged.empty()) h->need_full = true;   // a bulk load onto an empty handle: one full build beats a delta per tenant
     for (int64_t i = 0; i < n; i++) {
         sv tenant;
@@ -1016,8 +1414,8 @@ int32_t bfq_rindex_load_keys(bfq_rindex* h, const uint8_t* keys, const int64_t* 
         auto it = h->staged.find(key);
         int64_t id;
         if (it == h->staged.end()) {
-            id = (int64_t) h->by_id->size();
-            h->by_id->push_back(key);
+            id = (int64_t) h->by_id->e.size();
+            h->by_id->e.push_back(key);
             h->alive.push_back(1);
             h->dirty.insert(key.first);
             h->staged.emplace(std::move(key), id);
@@ -1032,13 +1430,13 @@ int32_t bfq_rindex_load_keys(bfq_rindex* h, const uint8_t* keys, const int64_t* 
 // retainMessageKey(tenant, topic) of every id in a match result, in result order: the keys of the follow-up reader.get calls of
 // RetainStoreCoProc.match (RS/RetainStoreCoProc.java:177-188), as one batch. Returns the blob length; copies if it fits.
 // The ids are resolved in the id table of the snapshot the match ran on, so a reset + reload between the match and this call
-// does not change the answer. h->mu is still taken: add / load_keys append to that same table until the next reset.
+// does not change the answer. h->mu is taken shared: add / load_keys append to that same table until the next reset.
 int64_t bfq_rresult_retain_keys(bfq_rindex* h, const bfq_rresult* r, uint8_t* blob_out, int64_t blob_cap, int64_t* key_off_out) {
     if (!h || !r) return BFQ_E_INVALID;
-    std::lock_guard<std::mutex> g(h->mu);
+    std::shared_lock<std::shared_mutex> g(h->mu);
     int64_t at = 0;
     const int64_t n = (int64_t) r->ids.size();
-    const IdTable& by_id = *r->by_id;   // set by bfq_rmatch, which runs only after a commit
+    const auto& by_id = r->by_id->e;   // set by bfq_rmatch, which runs only after a commit
     for (int64_t i = 0; i < n; i++) {
         const int64_t id = r->ids[(size_t) i];
         if (id < 0 || id >= (int64_t) by_id.size()) return BFQ_E_RANGE;
@@ -1053,7 +1451,7 @@ int64_t bfq_rresult_retain_keys(bfq_rindex* h, const bfq_rresult* r, uint8_t* bl
 
 int32_t bfq_rindex_remove(bfq_rindex* h, const uint8_t* tenant, int64_t tn, const uint8_t* topic, int64_t n) {
     if (!h) return fail(BFQ_E_INVALID, "handle is NULL");
-    std::lock_guard<std::mutex> g(h->mu);
+    WriteLock g(h);
     auto it = h->staged.find({std::string((const char*) tenant, (size_t) tn), std::string((const char*) topic, (size_t) n)});
     if (it != h->staged.end()) {
         h->alive[(size_t) it->second] = 0;
@@ -1065,29 +1463,39 @@ int32_t bfq_rindex_remove(bfq_rindex* h, const uint8_t* tenant, int64_t tn, cons
 
 int32_t bfq_rindex_commit(bfq_rindex* h) {
     if (!h) return fail(BFQ_E_INVALID, "handle is NULL");
-    std::lock_guard<std::mutex> g(h->mu);
+    WriteLock g(h);
     int32_t rc = commit_delta(h);
     if (rc == NEED_FULL) rc = rebuild_full(h);
-    if (rc == BFQ_OK) h->committed = h->by_id;
+    if (rc == BFQ_OK) {
+        h->committed = h->by_id;
+        h->generation++;
+    }
     return rc;
 }
 
 int32_t bfq_rindex_stats(bfq_rindex* h, int64_t* stats, int32_t n) {
     if (!h || (!stats && n > 0)) return fail(BFQ_E_INVALID, "bad argument");
-    std::lock_guard<std::mutex> g(h->mu);
-    const int64_t v[11] = {h->n_topics, (int64_t) h->regions.size(), h->n_nodes, h->garbage_nodes, h->used_slots,
+    std::shared_lock<std::shared_mutex> g(h->mu);
+    int64_t n_ws = 0, ws_bytes = 0;
+    {
+        std::lock_guard<std::mutex> p(h->pool->mu);
+        n_ws = (int64_t) h->pool->held.size();
+        for (const RWorkspace* w : h->pool->held) ws_bytes += w->bytes_held;
+    }
+    const int64_t key_bytes = h->by_id->key_device_bytes;
+    const int64_t v[14] = {h->n_topics, (int64_t) h->regions.size(), h->n_nodes, h->garbage_nodes, h->used_slots,
                            (int64_t) h->n_blocks * BLOCK_USABLE, h->full_commits, h->delta_commits, h->last_rebuilt,
-                           h->device_bytes(), h->overflowed_blocks};
-    for (int32_t i = 0; i < n && i < 11; i++) stats[i] = v[i];
+                           h->snapshot_bytes() + ws_bytes + key_bytes, h->overflowed_blocks, n_ws, ws_bytes, key_bytes};
+    for (int32_t i = 0; i < n && i < 14; i++) stats[i] = v[i];
     return BFQ_OK;
 }
 
 int32_t bfq_rindex_lookup(bfq_rindex* h, int64_t id, uint8_t* tenant_out, int64_t tenant_cap, int64_t* tenant_len,
                           uint8_t* topic_out, int64_t topic_cap, int64_t* topic_len) {
     if (!h) return fail(BFQ_E_INVALID, "handle is NULL");
-    std::lock_guard<std::mutex> g(h->mu);
-    if (id < 0 || id >= (int64_t) h->by_id->size()) return fail(BFQ_E_RANGE, "id out of range");
-    const auto& e = (*h->by_id)[(size_t) id];
+    std::shared_lock<std::shared_mutex> g(h->mu);
+    if (id < 0 || id >= (int64_t) h->by_id->e.size()) return fail(BFQ_E_RANGE, "id out of range");
+    const auto& e = h->by_id->e[(size_t) id];
     if (tenant_len) *tenant_len = (int64_t) e.first.size();
     if (topic_len) *topic_len = (int64_t) e.second.size();
     if (tenant_out && (int64_t) e.first.size() <= tenant_cap) memcpy(tenant_out, e.first.data(), e.first.size());
@@ -1099,171 +1507,56 @@ int32_t bfq_rmatch(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_
                    const uint8_t* filters, const int64_t* filter_off, const int32_t* filter_tenant, int64_t n,
                    const int64_t* limit, bfq_rresult** out) {
     if (!h || !out || n < 0 || n_tenants < 0) return fail(BFQ_E_INVALID, "bad argument");
-    std::lock_guard<std::mutex> g(h->mu);
+    BFQ_CUDA_TRY(cudaSetDevice(h->device));
+    auto g = read_lock(h);   // declared first: released after the lease below has drained its stream
+    CallLease lease{h->pool};
+    int32_t rc = acquire(h, &lease.w);
+    if (rc != BFQ_OK) return rc;
+    RWorkspace* w = lease.w;
     if (!h->have_snapshot) return fail(BFQ_E_STATE, "bfq_rmatch before the first bfq_rindex_commit");
     for (int64_t i = 0; i < n; i++)
         if (filter_tenant[i] < 0 || filter_tenant[i] >= n_tenants) return fail(BFQ_E_RANGE, "filter_tenant out of range");
-    BFQ_CUDA_TRY(cudaSetDevice(h->device));
-    cudaStream_t st = h->stream;
+    cudaStream_t st = w->stream;
     auto t0 = std::chrono::steady_clock::now();
-    const size_t nn = (size_t) std::max<int64_t>(n, 1), nt = (size_t) std::max(n_tenants, 1);
-    std::vector<int32_t> troot(nt, -1);
-    for (int32_t t = 0; t < n_tenants; t++) {
-        auto it = h->tenant_root.find(std::string((const char*) tenants + tenant_off[t], (size_t) (tenant_off[t + 1] - tenant_off[t])));
-        if (it != h->tenant_root.end()) troot[(size_t) t] = it->second;
-    }
-    const int64_t fbytes = n ? filter_off[n] : 0;
-    BFQ_CUDA_TRY(h->d_filters.reserve((size_t) std::max<int64_t>(fbytes, 1)));
-    BFQ_CUDA_TRY(h->d_filter_off.reserve(nn + 1));
-    BFQ_CUDA_TRY(h->d_filter_tenant.reserve(nn));
-    BFQ_CUDA_TRY(h->d_tenant_root.reserve(nt));
-    BFQ_CUDA_TRY(h->d_limit.reserve(nn));
-    BFQ_CUDA_TRY(h->d_span_begin.reserve(nn));
-    BFQ_CUDA_TRY(h->d_span_count.reserve(nn));
-    BFQ_CUDA_TRY(h->d_overflow.reserve(nn));
-    BFQ_CUDA_TRY(h->d_total.reserve(nn));
-    BFQ_CUDA_TRY(h->d_kept.reserve(nn));
-    BFQ_CUDA_TRY(h->d_offsets.reserve(nn + 1));
-    BFQ_CUDA_TRY(h->d_counters.reserve(RC_COUNT));
-    if (h->d_ranges.cap == 0) BFQ_CUDA_TRY(h->d_ranges.reserve(std::max<size_t>(1 << 18, 8 * nn)));
-    auto* res = new bfq_rresult();
+    std::unique_ptr<bfq_rresult> res(new bfq_rresult());
     res->by_id = h->committed;
+    res->generation = h->generation;
     res->offsets.assign((size_t) n + 1, 0);
     res->totals.assign((size_t) n, 0);
     if (n == 0) {
-        *out = res;
+        *out = res.release();
         return BFQ_OK;
     }
-    BFQ_CUDA_TRY(cudaMemcpyAsync(h->d_filters.p, filters, (size_t) fbytes, cudaMemcpyHostToDevice, st));
-    BFQ_CUDA_TRY(cudaMemcpyAsync(h->d_filter_off.p, filter_off, (size_t) (n + 1) * 8, cudaMemcpyHostToDevice, st));
-    BFQ_CUDA_TRY(cudaMemcpyAsync(h->d_filter_tenant.p, filter_tenant, (size_t) n * 4, cudaMemcpyHostToDevice, st));
-    BFQ_CUDA_TRY(cudaMemcpyAsync(h->d_tenant_root.p, troot.data(), nt * 4, cudaMemcpyHostToDevice, st));
-    if (limit) BFQ_CUDA_TRY(cudaMemcpyAsync(h->d_limit.p, limit, (size_t) n * 8, cudaMemcpyHostToDevice, st));
+    // the batch into one device block of the workspace, straight from the caller's memory: the driver overlaps its own staging
+    // of pageable memory with the transfer, where a copy into pinned memory first would add a host pass over the whole batch
+    const int64_t fbytes = filter_off[n];
+    uint8_t* d_filters = nullptr;
+    int64_t *d_filter_off = nullptr, *d_limit = nullptr;
+    int32_t* d_filter_tenant = nullptr;
+    rc = carve(w->d_in, "bfq_rmatch inputs", [&](Carve& c) {
+        d_filters = c.take<uint8_t>((size_t) fbytes);
+        d_filter_off = c.take<int64_t>((size_t) n + 1);
+        d_filter_tenant = c.take<int32_t>((size_t) n);
+        d_limit = limit ? c.take<int64_t>((size_t) n) : nullptr;
+    });
+    if (rc != BFQ_OK) return rc;
+    BFQ_CUDA_TRY(cudaMemcpyAsync(d_filters, filters, (size_t) fbytes, cudaMemcpyHostToDevice, st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(d_filter_off, filter_off, (size_t) (n + 1) * 8, cudaMemcpyHostToDevice, st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(d_filter_tenant, filter_tenant, (size_t) n * 4, cudaMemcpyHostToDevice, st));
+    if (limit) BFQ_CUDA_TRY(cudaMemcpyAsync(d_limit, limit, (size_t) n * 8, cudaMemcpyHostToDevice, st));
     auto t1 = std::chrono::steady_clock::now();
-    for (auto& e : h->ev)
-        if (!e) BFQ_CUDA_TRY(cudaEventCreate(&e));
-    BFQ_CUDA_TRY(cudaEventRecord(h->ev[0], st));   // the inputs are (enqueued to be) resident: device time of the kernels from here
-
-    RMatchParams p{};
-    p.nodes = h->d_nodes.p;
-    p.slots = h->d_slots.p;
-    p.tags = reinterpret_cast<const uint4*>(h->d_tags.p);
-    p.n_blocks = h->n_blocks;
-    p.filters = h->d_filters.p;
-    p.filter_off = h->d_filter_off.p;
-    p.filter_tenant = h->d_filter_tenant.p;
-    p.tenant_root = h->d_tenant_root.p;
-    p.n_filters = n;
-    p.span_begin = h->d_span_begin.p;
-    p.span_count = h->d_span_count.p;
-    p.total = h->d_total.p;
-    p.overflow_list = h->d_overflow.p;
-    p.counters = h->d_counters.p;
-    unsigned long long hc[RC_COUNT];
-    const int sms = device_sm_count();
-    int ctas_per_sm = 4;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, rmatch_kernel<false>, R_WARPS * 32, 0);
-    ctas_per_sm = std::max(1, ctas_per_sm);
-    // filters that share a tenant and leading levels walk the same part of the topic trie: group them so that the warps
-    // running at the same time hit the same node records in L2 (the forward path's locality order, reused)
-    const uint32_t* order = nullptr;
-    if (n >= 4096) {
-        BFQ_CUDA_TRY(h->d_ord_keys.reserve(nn));
-        BFQ_CUDA_TRY(h->d_ord_leader.reserve(nn));
-        BFQ_CUDA_TRY(h->d_order.reserve(nn));
-        BFQ_CUDA_TRY(h->d_hist.reserve(order_scratch_words(n, n_tenants)));
-        BFQ_CUDA_TRY(h->d_ord_ctr.reserve(CTR_COUNT));
-        OrderParams q{};
-        q.n_topics = n;
-        q.topics = h->d_filters.p;
-        q.topic_off = h->d_filter_off.p;
-        q.topic_tenant = h->d_filter_tenant.p;
-        q.n_tenants = n_tenants;
-        q.keys = h->d_ord_keys.p;
-        q.leader = h->d_ord_leader.p;
-        q.order = h->d_order.p;
-        q.hash_tab = nullptr;
-        q.hash_mask = 0;
-        q.hist = h->d_hist.p;
-        q.dedup = 0;
-        q.counters = h->d_ord_ctr.p;
-        BFQ_CUDA_TRY(launch_order(q, st));
-        h->launches += 3;
-        order = q.order;
-    }
-    for (int attempt = 0; attempt < 8; attempt++) {
-        p.ranges = h->d_ranges.p;
-        p.ranges_cap = h->d_ranges.cap;
-        p.work_list = order;
-        p.n_work = 0;
-        BFQ_CUDA_TRY(cudaMemsetAsync(h->d_counters.p, 0, sizeof(hc), st));
-        int64_t ctas = std::min<int64_t>((n + R_WARPS - 1) / R_WARPS, (int64_t) sms * ctas_per_sm);
-        BFQ_CUDA_TRY(cudaEventRecord(h->ev[2], st));
-        rmatch_kernel<false><<<(unsigned) std::max<int64_t>(ctas, 1), R_WARPS * 32, 0, st>>>(p);
-        BFQ_CUDA_TRY(cudaEventRecord(h->ev[3], st));
-        h->launches++;
-        BFQ_CUDA_TRY(cudaGetLastError());
-        BFQ_CUDA_TRY(cudaMemcpyAsync(hc, h->d_counters.p, sizeof(hc), cudaMemcpyDeviceToHost, st));
-        BFQ_CUDA_TRY(cudaStreamSynchronize(st));
-        if (hc[RC_OVERFLOW] > 0) {
-            const uint64_t capF = (uint64_t) h->max_nodes_per_depth + 2;
-            const uint64_t capR = 3 * ((uint64_t) h->n_nodes + 2) + 2;
-            const uint64_t per_warp = 2 * capF + capR;
-            uint64_t warps = std::min<uint64_t>(hc[RC_OVERFLOW], std::max<uint64_t>(8, (1ull << 31) / (per_warp * sizeof(uint2))));
-            warps = std::min<uint64_t>((warps + 7) / 8 * 8, (uint64_t) sms * 8);
-            BFQ_CUDA_TRY(h->d_scratch.reserve((size_t) (warps * per_warp)));
-            p.scratch = h->d_scratch.p;
-            p.scratch_frontier_cap = capF;
-            p.scratch_ranges_cap = capR;
-            p.work_list = h->d_overflow.p;
-            p.n_work = (int64_t) hc[RC_OVERFLOW];
-            rmatch_kernel<true><<<(unsigned) (warps / 8), R_WARPS * 32, 0, st>>>(p);
-            h->launches++;
-            BFQ_CUDA_TRY(cudaGetLastError());
-            BFQ_CUDA_TRY(cudaMemcpyAsync(hc, h->d_counters.p, sizeof(hc), cudaMemcpyDeviceToHost, st));
-            BFQ_CUDA_TRY(cudaStreamSynchronize(st));
-            if (hc[RC_ERROR] != 0) {
-                delete res;
-                return fail(BFQ_E_STATE, "tier-2 scratch exhausted");
-            }
-        }
-        if (hc[RC_RANGES] <= h->d_ranges.cap) break;
-        const size_t want = (size_t) (hc[RC_RANGES] + hc[RC_RANGES] / 4 + 1024);
-        if (want >= 0xFFFFFFF0ull || attempt == 7) {
-            delete res;
-            return fail(BFQ_E_RANGE, "too many matched ranges in one batch; split the batch");
-        }
-        BFQ_CUDA_TRY(h->d_ranges.reserve(want));
-    }
-    // kept = min(total, limit); exclusive scan; expand to ids
-    rkept_kernel<<<(unsigned) ((n + 255) / 256), 256, 0, st>>>(n, h->d_total.p, limit ? h->d_limit.p : nullptr, h->d_kept.p);
-    size_t tmp_bytes = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, h->d_kept.p, h->d_offsets.p, (int) n, st);
-    BFQ_CUDA_TRY(h->d_scan_tmp.reserve(tmp_bytes));
-    cub::DeviceScan::ExclusiveSum(h->d_scan_tmp.p, tmp_bytes, h->d_kept.p, h->d_offsets.p, (int) n, st);
-    h->launches += 2;
-    // only the grand total is needed on the host before the expansion (to size the id buffer): two scalars, not the arrays
-    BFQ_CUDA_TRY(h->h_small.reserve(4));
-    BFQ_CUDA_TRY(cudaMemcpyAsync(h->h_small.p, h->d_offsets.p + (n - 1), 8, cudaMemcpyDeviceToHost, st));
-    BFQ_CUDA_TRY(cudaMemcpyAsync(h->h_small.p + 1, h->d_kept.p + (n - 1), 8, cudaMemcpyDeviceToHost, st));
-    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
-    const unsigned long long total_ids = h->h_small.p[0] + h->h_small.p[1];
-    BFQ_CUDA_TRY(h->d_ids.reserve((size_t) std::max<unsigned long long>(total_ids, 1)));
-    rexpand_kernel<<<(unsigned) ((n * 32 + 255) / 256), 256, 0, st>>>(n, h->d_span_begin.p, h->d_span_count.p, h->d_ranges.p,
-                                                                      h->d_offsets.p, h->d_kept.p, h->d_dfs_to_id.p,
-                                                                      h->d_bfs_to_id.p, h->d_ids.p);
-    h->launches++;
-    BFQ_CUDA_TRY(cudaGetLastError());
-    BFQ_CUDA_TRY(cudaEventRecord(h->ev[1], st));
+    RCoreOut co;
+    rc = rmatch_core(h, w, RCoreIn{tenants, tenant_off, n_tenants, d_filters, d_filter_off, d_filter_tenant, n, d_limit, false}, &co);
+    if (rc != BFQ_OK) return rc;
     auto t2 = std::chrono::steady_clock::now();
     // the result owns its arrays: offsets / totals / ids are read back straight into them (same 8-byte element types)
     static_assert(sizeof(unsigned long long) == sizeof(int64_t), "offsets are copied without conversion");
-    res->ids.resize((size_t) total_ids);
-    BFQ_CUDA_TRY(cudaMemcpyAsync(res->offsets.data(), h->d_offsets.p, (size_t) n * 8, cudaMemcpyDeviceToHost, st));
-    BFQ_CUDA_TRY(cudaMemcpyAsync(res->totals.data(), h->d_total.p, (size_t) n * 8, cudaMemcpyDeviceToHost, st));
-    if (total_ids) BFQ_CUDA_TRY(cudaMemcpyAsync(res->ids.data(), h->d_ids.p, (size_t) total_ids * 8, cudaMemcpyDeviceToHost, st));
+    res->ids.resize((size_t) co.n_ids);
+    BFQ_CUDA_TRY(cudaMemcpyAsync(res->offsets.data(), w->d_offsets.p, (size_t) (n + 1) * 8, cudaMemcpyDeviceToHost, st));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(res->totals.data(), w->d_total.p, (size_t) n * 8, cudaMemcpyDeviceToHost, st));
+    if (co.n_ids) BFQ_CUDA_TRY(cudaMemcpyAsync(res->ids.data(), w->d_ids.p, (size_t) co.n_ids * 8, cudaMemcpyDeviceToHost, st));
     BFQ_CUDA_TRY(cudaStreamSynchronize(st));
-    res->offsets[(size_t) n] = (int64_t) total_ids;
+    g.unlock();
     auto t3 = std::chrono::steady_clock::now();
     auto ms = [](auto a, auto b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
     res->ms[0] = ms(t0, t1);
@@ -1272,14 +1565,14 @@ int32_t bfq_rmatch(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_
     res->ms[3] = ms(t0, t3);
     {
         float a = 0, b = 0;
-        cudaEventElapsedTime(&a, h->ev[0], h->ev[1]);
-        cudaEventElapsedTime(&b, h->ev[2], h->ev[3]);
+        cudaEventElapsedTime(&a, w->ev[0], w->ev[1]);
+        cudaEventElapsedTime(&b, w->ev[2], w->ev[3]);
         res->ms[4] = a;                       // device time from "inputs resident" to "ids expanded" (all kernels + the host's counter reads between them)
         res->ms[5] = b;                       // device time of rmatch_kernel (the last attempt)
-        res->ms[6] = (double) hc[RC_RANGES];  // rank ranges emitted (8 bytes each): the kernel's output size
-        res->ms[7] = (double) hc[RC_OVERFLOW];
+        res->ms[6] = (double) co.n_ranges;    // rank ranges emitted (8 bytes each): the kernel's output size
+        res->ms[7] = (double) co.n_overflow;
     }
-    *out = res;
+    *out = res.release();
     return BFQ_OK;
 }
 
@@ -1290,11 +1583,125 @@ const int64_t* bfq_rresult_ids(const bfq_rresult* r, int64_t* n) {
     return r->ids.data();
 }
 const int64_t* bfq_rresult_total_matches(const bfq_rresult* r) { return r->totals.data(); }
+uint64_t bfq_rresult_generation(const bfq_rresult* r) { return r ? r->generation : 0; }
 int32_t bfq_rresult_timings(const bfq_rresult* r, double* ms, int32_t n) {
     if (!r || !ms) return fail(BFQ_E_INVALID, "bad argument");
     for (int32_t i = 0; i < n && i < 8; i++) ms[i] = r->ms[i];
     return BFQ_OK;
 }
 void bfq_rresult_free(bfq_rresult* r) { delete r; }
+
+int32_t bfq_rmatch_device(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_off, int32_t n_tenants,
+                          const uint8_t* d_filters, const int64_t* d_filter_off, const int32_t* d_filter_tenant, int64_t n,
+                          const int64_t* d_limit, void* stream, bfq_rdevice_result* out) {
+    if (!h || !out || n < 0 || n_tenants < 0) return fail(BFQ_E_INVALID, "bad argument");
+    if (n_tenants > 0 && (!tenants || !tenant_off)) return fail(BFQ_E_INVALID, "NULL tenant list");
+    if (n > 0 && (!d_filters || !d_filter_off || !d_filter_tenant)) return fail(BFQ_E_INVALID, "NULL filter arrays");
+    memset(out, 0, sizeof(*out));
+    BFQ_CUDA_TRY(cudaSetDevice(h->device));
+    auto g = read_lock(h);   // declared first: released after the lease below has drained its stream
+    CallLease lease{h->pool};
+    int32_t rc = acquire(h, &lease.w);
+    if (rc != BFQ_OK) return rc;
+    RWorkspace* w = lease.w;
+    if (!h->have_snapshot) return fail(BFQ_E_STATE, "bfq_rmatch_device before the first bfq_rindex_commit");
+    // the batch was written on the caller's stream: the match runs on the workspace's own stream, after it
+    BFQ_CUDA_TRY(cudaEventRecord(w->ev_in, (cudaStream_t) stream));
+    BFQ_CUDA_TRY(cudaStreamWaitEvent(w->stream, w->ev_in, 0));
+    RCoreOut co;
+    rc = rmatch_core(h, w, RCoreIn{tenants, tenant_off, n_tenants, d_filters, d_filter_off, d_filter_tenant, n, d_limit, true}, &co);
+    if (rc != BFQ_OK) return rc;
+    BFQ_CUDA_TRY(cudaStreamSynchronize(w->stream));
+    auto* L = new RLease();
+    L->h = h;
+    L->pool = h->pool;
+    L->by_id = h->committed;
+    out->generation = h->generation;
+    g.unlock();
+    out->d_offsets = reinterpret_cast<const int64_t*>(w->d_offsets.p);
+    out->d_ids = w->d_ids.p;
+    out->d_total = reinterpret_cast<const int64_t*>(w->d_total.p);
+    out->n_filters = n;
+    out->n_ids = (int64_t) co.n_ids;
+    out->n_ranges = (int64_t) co.n_ranges;
+    out->n_overflow_filters = (int64_t) co.n_overflow;
+    if (n > 0) {
+        float a = 0, b = 0;
+        cudaEventElapsedTime(&a, w->ev[0], w->ev[1]);
+        cudaEventElapsedTime(&b, w->ev[2], w->ev[3]);
+        out->device_ms = a;
+        out->kernel_ms = b;
+    }
+    L->ws = w;
+    lease.w = nullptr;   // the result keeps the workspace until bfq_rdevice_result_release
+    out->lease = L;
+    return BFQ_OK;
+}
+
+void bfq_rdevice_result_release(bfq_rdevice_result* res) {
+    if (!res || !res->lease) return;
+    auto* L = static_cast<RLease*>(res->lease);
+    cudaSetDevice(L->pool->device);
+    // never hand a busy workspace back: every key gather on the result, on each stream it ran on
+    for (size_t i = 0; i < L->used_on.size(); i++) cudaEventSynchronize(L->ws->ev_use[i]);
+    give_back(L->pool, L->ws);
+    delete L;
+    res->lease = nullptr;
+}
+
+int32_t bfq_rretain_keys_device(bfq_rindex* h, const bfq_rdevice_result* res, int64_t* d_key_off, uint8_t* d_keys, int64_t cap,
+                                void* stream, int64_t* n_bytes) {
+    if (!h || !res || !d_key_off || !n_bytes) return fail(BFQ_E_INVALID, "bad argument");
+    if (!res->lease) return fail(BFQ_E_INVALID, "no match behind this result");
+    auto* L = static_cast<RLease*>(res->lease);
+    if (L->h != h) return fail(BFQ_E_INVALID, "the result belongs to another handle");
+    const int64_t n = res->n_ids;
+    if (n >= (int64_t) INT32_MAX) return fail(BFQ_E_RANGE, "too many ids in one result");
+    BFQ_CUDA_TRY(cudaSetDevice(h->device));
+    std::lock_guard<std::mutex> u(L->use_mu);
+    RWorkspace* w = L->ws;
+    std::shared_ptr<KeyBufs> kb;
+    {
+        auto g = read_lock(h);   // the id table is read while its key table is extended
+        const int32_t rc = extend_keys(*L->by_id, h->device, w->stream, &kb);
+        if (rc != BFQ_OK) return rc;
+    }
+    if (std::find(L->keys.begin(), L->keys.end(), kb) == L->keys.end()) L->keys.push_back(kb);
+    cudaStream_t st = (cudaStream_t) stream;
+    size_t k = 0;
+    while (k < L->used_on.size() && L->used_on[k] != st) k++;
+    if (k == L->used_on.size()) {
+        if (k == w->ev_use.size()) {
+            cudaEvent_t e = nullptr;
+            BFQ_CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+            w->ev_use.push_back(e);
+        }
+        L->used_on.push_back(st);
+    }
+    RecordOnExit rec(w->ev_use[k], st);
+    // sizing pass, scan, then the bytes if they fit
+    BFQ_CUDA_TRY(cudaMemsetAsync(d_key_off, 0, 8, st));
+    if (n > 0) {
+        BFQ_CUDA_TRY(w->d_key_len.reserve((size_t) n));
+        rkey_len_kernel<<<(unsigned) ((n + 255) / 256), 256, 0, st>>>(n, w->d_ids.p, kb->off.p, w->d_key_len.p);
+        BFQ_CUDA_TRY(cudaGetLastError());
+        size_t tmp_bytes = 0;
+        cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, w->d_key_len.p, d_key_off + 1, (int) n, st);
+        BFQ_CUDA_TRY(w->d_key_tmp.reserve(tmp_bytes));
+        BFQ_CUDA_TRY(cub::DeviceScan::InclusiveSum(w->d_key_tmp.p, tmp_bytes, w->d_key_len.p, d_key_off + 1, (int) n, st));
+        h->launches += 2;
+    }
+    BFQ_CUDA_TRY(w->h_small.reserve(RC_COUNT + 1));
+    BFQ_CUDA_TRY(cudaMemcpyAsync(w->h_small.p + RC_COUNT, d_key_off + n, 8, cudaMemcpyDeviceToHost, st));
+    BFQ_CUDA_TRY(cudaStreamSynchronize(st));
+    const int64_t total = (int64_t) w->h_small.p[RC_COUNT];
+    *n_bytes = total;
+    if (d_keys && n > 0 && total <= cap) {
+        rkey_copy_kernel<<<(unsigned) ((n * 32 + 255) / 256), 256, 0, st>>>(n, w->d_ids.p, kb->off.p, kb->bytes.p, d_key_off, d_keys);
+        h->launches++;
+        BFQ_CUDA_TRY(cudaGetLastError());
+    }
+    return BFQ_OK;
+}
 
 }  // extern "C"

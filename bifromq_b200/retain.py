@@ -33,6 +33,7 @@ class RMatchResult:
         lib.bfq_rresult_timings(handle, ms.ctypes.data, 8)
         self.timings_ms = dict(zip(["h2d", "kernels", "d2h", "total", "device_all_kernels", "device_rmatch_kernel"], ms[:6].tolist()))
         self.n_ranges, self.n_overflow_filters = int(ms[6]), int(ms[7])
+        self.generation = int(lib.bfq_rresult_generation(handle))
         self.retain_keys = None
         if with_retain_keys and index_handle is not None:
             # the keys of RetainStoreCoProc.match's follow-up reader.get calls, as one batch (bfq_rresult_retain_keys)
@@ -48,6 +49,39 @@ class RMatchResult:
 
     def matches(self, i):
         return self.ids[self.offsets[i]:self.offsets[i + 1]]
+
+
+class RDeviceResult:
+    """One bfq_rmatch_device result: device pointers (d_offsets, d_ids, d_total) + counts; the arrays stay valid until
+    release()."""
+
+    def __init__(self, raw, owner):
+        self.raw = raw
+        self._owner = owner   # the index: keeps it alive for as long as this result is
+
+    def __getattr__(self, name):   # d_ids, n_ids, generation, kernel_ms, ... straight from the C struct
+        if name == "raw":
+            raise AttributeError(name)
+        return getattr(self.raw, name)
+
+    def retain_keys_device(self, d_key_off_ptr, d_keys_ptr, cap, stream=0):
+        """bfq_rretain_keys_device: the retainMessageKey of every id, in result order, gathered on the device. d_key_off_ptr:
+        int64 [n_ids + 1] (always written); the bytes go to d_keys_ptr only if they fit cap (None only sizes). -> total bytes"""
+        n = C.c_int64(0)
+        N.check(N.lib.bfq_rretain_keys_device(self._owner._h, C.byref(self.raw), d_key_off_ptr, d_keys_ptr, cap, stream, C.byref(n)))
+        return n.value
+
+    def release(self):
+        if getattr(self, "raw", None) is not None and self.raw.lease:
+            N.lib.bfq_rdevice_result_release(C.byref(self.raw))
+
+    close = release
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
 
 
 class GpuTopicMatchIndex:
@@ -90,7 +124,7 @@ class GpuTopicMatchIndex:
         N.check(N.lib.bfq_rindex_commit(self._h))
 
     STAT_NAMES = ["topics", "tenants", "nodes", "garbage_nodes", "used_slots", "usable_slots", "full_commits", "delta_commits",
-                  "rebuilt_tenants", "device_bytes", "overflowed_blocks"]
+                  "rebuilt_tenants", "device_bytes", "overflowed_blocks", "workspaces", "workspace_bytes", "key_table_bytes"]
 
     def stats(self):
         """bfq_rindex_stats of the committed snapshot, by name"""
@@ -122,6 +156,15 @@ class GpuTopicMatchIndex:
         N.check(N.lib.bfq_rmatch(self._h, N.ptr(tb), N.ptr(toff), len(tenants), N.ptr(filters_blob), N.ptr(filter_off), N.ptr(ft), n,
                                  N.ptr(lim) if lim is not None else None, C.byref(r)))
         return RMatchResult(r, self._h, with_retain_keys)
+
+    def match_device(self, tenants, d_filters_ptr, d_filter_off_ptr, d_filter_tenant_ptr, n, d_limit_ptr=None, stream=0):
+        """bfq_rmatch_device: n filters already in device memory (uint8 blob, int64 offsets [n + 1], int32 tenant index per
+        filter, optional int64 limit per filter; None = unlimited), written on `stream`. -> RDeviceResult, ready when returned"""
+        tb, toff = N.as_blob(tenants)
+        out = N.BfqRDeviceResult()
+        N.check(N.lib.bfq_rmatch_device(self._h, N.ptr(tb), N.ptr(toff), len(tenants), d_filters_ptr, d_filter_off_ptr,
+                                        d_filter_tenant_ptr, n, d_limit_ptr, stream, C.byref(out)))
+        return RDeviceResult(out, self)
 
     def match(self, tenant, filters, limit=None):
         blob, off = N.as_blob(filters)

@@ -640,7 +640,8 @@ int32_t bfq_rindex_add(bfq_rindex* h, const uint8_t* tenants, const int64_t* ten
  * alone. ids_out[i] = the topic's id, or -1 for bytes that are not a retain key (skipped). */
 int32_t bfq_rindex_load_keys(bfq_rindex* h, const uint8_t* keys, const int64_t* key_off, int64_t n, int64_t* ids_out);
 int32_t bfq_rindex_remove(bfq_rindex* h, const uint8_t* tenant, int64_t tn, const uint8_t* topic, int64_t n);
-/* Publishes the staged topics as the snapshot that bfq_rmatch reads. Each tenant's trie is one region of the device arrays.
+/* Publishes the staged topics as the snapshot that bfq_rmatch reads; the snapshot's generation is the number of successful
+ * commits on the handle so far (a commit with nothing changed counts too). Each tenant's trie is one region of the device arrays.
  * Delta path: a commit rebuilds only the tenants whose staged topic set changed since the last commit (an add of a new
  * (tenant, topic) or a remove of a staged one; re-adding an existing topic changes nothing). Each rebuilt tenant gets a
  * fresh region behind the existing ones, and its exact edges are inserted into the device hash table by a kernel. The
@@ -656,7 +657,10 @@ int32_t bfq_rindex_commit(bfq_rindex* h);
 /* stats[k], k < n, of the committed snapshot: 0 live topics, 1 live tenants, 2 node records (garbage included), 3 garbage
  * nodes, 4 occupied hash-table slots (garbage included), 5 usable hash-table slots, 6 full commits so far, 7 delta commits
  * so far (a commit with nothing changed counts as neither), 8 tenants whose region the last commit built (0 when nothing
- * changed), 9 device bytes held by the handle, 10 hash-table blocks that overflowed into the next block */
+ * changed), 9 device bytes held by the handle (snapshot, workspaces and key table: the sum of 12, 13 and the snapshot's),
+ * 10 hash-table blocks that overflowed into the next block, 11 match workspaces the handle holds (idle in its pool or leased
+ * to a call or a device result), 12 their device bytes (as each was when its last call ended), 13 device bytes of the
+ * retain-key table of the current id table (bfq_rretain_keys_device; 0 until the first key call, and again after a reset) */
 int32_t bfq_rindex_stats(bfq_rindex* h, int64_t* stats, int32_t n);
 /* topic id -> (tenant, topic) strings, resolved against the STAGED ids: after bfq_rindex_reset ids restart at 0, so an id of an
  * earlier result may name another topic here (bfq_rresult_retain_keys resolves against the result's own snapshot instead) */
@@ -668,7 +672,10 @@ int32_t bfq_rindex_lookup(bfq_rindex* h, int64_t id, uint8_t* tenant_out, int64_
  * loop (it keeps iterating until `limit` LIVE messages are found, RetainStoreCoProc.java:177-188), whereas this call
  * truncates to `limit` topic ids before the caller has looked at any message: a caller that drops expired messages must
  * ask for more than `limit` (total_matches tells how many exist) or pass limit < 0 and cut after its own expiry check.
- * Thread-safe: calls on one handle are serialised, every result owns its arrays. */
+ * Thread-safe: any number of threads may match on one handle at once. Every match leases its own workspace (stream, device
+ * scratch, pinned counters) from the handle's pool and holds the handle lock SHARED until its kernels have read the snapshot;
+ * add / load_keys / remove / reset / commit take it exclusive, so a commit waits for the matches in flight and a match waits
+ * for a running commit. A result owns its arrays; the workspace goes back to the pool when the call returns. */
 int32_t bfq_rmatch(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_off, int32_t n_tenants,
                    const uint8_t* filters, const int64_t* filter_off, const int32_t* filter_tenant, int64_t n_filters,
                    const int64_t* limit, bfq_rresult** out);
@@ -684,6 +691,7 @@ const int64_t* bfq_rresult_total_matches(const bfq_rresult* r);      /* [n_filte
  * "inputs resident" to "ids expanded" (CUDA events on the call's stream); ms[5]: device time of rmatch_kernel alone;
  * ms[6]: rank ranges the kernel emitted (8 bytes each); ms[7]: filters that needed the global-scratch tier */
 int32_t bfq_rresult_timings(const bfq_rresult* r, double* ms, int32_t n);
+uint64_t bfq_rresult_generation(const bfq_rresult* r);               /* the snapshot the match ran on (bfq_rindex_commit) */
 /* retainMessageKey of every id of the result, in result order, as one (blob, key_off[n_ids + 1]) batch: the keys of the
  * follow-up reader.get calls of RetainStoreCoProc.match (RS/RetainStoreCoProc.java:177-188). Returns the blob length (or a
  * negative BFQ_E_*); copies only if it fits blob_cap; key_off_out may be NULL. The ids are resolved against the id table of
@@ -691,6 +699,41 @@ int32_t bfq_rresult_timings(const bfq_rresult* r, double* ms, int32_t n);
  * and the next commit) still gets the keys of the topics the result matched. */
 int64_t bfq_rresult_retain_keys(bfq_rindex* h, const bfq_rresult* r, uint8_t* blob_out, int64_t blob_cap, int64_t* key_off_out);
 void bfq_rresult_free(bfq_rresult* r);
+
+/* bfq_rmatch with the batch already in device memory and the answer left there. d_filters / d_filter_off[n + 1] /
+ * d_filter_tenant[n] / d_limit[n] are device arrays written on `stream` (a cudaStream_t, NULL = default stream); d_limit NULL =
+ * unlimited. The match runs on the leased workspace's own stream, after the work already enqueued on `stream`, and the call
+ * returns once the ids are on the device: the arrays in *out are ready for any stream. The tenant list is host memory. A
+ * filter_tenant outside [0, n_tenants) is found on the device and fails the whole call with BFQ_E_RANGE, leaving *out
+ * empty. NULL arrays: BFQ_E_INVALID; before the first commit: BFQ_E_STATE; other errors as bfq_rmatch. Answers (offsets, ids
+ * in order, totals) are bfq_rmatch's: both run the same match.
+ * The arrays belong to a workspace leased to the result until bfq_rdevice_result_release, which first waits for everything
+ * the library enqueued for the result (bfq_rretain_keys_device, on every stream it ran on) and then returns the workspace to
+ * the handle's pool. The caller's own work that reads the arrays must be ordered before the release by the caller. */
+typedef struct {
+    const int64_t* d_offsets;       /* [n_filters + 1]: filter i's ids are d_ids[d_offsets[i] .. d_offsets[i + 1]) */
+    const int64_t* d_ids;           /* [n_ids] */
+    const int64_t* d_total;         /* [n_filters] matches before the limit */
+    int64_t n_filters, n_ids;
+    int64_t n_ranges;               /* rank ranges rmatch_kernel emitted (its last attempt) */
+    int64_t n_overflow_filters;     /* filters that needed the global-scratch tier */
+    uint64_t generation;            /* snapshot the match ran on */
+    double device_ms;               /* device time from "inputs resident" to "ids expanded" (CUDA events) */
+    double kernel_ms;               /* device time of rmatch_kernel (its last attempt) */
+    void* lease;                    /* opaque; owned by the library until bfq_rdevice_result_release */
+} bfq_rdevice_result;
+int32_t bfq_rmatch_device(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_off, int32_t n_tenants,
+                          const uint8_t* d_filters, const int64_t* d_filter_off, const int32_t* d_filter_tenant, int64_t n_filters,
+                          const int64_t* d_limit, void* stream, bfq_rdevice_result* out);
+void bfq_rdevice_result_release(bfq_rdevice_result* res);
+/* bfq_rresult_retain_keys for a device result, gathered on the device on `stream`: the retainMessageKey of every id, in result
+ * order. Sizing follows bfq_expand_device: d_key_off[n_ids + 1] (int64, device) is always written, the bytes go to d_keys only
+ * if *n_bytes <= cap (d_keys = NULL only sizes). Bytes are those of bfq_rresult_retain_keys on the same ids. The keys come
+ * from a device table of the id table the match resolved against: built on the first key call, extended for ids added since,
+ * dropped with the id table (a result taken before a reset and reload still gets its own snapshot's keys). The copy may
+ * still run on `stream` when the call returns; bfq_rdevice_result_release waits for it. Calls on one result are serialised. */
+int32_t bfq_rretain_keys_device(bfq_rindex* h, const bfq_rdevice_result* res, int64_t* d_key_off, uint8_t* d_keys, int64_t cap,
+                                void* stream, int64_t* n_bytes);
 
 #ifdef __cplusplus
 }
