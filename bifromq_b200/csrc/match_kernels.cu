@@ -718,24 +718,17 @@ struct OrderKernelParams {
 constexpr int ORDER_WINDOW_QUADS = 3;
 constexpr int ORDER_WINDOW_WORDS = 4 * ORDER_WINDOW_QUADS;   // the order key looks at the first 48 bytes: three levels of ordinary topics end well before
 
-// bytes [0, len) of the topic at offset ob equal the caller's topic, whose first ORDER_WINDOW_WORDS words are already in
-// registers (ka, masked to len) and whose tail is re-read.
-__device__ __forceinline__ bool same_topic(const uint8_t* topics, int64_t oa, const uint32_t (&ka)[ORDER_WINDOW_WORDS], int64_t ob, int len) {
-    TopicQuads wb(topics, ob, len);
-    uint32_t diff = 0;
-#pragma unroll
-    for (int j = 0; j < ORDER_WINDOW_QUADS; j++)
-        if (16 * j < len) {
-            uint32_t w[4];
-            wb.next(w);
-#pragma unroll
-            for (int i = 0; i < 4; i++) diff |= ka[4 * j + i] ^ w[i];
-        }
-    if (diff) return false;
-    if (len <= 4 * ORDER_WINDOW_WORDS) return true;
-    TopicQuads wa(topics, oa + 4 * ORDER_WINDOW_WORDS, len - 4 * ORDER_WINDOW_WORDS);
-    wb.len = len;
-    for (int j = ORDER_WINDOW_QUADS; 16 * j < len; j++) {
+// The (tenant, topic) pairs of topics a and b are equal: same tenant (every out-of-range index counts as one tenant), same
+// length, same bytes.
+__device__ __forceinline__ bool same_pair(const OrderKernelParams& q, uint32_t a, uint32_t b) {
+    int ta = q.topic_tenant[a], tb = q.topic_tenant[b];
+    if (ta < 0 || ta >= q.n_tenants) ta = -1;
+    if (tb < 0 || tb >= q.n_tenants) tb = -1;
+    const int64_t oa = q.topic_off[a], ob = q.topic_off[b];
+    const int64_t len = max((int64_t) 0, q.topic_off[a + 1] - oa);
+    if (ta != tb || max((int64_t) 0, q.topic_off[b + 1] - ob) != len || len > 0x3FFFFFFF) return false;
+    TopicQuads wa(q.topics, oa, (int) len), wb(q.topics, ob, (int) len);
+    for (int j = 0; 16 * j < len; j++) {
         uint32_t x[4], y[4];
         wa.next(x);
         wb.next(y);
@@ -744,78 +737,47 @@ __device__ __forceinline__ bool same_topic(const uint8_t* topics, int64_t oa, co
     return true;
 }
 
-// key = tenant index (T bits) | hash(level 0) | hash(levels 0..1) | hash(levels 0..2): equal leading levels => equal digits =>
-// one bucket. Hash collisions only merge groups. Topics with fewer levels use digit 0.
-__global__ void __launch_bounds__(256, 4) order_prep_kernel(const OrderKernelParams q, int tenant_bits, int key_bits) {
-    const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= q.n_topics) return;
+// One pass over topic i: its first ORDER_WINDOW_WORDS words go to k (the order key's window, zero past the end), and the
+// 64-bit de-dup hash of (tenant, length, bytes) is returned (two independent 32-bit multiply-xor lanes, one IMAD each per word,
+// folded by fmix64 and cut to q.dedup_hash_mask). Without de-dup only the window is read.
+__device__ __forceinline__ uint64_t read_topic(const OrderKernelParams& q, int64_t i, int& hlen, int& tn, uint32_t (&k)[ORDER_WINDOW_WORDS]) {
     const int64_t o = q.topic_off[i];
-    const int64_t full_len = max((int64_t) 0, q.topic_off[i + 1] - o);
-    const int hlen = (int) min(full_len, (int64_t) 0x3FFFFFFF);
-    int tn = q.topic_tenant[i];
+    hlen = (int) min(max((int64_t) 0, q.topic_off[i + 1] - o), (int64_t) 0x3FFFFFFF);
+    tn = q.topic_tenant[i];
     if (tn < 0 || tn >= q.n_tenants) tn = -1;   // all out-of-range tenant indices match nothing: one group
-    // ---- one pass over the topic: the first ORDER_WINDOW_WORDS words feed the order key, all of them the 64-bit hash
-    // (two independent 32-bit multiply-xor lanes, one IMAD each per word, folded into 64 bits at the end)
-    uint32_t k[ORDER_WINDOW_WORDS];
     uint32_t h1 = (uint32_t) hlen * 0x9E3779B1u + (uint32_t) tn, h2 = (uint32_t) tn * 0x85EBCA77u ^ (uint32_t) hlen;
-    {
-        TopicQuads tq(q.topics, o, hlen);
+    TopicQuads tq(q.topics, o, hlen);
 #pragma unroll
-        for (int j = 0; j < ORDER_WINDOW_QUADS; j++) {
-            uint32_t w[4] = {0u, 0u, 0u, 0u};
-            if (16 * j < hlen) tq.next(w);
+    for (int j = 0; j < ORDER_WINDOW_QUADS; j++) {
+        uint32_t w[4] = {0u, 0u, 0u, 0u};
+        if (16 * j < hlen) tq.next(w);
 #pragma unroll
-            for (int x = 0; x < 4; x++) {
-                k[4 * j + x] = w[x];
-                h1 = (h1 ^ w[x]) * 0xCC9E2D51u;
-                h2 = (h2 + w[x]) * 0x1B873593u ^ (h2 >> 15);
-            }
-        }
-        if (q.dedup)
-            for (int j = ORDER_WINDOW_QUADS; 16 * j < hlen; j++) {
-                uint32_t w[4];
-                tq.next(w);
-#pragma unroll
-                for (int x = 0; x < 4; x++) {
-                    h1 = (h1 ^ w[x]) * 0xCC9E2D51u;
-                    h2 = (h2 + w[x]) * 0x1B873593u ^ (h2 >> 15);
-                }
-            }
-    }
-    uint64_t h = ((uint64_t) h1 << 32) | h2;
-    // ---- de-duplication: first inserter leads
-    uint32_t lead = (uint32_t) i;
-    if (q.dedup) {
-        h = fmix64(h) & q.dedup_hash_mask;
-        const unsigned long long mine = ((unsigned long long) (uint32_t) (h >> 32) << 32) | (unsigned long long) (uint32_t) i;
-        uint32_t slot = (uint32_t) h & q.hash_mask;
-        while (true) {
-            // read through to L2: an L1-cached "empty" would send every later duplicate of a popular topic on this SM into the
-            // CAS below, and thousands of same-address atomics serialise (the prep kernel sat at ~90 us whatever its
-            // instruction count until this load bypassed L1)
-            unsigned long long cur = __ldcg(&q.hash_tab[slot]);
-            if (cur == ~0ull) {
-                cur = atomicCAS(&q.hash_tab[slot], ~0ull, mine);
-                if (cur == ~0ull) break;   // claimed: this topic leads
-            }
-            if ((uint32_t) (cur >> 32) == (uint32_t) (h >> 32)) {
-                const uint32_t j = (uint32_t) cur;
-                int tj = q.topic_tenant[j];
-                if (tj < 0 || tj >= q.n_tenants) tj = -1;
-                const int64_t oj = q.topic_off[j];
-                if (tj == tn && q.topic_off[j + 1] - oj == full_len && full_len <= 0x3FFFFFFF && same_topic(q.topics, o, k, oj, hlen)) {
-                    lead = j;
-                    break;
-                }
-            }
-            slot = (slot + 1) & q.hash_mask;
+        for (int x = 0; x < 4; x++) {
+            k[4 * j + x] = w[x];
+            h1 = (h1 ^ w[x]) * 0xCC9E2D51u;
+            h2 = (h2 + w[x]) * 0x1B873593u ^ (h2 >> 15);
         }
     }
-    q.leader[i] = lead;
-    if (lead != (uint32_t) i) return;
-    // ---- order key of a leader: one digit per level among the first three, each the hash of the PREFIX that ends with the
-    // level (so equal leading levels give equal digits). One pass over the window words with a running hash; a digit is taken
-    // at each of the first three '/' (or at the end of the window for the last, unterminated level).
+    if (!q.dedup) return 0;
+    for (int j = ORDER_WINDOW_QUADS; 16 * j < hlen; j++) {
+        uint32_t w[4];
+        tq.next(w);
+#pragma unroll
+        for (int x = 0; x < 4; x++) {
+            h1 = (h1 ^ w[x]) * 0xCC9E2D51u;
+            h2 = (h2 + w[x]) * 0x1B873593u ^ (h2 >> 15);
+        }
+    }
+    return fmix64(((uint64_t) h1 << 32) | h2) & q.dedup_hash_mask;
+}
+
+// key = tenant index (T bits) | hash(level 0) | hash(levels 0..1) | hash(levels 0..2): equal leading levels => equal digits =>
+// one bucket. Hash collisions only merge groups. Topics with fewer levels use digit 0. One digit per level among the first
+// three, each the hash of the PREFIX that ends with the level; one pass over the window words with a running hash, a digit
+// taken at each of the first three '/' (or at the end of the window for the last, unterminated level). Returns the bucket:
+// the key's leading hist_bits bits.
+__device__ __forceinline__ uint32_t order_bucket(const uint32_t (&k)[ORDER_WINDOW_WORDS], int hlen, int tn, int tenant_bits, int key_bits,
+                                                 int hist_bits) {
     const int len = min(hlen, 4 * ORDER_WINDOW_WORDS);
     const int rest = key_bits - tenant_bits;
     const int b0 = rest / 3 + (rest % 3 > 0), b1 = rest / 3 + (rest % 3 > 1), b2 = rest / 3;
@@ -841,7 +803,36 @@ __global__ void __launch_bounds__(256, 4) order_prep_kernel(const OrderKernelPar
     key = (key << b0) | (b0 ? dig[0] >> (32 - b0) : 0u);
     key = (key << b1) | (b1 && closed >= 1 ? dig[1] >> (32 - b1) : 0u);
     key = (key << b2) | (b2 && closed >= 2 ? dig[2] >> (32 - b2) : 0u);
-    const uint32_t bucket = key_bits > q.hist_bits ? key >> (key_bits - q.hist_bits) : key;
+    return key_bits > hist_bits ? key >> (key_bits - hist_bits) : key;
+}
+
+// One thread per topic. The order key's bucket is computed first, so nothing of the topic's window is live across the de-dup
+// probe: the kernel fits 48 registers, 5 CTAs per SM instead of 4, and the probe (a chain of dependent L2 round trips, with a
+// byte compare against the leader at every tag match) is hidden by more resident warps. An empty slot is claimed with
+// atomicCAS and no load before it: the CAS returns what it found, one L2 round trip per step. Slots never change once
+// claimed, so the first inserter of a (tenant, topic) pair leads and every later one finds it. A leader counts itself into
+// the bucket histogram.
+__global__ void __launch_bounds__(256, 5) order_prep_kernel(const OrderKernelParams q, int tenant_bits, int key_bits) {
+    const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= q.n_topics) return;
+    uint32_t k[ORDER_WINDOW_WORDS];
+    int hlen, tn;
+    const uint64_t h = read_topic(q, i, hlen, tn, k);
+    const uint32_t bucket = order_bucket(k, hlen, tn, tenant_bits, key_bits, q.hist_bits);
+    uint32_t lead = (uint32_t) i;
+    if (q.dedup) {
+        const unsigned long long mine = ((unsigned long long) (uint32_t) (h >> 32) << 32) | (unsigned long long) (uint32_t) i;
+        for (uint32_t slot = (uint32_t) h & q.hash_mask;; slot = (slot + 1) & q.hash_mask) {
+            const unsigned long long cur = atomicCAS(&q.hash_tab[slot], ~0ull, mine);
+            if (cur == ~0ull) break;   // claimed: this topic leads
+            if ((uint32_t) (cur >> 32) == (uint32_t) (h >> 32) && same_pair(q, (uint32_t) i, (uint32_t) cur)) {
+                lead = (uint32_t) cur;
+                break;
+            }
+        }
+    }
+    q.leader[i] = lead;
+    if (lead != (uint32_t) i) return;
     q.keys[i] = bucket;
     atomicAdd(&q.hist[bucket], 1u);
 }
