@@ -25,7 +25,7 @@ using namespace bfq;
 
 struct bfq_result {
     bfq_index* owner = nullptr;
-    std::shared_ptr<Pool> pool;
+    std::shared_ptr<Pool<Workspace>> pool;
     std::shared_ptr<Snapshot> snap;      // the snapshot the match ran on (ranks resolve against it)
     Workspace* ws = nullptr;             // leased: the arrays below live in its pinned buffers
     int64_t n_topics = 0, n_ranges = 0, n_throttled = 0;
@@ -37,46 +37,16 @@ struct bfq_result {
 
 namespace {
 
-constexpr size_t POOL_KEEP = 4;   // idle workspaces kept for reuse; more are freed when they come back
-
 int32_t acquire(bfq_index* h, std::shared_ptr<Snapshot>* snap, Workspace** ws, const char* who) {
-    Workspace* w = nullptr;
     {
         std::lock_guard<std::mutex> g(h->mu);
         if (!h->snap) return fail(BFQ_E_STATE, std::string(who) + " before the first bfq_index_commit");
         *snap = h->snap;
     }
-    {
-        std::lock_guard<std::mutex> g(h->pool->mu);
-        if (!h->pool->idle.empty()) {
-            w = h->pool->idle.back();
-            h->pool->idle.pop_back();
-        }
-    }
-    if (!w) {
-        w = new Workspace();
-        cudaError_t e = w->init(h->device);
-        if (e != cudaSuccess) {
-            delete w;
-            return fail(BFQ_E_CUDA, std::string("workspace: ") + cudaGetErrorString(e));
-        }
-    }
-    w->dl_n_packs = -1;   // a new lease starts without a delivery nesting: one left by the previous lease is not this result's
-    *ws = w;
+    const int32_t rc = h->pool->acquire(ws);
+    if (rc != BFQ_OK) return rc;
+    (*ws)->dl_n_packs = -1;   // a new lease starts without a delivery nesting: one left by the previous lease is not this result's
     return BFQ_OK;
-}
-
-void give_back(const std::shared_ptr<Pool>& pool, Workspace* w) {
-    if (!w) return;
-    {
-        std::lock_guard<std::mutex> g(pool->mu);
-        if (!pool->closed && pool->idle.size() < POOL_KEEP) {
-            pool->idle.push_back(w);
-            return;
-        }
-    }
-    cudaSetDevice(pool->device);
-    delete w;
 }
 
 
@@ -355,7 +325,10 @@ int32_t finish_core(const CoreCtx& c, const SubBatch& sb, CoreOut* out, bool* re
         warps = std::min<uint64_t>(warps, (uint64_t) device_sm_count() * 8);
         warps = (warps + 7) / 8 * 8;
         if (w->d_scratch.cap < (size_t) (warps * per_warp)) {
-            BFQ_CUDA_TRY(cudaDeviceSynchronize());   // the other compute stream of this workspace may be in tier 2 on the old scratch
+            // the old scratch is freed: tier 2 may still run on it on the workspace's other work stream, or on the device
+            // path, on the caller's stream the match runs on
+            BFQ_CUDA_TRY(w->drain());
+            if (done) BFQ_CUDA_TRY(cudaStreamSynchronize(stream));
             BFQ_CUDA_TRY(w->d_scratch.reserve((size_t) (warps * per_warp)));
         }
         p.scratch = w->d_scratch.p;
@@ -422,7 +395,7 @@ void count_retry(bfq_index* h) {
     h->buffer_retries++;
 }
 
-// grows the buffers a retry asked for (the caller has synchronised the device)
+// grows the buffers a retry asked for (the caller has waited for every stream that writes them)
 int32_t grow_for_retry(Workspace* w, const CoreOut& co, int64_t n, int C) {
     if (co.want_dyn) {
         const size_t want = (size_t) ((uint64_t) n * INLINE_RANGES + (co.want_dyn + co.want_dyn / 4 + 1024) * (uint64_t) C);
@@ -475,7 +448,8 @@ int32_t device_wait(DeviceLease* L) {
         if (rc == BFQ_OK) break;
         if (rc != BFQ_RETRY_GROW) return L->rc = rc;
         count_retry(L->h);
-        if (cudaDeviceSynchronize() != cudaSuccess) return L->rc = fail(BFQ_E_CUDA, "cudaDeviceSynchronize");
+        // the buffers that grow are written by the match alone, on the caller's stream
+        if (cudaStreamSynchronize(L->ctx.stream) != cudaSuccess) return L->rc = fail(BFQ_E_CUDA, "cudaStreamSynchronize");
         rc = grow_for_retry(L->ws, L->co, L->n, 1);
         if (rc == BFQ_OK) rc = device_enqueue(L);
         if (rc != BFQ_OK) return L->rc = rc;
@@ -1409,15 +1383,10 @@ int32_t bfq_match(bfq_index* h, const uint8_t* tenants, const int64_t* tenant_of
     if (n_tenants > 0 && (!tenants || !tenant_off)) return fail(BFQ_E_INVALID, "NULL tenant list");
     BFQ_CUDA_TRY(cudaSetDevice(h->device));
     std::shared_ptr<Snapshot> snap;
-    Workspace* w = nullptr;
-    int32_t rc = acquire(h, &snap, &w, "bfq_match");
+    CallLease<Workspace> lease(*h->pool);   // the workspace goes back to the pool on every error path; on success the result keeps it
+    int32_t rc = acquire(h, &snap, &lease.w, "bfq_match");
     if (rc != BFQ_OK) return rc;
-    // the workspace goes back to the pool on every error path; on success the result keeps it
-    struct Lease {
-        bfq_index* h;
-        Workspace* w;
-        ~Lease() { if (w) { cudaSetDevice(h->device); cudaDeviceSynchronize(); give_back(h->pool, w); } }
-    } lease{h, w};
+    Workspace* w = lease.w;
     // topic_tenant[i] is range-checked on the device (an index outside [0, n_tenants) yields an empty result)
     auto t0 = std::chrono::steady_clock::now();
     const size_t nn = (size_t) std::max<int64_t>(n, 1);
@@ -1545,7 +1514,7 @@ int32_t bfq_match(bfq_index* h, const uint8_t* tenants, const int64_t* tenant_of
             const int64_t total_c = (int64_t) hc[CTR_ROUTES], thr_c = co.chunk_throttled[c];
             // host result buffers grow by reallocation: wait for the copies in flight before moving them
             if ((size_t) (rbase + total_c) > w->h_ranges.cap || (size_t) (tbase + thr_c) > w->h_throttled.cap) {
-                BFQ_CUDA_TRY(cudaDeviceSynchronize());
+                BFQ_CUDA_TRY(w->drain());
                 if ((size_t) (rbase + total_c) > w->h_ranges.cap) {
                     PinnedBuf<uint2> nb;
                     BFQ_CUDA_TRY(nb.reserve((size_t) ((rbase + total_c) * (C - c > 1 ? 2 : 1) + (1 << 16))));
@@ -1575,7 +1544,7 @@ int32_t bfq_match(bfq_index* h, const uint8_t* tenants, const int64_t* tenant_of
         if (!retry) break;
         // a slice of the range / throttled buffers was too small: grow them and redo the batch un-chunked
         count_retry(h);
-        BFQ_CUDA_TRY(cudaDeviceSynchronize());
+        BFQ_CUDA_TRY(w->drain());
         rc = grow_for_retry(w, co, n, C);
         if (rc != BFQ_OK) return rc;
         C = 1;
@@ -1595,8 +1564,7 @@ int32_t bfq_match(bfq_index* h, const uint8_t* tenants, const int64_t* tenant_of
     r->owner = h;
     r->pool = h->pool;
     r->snap = std::move(snap);
-    r->ws = w;
-    lease.w = nullptr;   // the result holds the workspace from here on
+    r->ws = lease.take();   // the result holds the workspace from here on
     r->n_topics = n;
     r->n_ranges = co.n_ranges;
     r->n_throttled = co.n_throttled;
@@ -1694,7 +1662,7 @@ int32_t bfq_result_timings(const bfq_result* r, double* ms, int32_t n) {
 }
 void bfq_result_free(bfq_result* r) {
     if (!r) return;
-    give_back(r->pool, r->ws);
+    r->pool->give_back(r->ws);
     delete r;
 }
 
@@ -1720,7 +1688,7 @@ int32_t bfq_match_device_async(bfq_index* h, const uint8_t* tenants, const int64
     if (rc == BFQ_OK) rc = device_enqueue(L);
     if (rc != BFQ_OK) {
         cudaStreamSynchronize(st);
-        give_back(h->pool, L->ws);
+        h->pool->give_back(L->ws);
         delete L;
         return rc;
     }
@@ -1744,8 +1712,8 @@ void bfq_device_result_release(bfq_device_result* out) {
     cudaSetDevice(L->pool->device);
     // never hand a busy workspace back: the match, and every call that used the result since, on each of its streams
     cudaEventSynchronize(L->ws->ev_done);
-    for (size_t i = 0; i < L->used_on.size(); i++) cudaEventSynchronize(L->ws->ev_use[i]);
-    give_back(L->pool, L->ws);
+    L->uses.wait(L->ws->use_events);
+    L->pool->give_back(L->ws);
     delete L;
     out->lease = nullptr;
 }

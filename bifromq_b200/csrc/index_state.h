@@ -1,5 +1,5 @@
 // index_state.h — the state behind a forward index handle, shared by capi.cu (index, commits, match) and result_calls.cu (the
-// calls on a completed device result): snapshots, workspaces and their pool, the handle, and a device match in flight.
+// calls on a completed device result): snapshots, workspaces, the handle, and a device match in flight.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -13,6 +13,7 @@
 #include "cuda_buf.h"
 #include "fanout.h"
 #include "index_builder.h"
+#include "lease.h"
 #include "match_kernels.cuh"
 
 namespace bfq {
@@ -89,8 +90,8 @@ struct Snapshot {
 constexpr int MAX_CHUNKS = 8;
 
 // Everything ONE match in flight needs: streams, device scratch, pinned result buffers. A workspace is leased from the
-// index's pool for the duration of a call AND of the result it produced (the result's arrays live in it), so concurrent
-// matches on one handle never share a buffer. Returned to the pool by bfq_result_free / bfq_device_result_release.
+// index's pool (lease.h) for the duration of a call AND of the result it produced (the result's arrays live in it), so
+// concurrent matches on one handle never share a buffer. Returned to the pool by bfq_result_free / bfq_device_result_release.
 struct Workspace {
     int device = 0;
     cudaStream_t stream = nullptr, copy_stream = nullptr, work_stream[2] = {nullptr, nullptr};
@@ -98,7 +99,7 @@ struct Workspace {
     cudaEvent_t ev_h2d[MAX_CHUNKS] = {};
     cudaEvent_t evk[2] = {nullptr, nullptr};
     cudaEvent_t ev_done = nullptr;   // device path: recorded behind the last thing a match enqueued (what wait() waits for)
-    std::vector<cudaEvent_t> ev_use; // device path: one per stream the result was used on after the match (lease.h), created on demand
+    UseEvents use_events;            // device path: one per stream the result was used on after the match (lease.h)
     // resolved tenant table of the previous call on this workspace (reused when the same list comes again)
     uint64_t tab_generation = ~0ull;
     std::vector<uint8_t> tab_blob;
@@ -159,29 +160,24 @@ struct Workspace {
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev_done, cudaEventDisableTiming);
         return e;
     }
+    // waits for everything enqueued on the workspace's four streams (a device match runs on the caller's stream instead)
+    cudaError_t drain() {
+        cudaError_t e = cudaSuccess;
+        for (cudaStream_t s : {stream, copy_stream, work_stream[0], work_stream[1]}) {
+            const cudaError_t x = cudaStreamSynchronize(s);
+            if (e == cudaSuccess) e = x;
+        }
+        return e;
+    }
     ~Workspace() {
         cudaSetDevice(device);   // the buffers are freed after this body, on this device
         for (auto& e : ev) if (e) cudaEventDestroy(e);
         for (auto& e : evk) if (e) cudaEventDestroy(e);
         for (auto& e : ev_h2d) if (e) cudaEventDestroy(e);
         if (ev_done) cudaEventDestroy(ev_done);
-        for (auto& e : ev_use) cudaEventDestroy(e);
         if (copy_stream) cudaStreamDestroy(copy_stream);
         for (auto& w : work_stream) if (w) cudaStreamDestroy(w);
         if (stream) cudaStreamDestroy(stream);
-    }
-};
-
-// idle workspaces of one index. Shared with every result / lease in flight, so that freeing a result after its index was
-// destroyed (a garbage-collected host language decides the order) still has a valid place to return its workspace to.
-struct Pool {
-    std::mutex mu;
-    std::vector<Workspace*> idle;
-    int device = 0;
-    bool closed = false;
-    ~Pool() {
-        cudaSetDevice(device);
-        for (Workspace* w : idle) delete w;
     }
 };
 
@@ -205,7 +201,7 @@ struct CoreCtx {
 // A device-side match in flight (bfq_match_device_async .. bfq_device_result_wait .. bfq_device_result_release)
 struct DeviceLease {
     bfq_index* h = nullptr;
-    std::shared_ptr<Pool> pool;
+    std::shared_ptr<Pool<Workspace>> pool;
     std::shared_ptr<Snapshot> snap;
     Workspace* ws = nullptr;
     CoreCtx ctx{};
@@ -214,10 +210,7 @@ struct DeviceLease {
     int32_t rc = BFQ_OK;
     CoreOut co;
     double tier0_ms = 0;
-    // streams the result was used on after the match; stream i's last use is recorded on ws->ev_use[i] (lease.h). One event
-    // per stream: re-recording covers that stream's earlier uses, but not another stream's.
-    std::mutex use_mu;
-    std::vector<cudaStream_t> used_on;
+    StreamUses uses;   // the streams the result was used on after the match (lease.h)
 };
 
 }  // namespace bfq
@@ -225,12 +218,12 @@ struct DeviceLease {
 // the handle (global: the C-ABI names it)
 struct bfq_index {
     int device = 0;
-    std::mutex mu;         // current snapshot pointer, workspace pool, statistics
+    std::mutex mu;         // current snapshot pointer, statistics
     std::mutex stage_mu;   // staging area: reset / load / apply and the (long) host-side rebuild of commit
     bfq::Staging staging;
     std::shared_ptr<bfq::Snapshot> snap;
     uint64_t next_generation = 1;
-    std::shared_ptr<bfq::Pool> pool = std::make_shared<bfq::Pool>();   // idle workspaces
+    std::shared_ptr<bfq::Pool<bfq::Workspace>> pool = std::make_shared<bfq::Pool<bfq::Workspace>>();
     std::shared_ptr<bfq::DelivererTable> deliverers = std::make_shared<bfq::DelivererTable>();   // (subBrokerId, delivererKey) -> id, append-only
     int64_t order_min = 32768;           // batches smaller than this are matched in arrival order (BFQ_ORDER=0: never order)
     bool dedup = true;                   // BFQ_DEDUP=0: match duplicates of a (tenant, topic) pair separately
@@ -248,13 +241,6 @@ struct bfq_index {
 
     ~bfq_index() {
         if (janitor.joinable()) janitor.join();
-        cudaSetDevice(device);
-        std::vector<bfq::Workspace*> idle;
-        {
-            std::lock_guard<std::mutex> g(pool->mu);
-            pool->closed = true;   // workspaces still leased are freed when they come back
-            idle.swap(pool->idle);
-        }
-        for (bfq::Workspace* w : idle) delete w;
+        pool->close();
     }
 };

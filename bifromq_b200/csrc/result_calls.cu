@@ -28,19 +28,7 @@ int32_t bfq::lease_use(const bfq_device_result* res, cudaStream_t stream, const 
     auto* L = static_cast<DeviceLease*>(res->lease);
     if (!L->done || L->rc != BFQ_OK) return fail(BFQ_E_STATE, std::string(who) + " needs a completed match (bfq_device_result_wait)");
     BFQ_CUDA_TRY(cudaSetDevice(L->h->device));
-    std::lock_guard<std::mutex> g(L->use_mu);
-    size_t i = 0;
-    while (i < L->used_on.size() && L->used_on[i] != stream) i++;
-    if (i == L->used_on.size()) {
-        Workspace* w = L->ws;
-        if (w->ev_use.size() == i) {
-            cudaEvent_t e = nullptr;
-            BFQ_CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-            w->ev_use.push_back(e);
-        }
-        L->used_on.push_back(stream);
-    }
-    *ev = L->ws->ev_use[i];
+    BFQ_CUDA_TRY(L->uses.event_for(L->ws->use_events, stream, ev));
     return BFQ_OK;
 }
 

@@ -560,7 +560,7 @@ struct RWorkspace {
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};   // [0,1] around all kernels of a match, [2,3] around rmatch_kernel
     cudaEvent_t ev_in = nullptr;        // device path: recorded on the caller's stream, where the batch was written
-    std::vector<cudaEvent_t> ev_use;    // device result: one per stream a key gather ran on (RLease::used_on), created on demand
+    UseEvents use_events;               // device result: one per stream a key gather ran on (RLease::uses)
     std::atomic<int64_t> bytes_held{0}; // device_bytes() when the last call on it ended (bfq_rindex_stats)
     DeviceBuf<uint8_t> d_in, d_scan_tmp, d_key_tmp;   // d_in: the host path's batch, one block
     PinnedBuf<int32_t> h_tenant_root;
@@ -582,6 +582,13 @@ struct RWorkspace {
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev_in, cudaEventDisableTiming);
         return e;
     }
+    // before the workspace goes back to the pool: waits for its stream and notes the bytes it holds, which bfq_rindex_stats
+    // reads while another call may be growing its buffers
+    cudaError_t drain() {
+        const cudaError_t e = cudaStreamSynchronize(stream);
+        bytes_held = device_bytes();
+        return e;
+    }
     int64_t device_bytes() const {
         return (int64_t) (d_in.bytes() + d_scan_tmp.bytes() + d_key_tmp.bytes() + d_ids.bytes() + d_key_len.bytes() +
                           d_tenant_root.bytes() + d_span_begin.bytes() + d_span_count.bytes() + d_overflow.bytes() +
@@ -593,33 +600,18 @@ struct RWorkspace {
         cudaSetDevice(device);   // the buffers are freed after this body, on this device
         for (auto& e : ev) if (e) cudaEventDestroy(e);
         if (ev_in) cudaEventDestroy(ev_in);
-        for (auto& e : ev_use) cudaEventDestroy(e);
         if (stream) cudaStreamDestroy(stream);
-    }
-};
-
-// the workspaces of one handle. Shared with every device result in flight, so that releasing a result after its handle was
-// destroyed still has a place to return its workspace to.
-struct RPool {
-    std::mutex mu;
-    std::vector<RWorkspace*> idle;
-    std::vector<RWorkspace*> held;   // every workspace alive: idle and leased
-    int device = 0;
-    bool closed = false;
-    ~RPool() {
-        cudaSetDevice(device);
-        for (RWorkspace* w : idle) delete w;
     }
 };
 
 // a device result (bfq_rmatch_device .. bfq_rdevice_result_release)
 struct RLease {
     bfq_rindex* h = nullptr;
-    std::shared_ptr<RPool> pool;
+    std::shared_ptr<Pool<RWorkspace>> pool;
     RWorkspace* ws = nullptr;
     std::shared_ptr<IdTable> by_id;   // the id table of the snapshot the match ran on
     std::mutex use_mu;                // key gathers on this result, one at a time (they share the workspace's scratch)
-    std::vector<cudaStream_t> used_on;              // ws->ev_use[i]: the last gather on used_on[i]
+    StreamUses uses;                  // the streams the gathers ran on (lease.h)
     std::vector<std::shared_ptr<KeyBufs>> keys;     // key buffers the gathers read, held until release
 };
 
@@ -637,7 +629,7 @@ struct bfq_rindex {
     std::shared_mutex mu;
     std::mutex gate;   // a writer holds it while it waits for and holds mu: matches arriving meanwhile queue behind it
     cudaStream_t stream = nullptr;   // commits
-    std::shared_ptr<RPool> pool = std::make_shared<RPool>();
+    std::shared_ptr<Pool<RWorkspace>> pool = std::make_shared<Pool<RWorkspace>>();
     // staging: (tenant, topic) -> id ; id -> (tenant, topic)
     std::map<std::pair<std::string, std::string>, int64_t> staged;
     std::shared_ptr<IdTable> by_id = std::make_shared<IdTable>();   // staging: add / load_keys append here
@@ -673,14 +665,7 @@ struct bfq_rindex {
 
     ~bfq_rindex() {
         cudaSetDevice(device);   // the buffers are freed after this body, on this device
-        std::vector<RWorkspace*> idle;
-        {
-            std::lock_guard<std::mutex> g(pool->mu);
-            pool->closed = true;   // workspaces still leased are freed when they come back
-            idle.swap(pool->idle);
-            pool->held.clear();
-        }
-        for (RWorkspace* w : idle) delete w;
+        pool->close();
         if (stream) cudaStreamDestroy(stream);
     }
 };
@@ -1066,59 +1051,6 @@ int32_t commit_delta(bfq_rindex* h) {
     return BFQ_OK;
 }
 
-// ------------------------------------------------------------------------------------------------ workspaces
-constexpr size_t POOL_KEEP = 4;   // idle workspaces kept for reuse; more are freed when they come back
-
-int32_t acquire(bfq_rindex* h, RWorkspace** out) {
-    RPool& pool = *h->pool;
-    {
-        std::lock_guard<std::mutex> g(pool.mu);
-        if (!pool.idle.empty()) {
-            *out = pool.idle.back();
-            pool.idle.pop_back();
-            return BFQ_OK;
-        }
-    }
-    auto* w = new RWorkspace();
-    const cudaError_t e = w->init(h->device);
-    if (e != cudaSuccess) {
-        delete w;
-        return fail(BFQ_E_CUDA, std::string("workspace: ") + cudaGetErrorString(e));
-    }
-    std::lock_guard<std::mutex> g(pool.mu);
-    pool.held.push_back(w);
-    *out = w;
-    return BFQ_OK;
-}
-
-// the caller has waited for everything enqueued on w
-void give_back(const std::shared_ptr<RPool>& pool, RWorkspace* w) {
-    if (!w) return;
-    w->bytes_held = w->device_bytes();
-    {
-        std::lock_guard<std::mutex> g(pool->mu);
-        if (!pool->closed && pool->idle.size() < POOL_KEEP) {
-            pool->idle.push_back(w);
-            return;
-        }
-        pool->held.erase(std::remove(pool->held.begin(), pool->held.end(), w), pool->held.end());
-    }
-    cudaSetDevice(pool->device);
-    delete w;
-}
-
-// a workspace for the length of one call: back to the pool on every return, after its stream has drained
-struct CallLease {
-    std::shared_ptr<RPool> pool;
-    RWorkspace* w = nullptr;
-    ~CallLease() {
-        if (w) {
-            cudaStreamSynchronize(w->stream);
-            give_back(pool, w);
-        }
-    }
-};
-
 // ------------------------------------------------------------------------------------------------ retain keys on the device
 // Brings the device key table of t up to every id t holds and returns its buffers. The caller holds the handle lock (the ids
 // are read here); uploads run on st and are finished on return.
@@ -1479,8 +1411,8 @@ int32_t bfq_rindex_stats(bfq_rindex* h, int64_t* stats, int32_t n) {
     int64_t n_ws = 0, ws_bytes = 0;
     {
         std::lock_guard<std::mutex> p(h->pool->mu);
-        n_ws = (int64_t) h->pool->held.size();
-        for (const RWorkspace* w : h->pool->held) ws_bytes += w->bytes_held;
+        n_ws = (int64_t) h->pool->live.size();
+        for (const RWorkspace* w : h->pool->live) ws_bytes += w->bytes_held;
     }
     const int64_t key_bytes = h->by_id->key_device_bytes;
     const int64_t v[14] = {h->n_topics, (int64_t) h->regions.size(), h->n_nodes, h->garbage_nodes, h->used_slots,
@@ -1509,8 +1441,8 @@ int32_t bfq_rmatch(bfq_rindex* h, const uint8_t* tenants, const int64_t* tenant_
     if (!h || !out || n < 0 || n_tenants < 0) return fail(BFQ_E_INVALID, "bad argument");
     BFQ_CUDA_TRY(cudaSetDevice(h->device));
     auto g = read_lock(h);   // declared first: released after the lease below has drained its stream
-    CallLease lease{h->pool};
-    int32_t rc = acquire(h, &lease.w);
+    CallLease<RWorkspace> lease(*h->pool);
+    int32_t rc = h->pool->acquire(&lease.w);
     if (rc != BFQ_OK) return rc;
     RWorkspace* w = lease.w;
     if (!h->have_snapshot) return fail(BFQ_E_STATE, "bfq_rmatch before the first bfq_rindex_commit");
@@ -1600,8 +1532,8 @@ int32_t bfq_rmatch_device(bfq_rindex* h, const uint8_t* tenants, const int64_t* 
     memset(out, 0, sizeof(*out));
     BFQ_CUDA_TRY(cudaSetDevice(h->device));
     auto g = read_lock(h);   // declared first: released after the lease below has drained its stream
-    CallLease lease{h->pool};
-    int32_t rc = acquire(h, &lease.w);
+    CallLease<RWorkspace> lease(*h->pool);
+    int32_t rc = h->pool->acquire(&lease.w);
     if (rc != BFQ_OK) return rc;
     RWorkspace* w = lease.w;
     if (!h->have_snapshot) return fail(BFQ_E_STATE, "bfq_rmatch_device before the first bfq_rindex_commit");
@@ -1632,8 +1564,7 @@ int32_t bfq_rmatch_device(bfq_rindex* h, const uint8_t* tenants, const int64_t* 
         out->device_ms = a;
         out->kernel_ms = b;
     }
-    L->ws = w;
-    lease.w = nullptr;   // the result keeps the workspace until bfq_rdevice_result_release
+    L->ws = lease.take();   // the result keeps the workspace until bfq_rdevice_result_release
     out->lease = L;
     return BFQ_OK;
 }
@@ -1643,8 +1574,9 @@ void bfq_rdevice_result_release(bfq_rdevice_result* res) {
     auto* L = static_cast<RLease*>(res->lease);
     cudaSetDevice(L->pool->device);
     // never hand a busy workspace back: every key gather on the result, on each stream it ran on
-    for (size_t i = 0; i < L->used_on.size(); i++) cudaEventSynchronize(L->ws->ev_use[i]);
-    give_back(L->pool, L->ws);
+    L->uses.wait(L->ws->use_events);
+    L->ws->drain();
+    L->pool->give_back(L->ws);
     delete L;
     res->lease = nullptr;
 }
@@ -1668,17 +1600,9 @@ int32_t bfq_rretain_keys_device(bfq_rindex* h, const bfq_rdevice_result* res, in
     }
     if (std::find(L->keys.begin(), L->keys.end(), kb) == L->keys.end()) L->keys.push_back(kb);
     cudaStream_t st = (cudaStream_t) stream;
-    size_t k = 0;
-    while (k < L->used_on.size() && L->used_on[k] != st) k++;
-    if (k == L->used_on.size()) {
-        if (k == w->ev_use.size()) {
-            cudaEvent_t e = nullptr;
-            BFQ_CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-            w->ev_use.push_back(e);
-        }
-        L->used_on.push_back(st);
-    }
-    RecordOnExit rec(w->ev_use[k], st);
+    cudaEvent_t ev = nullptr;
+    BFQ_CUDA_TRY(L->uses.event_for(w->use_events, st, &ev));
+    RecordOnExit rec(ev, st);
     // sizing pass, scan, then the bytes if they fit
     BFQ_CUDA_TRY(cudaMemsetAsync(d_key_off, 0, 8, st));
     if (n > 0) {

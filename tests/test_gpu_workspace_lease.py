@@ -29,12 +29,13 @@ import test_gpu_delivery as FD
 import test_gpu_edges as E
 import test_gpu_fanout as F
 import test_gpu_fanout_budget as FB
+import test_gpu_inverse_edges as IE
 
 INT_MAX, I64_MAX = 2 ** 31 - 1, 2 ** 63 - 1
 E_STATE = -4
 
-# ------------------------------------------------------------------ restated thresholds (capi.cu, match_kernels.cu)
-POOL_KEEP = 4                # idle workspaces a handle keeps (capi.cu: POOL_KEEP)
+# ------------------------------------------------------------------ restated thresholds (lease.h, capi.cu, match_kernels.cu)
+POOL_KEEP = 4                # idle workspaces a handle keeps (lease.h: POOL_KEEP)
 ORDER_MIN = 32768            # default order_min_topics
 PIPELINE_TOPICS, SUB_BATCHES = 1 << 17, 4
 
@@ -406,6 +407,49 @@ def test_release_waits_on_every_stream_the_result_was_used_on(B):
     assert S1.query(), "release left the fan-out running on the stream the result was used on first"
     assert ev2.query()
     idx.close()
+
+
+@pytest.mark.gpu
+def test_host_matches_do_not_wait_for_unrelated_work(B):
+    """a match waits for its own workspace's streams only: a host match on a fresh handle, whose pinned range buffer must
+    grow, and a host inverse match both return while a sleep of seconds on an unrelated stream is still running"""
+    from bifromq_b200 import _native, retain
+    torch = B.torch
+    R = type("R", (), {"N": _native, "retain": retain})
+    pairs, tenants, topics, tt = F.groups_case()
+    ritopics, filters = IE.dollar_case()
+    # every kernel both matches launch is loaded before the sleep is queued (loading a kernel may synchronise the device)
+    warm = F.make_index(B, pairs)
+    warm.match_topics(tenants, topics, tt).close()
+    warm.close()
+    rwarm, _ = IE.make_index(R, ritopics)
+    IE.run(R, rwarm, filters)
+    rwarm.close()
+    idx = F.make_index(B, pairs)
+    ridx, entries = IE.make_index(R, ritopics)
+    S = torch.cuda.Stream(B.dev)
+    with torch.cuda.stream(S):
+        torch.cuda._sleep(1000)
+    S.synchronize()
+    ev = torch.cuda.Event()
+    with torch.cuda.stream(S):
+        torch.cuda._sleep(SLEEP_CYCLES * 250)   # about 5 s
+        ev.record(S)
+    res = idx.match_topics(tenants, topics, tt)
+    forward_waited = ev.query()
+    rres = IE.run(R, ridx, filters)
+    inverse_waited = ev.query()
+    S.synchronize()
+    assert not forward_waited, "a host match waited for a sleep on an unrelated stream"
+    assert not inverse_waited, "a host inverse match waited for a sleep on an unrelated stream"
+    want = F.oracle(pairs, tenants, topics, tt)
+    offsets, ranks = res.expand()
+    assert len(ranks) > 0
+    assert offsets.tolist() == want.offsets.tolist() and ranks.tolist() == want.ranks.tolist()
+    IE.check(rres, IE.Expect(entries), filters)
+    res.close()
+    idx.close()
+    ridx.close()
 
 
 def gather_world1(B):
